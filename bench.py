@@ -4,7 +4,7 @@ encoder/decoder fwd+bwd -> token CE -> (DDP all-reduce) -> clip + AdamW step.
     python bench.py --gpus 1 --steps 5 --warmup 3                     # our arm (one process per GPU; torchrun for N > 1)
     python bench.py --impl reference --gpus 1 --steps 2 --warmup 1    # the reference's CPU path (oracle port) on host cores
 
-One JSON line on stdout (rank 0).  See the bench contract in DESIGN.md.
+One JSON line on stdout (rank 0).
 """
 from __future__ import annotations
 
@@ -33,7 +33,8 @@ def _peaks():
             p = json.load(f)
         return {"bf16_tflops": p["bf16_tflops"], "bf16_tflops_sustained": p["bf16_tflops_sustained"], "hbm_gbs": p["hbm_gbs"],
                 "source": "MEASURED_PEAKS.json"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W board power): dense BF16 and HBM3 bandwidth.  Data-sheet rates, not measured ones.
+    return {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet"}
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -94,8 +95,7 @@ def run_cpu_reference(variant: str, clips: int, steps: int, warmup: int, layers=
 
 def bounded_cpu_sample(variant: str, steps: int = 2, warmup: int = 1):
     """A bounded sample of the workload on the host cores: REAL full-depth optimizer steps of the reference's CPU path
-    on ONE clip (the GPU arm's step is 32 clips; ~4 s per clip-step at medium on the B200 box's host), nothing
-    extrapolated.  Returns (clips/s, threads, description, seconds per step, steps run)."""
+    on ONE clip (the GPU arm's step is --batch-per-gpu clips), nothing extrapolated.  Returns (clips/s, threads, description, seconds per step, steps run)."""
     value, sec, threads = run_cpu_reference(variant, 1, steps, warmup)
     return value, threads, (f"{steps} full-depth optimizer steps of 1 clip each after {warmup} warm-up step(s): {variant}, fp32, torch CPU, "
                             f"{threads} threads, log-mel + fwd + CE + bwd + clip + AdamW ({sec:.2f} s per step)"), sec, steps
@@ -126,7 +126,7 @@ def reference_arm(args):
 
 # ------------------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clock / throttle-reason samples during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clock / throttle-reason samples during the timed region (read-only queries)."""
 
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -235,6 +235,24 @@ def torch_gpu_arm(args):
         dist.destroy_process_group()
 
 
+DUMP_SAMPLE = 1 << 21   # elements per sampled slab: 2 x 8 MB of float32
+
+
+def dump_outputs(out_dir: str, loss: float, slabs) -> None:
+    """What a caller of the training step holds after the last timed step: its loss, the updated fp32 master weights and
+    the gradients it applied.  The slabs hold ~10^9 elements, so both are sampled at the same fixed, seeded positions
+    (identical from run to run and build to build for the same --variant)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    gen = torch.Generator().manual_seed(20240607)
+    n = slabs.P.numel()
+    idx = torch.randint(0, n, (min(DUMP_SAMPLE, n),), generator=gen).sort().values.to(slabs.P.device)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([loss], dtype=np.float64))
+    np.save(os.path.join(out_dir, "weights_sample.npy"), slabs.P[idx].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "grads_sample.npy"), slabs.G[idx].float().cpu().numpy())
+
+
 def our_arm(args):
     import torch.distributed as dist
 
@@ -322,6 +340,8 @@ def our_arm(args):
     ms, loss = timed(args.steps, e2e=False)
     launches = _lib.LAUNCH_COUNT - launches0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, slabs)
     ms_e2e, loss_e2e = timed(args.steps, e2e=True)
     # roofline pass: the same K steps with every GEMM launch bracketed by CUDA events.  The weight-gradient side stream
     # is switched off for this pass so that launches do not overlap and a launch's event time is its own duration.
@@ -366,13 +386,13 @@ def our_arm(args):
                    "grad_sync": ("none" if world == 1 else ("olmoasr_b200.ddp.SlabGradSync (flat fp32 gradient slab, segment all-reduces)"
                                                             if ddp_impl == "slab" else "torch DistributedDataParallel")),
                    "state_layout": "parameter / gradient / moment / bf16-shadow slabs (olmoasr_b200/slab.py); AdamW refreshes the bf16 weights",
-                   "l2": "no flush needed: per-step working set (~60 GB of activations at medium/32) is >> the 126 MB L2",
+                   "l2": "no flush needed: the per-step working set (tens of GB of activations) is >> the 50 MB L2",
                    "loss": loss, "optimizer_steps_applied": applied, "peak_mem_gib": peak_mem},
         "e2e": {"value": e2e_value, "unit": "clips/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 4,
                 "ms_per_step": ms_e2e / args.steps, "loss": loss_e2e},
         "gpu_launches": launches,
         "clocks": clocks,
-        "roofline": {"bound": "tensor", "kernel": "gemm_tcgen05_kernel (all GEMM launches of K steps)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_wgmma_kernel (all GEMM launches of K steps)",
                      "achieved": gemm_tflops, "peak": peaks["bf16_tflops_sustained"], "unit": "TFLOP/s",
                      "frac": gemm_tflops / peaks["bf16_tflops_sustained"], "traffic": None,
                      "peak_source": peaks["source"] + " (sustained: kernel timed inside a long step)",
@@ -510,7 +530,7 @@ def rtf_arm(args):
             "config": {"workload": f"{variant} greedy kv-cache decode (BASELINE.json configs[4]): N concurrent 30 s synthetic clips, "
                                    f"{sample_len} sampled tokens each (random-init weights never emit eot), value = RTF at N = {best['n_clips']}",
                        "sweep": sweep, "launches_per_decode_step": eng.launches_per_step,
-                       "l2": "every step re-reads the decoder weights (278 MB) and N x 55 MB of cross K/V: > 126 MB L2 from N = 1"},
+                       "l2": "every step re-reads the decoder weights (278 MB) and N x 55 MB of cross K/V: > 50 MB L2 from N = 1"},
             "e2e": {"value": best["rtf"], "unit": "s per s of audio", "h2d_bytes_per_step": best["n_clips"] * 480000 * 2,
                     "d2h_bytes_per_step": best["n_clips"] * (len(task.initial_tokens) + sample_len) * 8},
             "gpu_launches": launches, "clocks": clocks,
@@ -532,13 +552,17 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "torch_gpu"])
     ap.add_argument("--variant", default="medium", choices=list(TRAIN_GFLOP_PER_CLIP))
-    ap.add_argument("--batch-per-gpu", type=int, default=32)
+    # 16 clips of the medium model fit the 80 GB of an H100 with room for the stock-PyTorch leg that follows
+    ap.add_argument("--batch-per-gpu", type=int, default=16)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-baseline", action="store_true")
-    ap.add_argument("--metric", default="train", choices=["train", "rtf"], help="train: clips/s (default, the driver's line); "
+    ap.add_argument("--metric", default="train", choices=["train", "rtf"], help="train: clips/s (default); "
                     "rtf: greedy-decode real-time factor sweep (BASELINE.json metric, second half)")
     ap.add_argument("--variant-rtf", default="small")
     ap.add_argument("--dtype", default="fp16", choices=["fp16", "bf16"], help="decode activation dtype for --metric rtf")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="train arm: after the timed steps write what the last timed step computed to DIR/<name>.npy "
+                         "(loss, and fixed seeded samples of the updated fp32 weights and of the gradients)")
     args = ap.parse_args()
     if args.metric == "rtf":
         (rtf_reference_arm if args.impl == "reference" else rtf_arm)(args)

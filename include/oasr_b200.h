@@ -1,5 +1,5 @@
 /*
- * liboasr_b200 -- C ABI of the B200 (sm_100a) kernels behind olmoasr_b200.
+ * liboasr_b200 -- C ABI of the H100 (sm_90a) kernels behind olmoasr_b200.
  *
  * The reference (allenai/OLMoASR) has no FFI layer: its hot path is plain PyTorch library calls
  * made from olmoasr/model.py, olmoasr/inf_model.py and (third-party) whisper/audio.py.  Each entry
@@ -44,7 +44,7 @@ OASR_API int oasr_device_sm_count(void);
  * those SMs free avoids it.  Process-wide; returns the previous value. */
 OASR_API int oasr_gemm_set_sm_budget(int n_sms);
 
-/* ---- dense GEMM on tcgen05 / TMEM ---------------------------------------------------------------
+/* ---- dense GEMM on wgmma -------------------------------------------------------------------------
  * Replaces F.linear in Linear.forward (olmoasr/model.py:97-101), its autograd dgrad / wgrad, the tied
  * logits matmul (model.py:768-770) and the two Conv1d calls (model.py:592-593) after im2col.
  *
@@ -63,7 +63,7 @@ OASR_API int oasr_gemm_set_sm_budget(int n_sms);
 #define OASR_EPI_BF16_RESIDUAL 2 /* C = bf16(aux + bf16(acc + bias))                            */
 #define OASR_EPI_BF16_GELU_BWD 3 /* C = bf16(bf16(acc) * gelu_erf'(aux))   aux = pre-activation  */
 #define OASR_EPI_F32 4           /* C(f32) = acc + bias                                         */
-#define OASR_EPI_F32_ATOMIC_ADD 5 /* C(f32) += acc   (split_k >= 1, C pre-initialised)           */
+#define OASR_EPI_F32_ATOMIC_ADD 5 /* C(f32) += acc   (split_k >= 1, C pre-initialised; one add per element) */
 
 OASR_API int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, int b_layout,
                    void* C, int64_t ldc, void* C2, const float* bias, const void* aux, int64_t ldaux,
@@ -100,13 +100,13 @@ OASR_API int oasr_layernorm_bwd(const void* dy, const void* x, const float* weig
  * causal != 0 applies key <= query; kv_len (B,) int32 (nullable) hides keys >= kv_len[b] -- together they are
  * the reference's `padding_mask + causal mask` (model.py:740-743, train_timestamps.py:314-315).
  * lse: (B,H,Tq) f32, log2 domain: log2(sum_k 2^(s_k * scale * log2 e)).
- * Backward: delta (B,H,Tq) f32 and dq_accum (B*Tq, H*64) f32 are scratch. */
+ * Backward: delta (B,H,Tq) f32 is scratch. */
 OASR_API int oasr_attention_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
                                 void* o, int64_t ldo, float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
                                 int64_t head_dim, int causal, const int32_t* kv_len, float scale, void* stream);
 OASR_API int oasr_attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
                                 const void* o, int64_t ldo, const void* dout, int64_t lddo, const float* lse,
-                                float* delta, float* dq_accum, void* dq, int64_t lddq, void* dk, int64_t lddk,
+                                float* delta, void* dq, int64_t lddq, void* dk, int64_t lddk,
                                 void* dv, int64_t lddv, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
                                 int64_t head_dim, int causal, const int32_t* kv_len, float scale, void* stream);
 

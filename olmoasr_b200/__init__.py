@@ -1,6 +1,6 @@
-"""olmoasr_b200 -- B200-native (sm_100a) implementation of the OLMoASR training / decode hot path behind the
+"""olmoasr_b200 -- H100-native (sm_90a) implementation of the OLMoASR training / decode hot path behind the
 reference's Python surface (olmoasr/__init__.py): `load_model`, `model`, `inf_model`, `log_mel_spectrogram`,
-`pad_or_trim`, `load_audio`.  See DESIGN.md for scope and INTEGRATION.md for how to swap it in."""
+`pad_or_trim`, `load_audio`.  See README.md for scope and INTEGRATION.md for how to swap it in."""
 import io
 import os
 from typing import Optional, Union

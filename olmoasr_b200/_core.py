@@ -36,19 +36,8 @@ def _sm_count() -> int:
 
 
 def _pick_block_n(M: int, N: int) -> int:
-    """Tile width for the persistent GEMM: fewest waves x tile cost; ties go to the wider tile."""
-    if N <= 64:
-        return 64
-    sms = _sm_count()
-    best, best_cost = 256, None
-    # measured on B200 (profiles/r01_gemm_bringup2_cluster.log): the 128-wide tile runs at ~70 % of the 256-wide
-    # tile's rate (64 vs 85 FLOP per operand byte), so it only wins when it saves >= 30 % of the waves
-    for bn, penalty in ((256, 1.0), (128, 1.4)):
-        tiles = math.ceil(M / 128) * math.ceil(N / bn)
-        cost = math.ceil(tiles / sms) * bn * penalty
-        if best_cost is None or cost < best_cost:
-            best, best_cost = bn, cost
-    return best
+    """Tile width for the persistent GEMM: 128 (the widest sm_90a tile, csrc/gemm_sm90.cu) unless N fits a 64-wide tile."""
+    return 64 if N <= 64 else 128
 
 
 def _pick_split_k(tiles: int, kblocks: int) -> int:
@@ -79,8 +68,8 @@ def linear_dgrad(dy: Tensor, w_bf16: Tensor, *, epi=K.EPI_BF16, aux=None, out=No
 
 def linear_wgrad(dy: Tensor, x: Tensor, n_valid: Optional[int] = None, side=None, out: Optional[Tensor] = None):
     """dW (N, K) f32 = dy^T x.  Both operands are read MN-major straight from their (M, *) row-major storage
-    (A = dy^T is "stored (K=M, M=N)", B = x is "stored (K=M, N=K)"); split-K + fp32 red.add when the output has
-    too few tiles to fill the GPU.  With `out` (a gradient-slab view, olmoasr_b200/slab.py) the product is ACCUMULATED
+    (A = dy^T is "stored (K=M, M=N)", B = x is "stored (K=M, N=K)"); split-K (partial products added up in split
+    order) when the output has too few tiles to fill the GPU.  With `out` (a gradient-slab view, olmoasr_b200/slab.py) the product is ACCUMULATED
     into it by the epilogue: no allocation, no zero fill, no hand-over through autograd."""
     M = dy.shape[0]
     N = dy.shape[1] if n_valid is None else n_valid
@@ -640,7 +629,7 @@ class ResidualAttentionBlock(nn.Module):
 # =====================================================================================================
 class _StemFn(torch.autograd.Function):
     """conv1 -> GELU -> conv2 (stride 2) -> GELU -> transpose -> + sinusoids (model.py:592-602) as
-    im2col + tcgen05 GEMM with fused bias/GELU epilogues, time-major throughout."""
+    im2col + wgmma GEMM with fused bias/GELU epilogues, time-major throughout."""
 
     @staticmethod
     def forward(ctx, enc, mel, w1, b1, w2, b2):

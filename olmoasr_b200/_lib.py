@@ -70,7 +70,7 @@ _SIGNATURES = {
     "oasr_attention_fwd": [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
                            c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_void_p, c_float, c_void_p],
     "oasr_attention_bwd": [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64,
-                           c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64,
+                           c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64,
                            c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_void_p, c_float, c_void_p],
     "oasr_ce_fwd": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_i64, c_void_p],
     "oasr_ce_finalize": [c_void_p, c_void_p, c_void_p],
@@ -161,7 +161,9 @@ def stream():
 
 
 # kernels launched per entry point (memsets not counted) -- bench.py reports the total as `gpu_launches`
-_LAUNCHES_PER_CALL = {"oasr_logmel": 3, "oasr_attention_bwd": 3, "oasr_dec_attention": 2, "oasr_dec_sample": 2}
+_LAUNCHES_PER_CALL = {"oasr_logmel": 3, "oasr_attention_bwd": 3, "oasr_dec_attention": 2, "oasr_dec_sample": 2,
+                      "oasr_ce_fwd": 2, "oasr_colsum_bf16": 2, "oasr_layernorm_bwd": 3, "oasr_grad_sqnorm": 2,
+                      "oasr_grad_sqnorm_flat": 2}
 LAUNCH_COUNT = 0
 
 

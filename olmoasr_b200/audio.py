@@ -3,7 +3,7 @@
 scripts/eval/eval.py:157-162, olmoasr/transcribe.py:148).
 
 `log_mel_spectrogram` here takes a waveform or a BATCH of waveforms that is (or is moved) on a CUDA device and
-runs the fused sm_100a kernel (csrc/logmel.cu).  The dynamic-range floor uses each clip's own maximum -- the
+runs the fused sm_90a kernel (csrc/logmel.cu).  The dynamic-range floor uses each clip's own maximum -- the
 per-sample semantics of the reference datasets.  There is no CPU implementation in this package.
 """
 from __future__ import annotations

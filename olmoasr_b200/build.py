@@ -1,4 +1,4 @@
-"""Build liboasr_b200.so in-tree with nvcc for sm_100a (cross-compiles on a GPU-less box).
+"""Build liboasr_b200.so in-tree with nvcc for sm_90a (H100; nvcc cross-compiles without a GPU).
 
     python -m olmoasr_b200.build [--force]
 
@@ -20,7 +20,7 @@ LIB = CSRC / "liboasr_b200.so"
 OBJ_DIR = CSRC / "_obj"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",

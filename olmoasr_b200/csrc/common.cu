@@ -27,7 +27,7 @@ int num_sms() {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       cached = n;
     else
-      cached = 148;
+      cached = 132;
   }
   return cached;
 }
@@ -153,6 +153,70 @@ int make_tmap_3d(CUtensorMap* out, const void* base, int elt_bytes, uint64_t d0,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   OASR_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(3d) failed: CUresult %d", (int)r);
   tmap_store(key, *out);
+  return OASR_OK;
+}
+
+}  // namespace oasr
+
+namespace oasr {
+
+void* scratch_alloc(size_t bytes, cudaStream_t st) {
+  static int pool_dev = -1;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) { set_last_error("scratch: no device"); return nullptr; }
+  if (pool_dev != dev) {   // keep freed scratch in the pool instead of returning it to the driver at every sync
+    cudaMemPool_t pool;
+    if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+      uint64_t keep = UINT64_MAX;
+      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+    }
+    pool_dev = dev;
+  }
+  void* p = nullptr;
+  const cudaError_t e = cudaMallocAsync(&p, bytes < 16 ? 16 : bytes, st);
+  if (e != cudaSuccess) {
+    set_last_error("scratch: cudaMallocAsync(%zu) -> %s", bytes, cudaGetErrorString(e));
+    return nullptr;
+  }
+  return p;
+}
+
+void scratch_free(void* p, cudaStream_t st) {
+  if (p) cudaFreeAsync(p, st);
+}
+
+namespace {
+__global__ void add_partials_cols_kernel(const float* __restrict__ part, int n_parts, int64_t n, float* __restrict__ out) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    float t = 0.f;
+    for (int k = 0; k < n_parts; ++k) t += part[k * n + i];
+    out[i] += t;
+  }
+}
+// one scalar from many partials: 1024 threads take fixed strided subsets, then a fixed tree
+__global__ void __launch_bounds__(1024) add_partials_scalar_kernel(const float* __restrict__ part, int n_parts, float* __restrict__ out) {
+  __shared__ float red[1024];
+  float t = 0.f;
+  for (int k = threadIdx.x; k < n_parts; k += 1024) t += part[k];
+  red[threadIdx.x] = t;
+  __syncthreads();
+  for (int w = 512; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) out[0] += red[0];
+}
+}  // namespace
+
+int add_partials(const float* part, int n_parts, int64_t n, float* out, cudaStream_t st) {
+  if (n == 1) {
+    add_partials_scalar_kernel<<<1, 1024, 0, st>>>(part, n_parts, out);
+  } else {
+    int64_t blocks = ceil_div(n, 256);
+    const int64_t cap = static_cast<int64_t>(num_sms()) * 8;
+    add_partials_cols_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, st>>>(part, n_parts, n, out);
+  }
+  OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
 

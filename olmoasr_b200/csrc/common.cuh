@@ -49,6 +49,17 @@ int make_tmap_3d(CUtensorMap* out, const void* base, int elt_bytes, uint64_t d0,
 
 __host__ __device__ inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// ---- deterministic reductions --------------------------------------------------------------------------
+// Sums that several blocks contribute to are never folded with floating-point atomics (their order, and so the
+// rounding of the result, would change from run to run).  Blocks write partials to stream-ordered scratch and one
+// more launch adds them up in a fixed order.
+// Scratch comes from the device's default memory pool on the caller's stream (cudaMallocAsync / cudaFreeAsync), so
+// concurrent streams never share it; the pool keeps freed memory cached.
+void* scratch_alloc(size_t bytes, cudaStream_t st);   // nullptr (and the error string set) on failure
+void scratch_free(void* p, cudaStream_t st);
+// out[i] += sum_{k < n_parts} part[k * n + i]   for i < n   (k ascending)
+int add_partials(const float* part, int n_parts, int64_t n, float* out, cudaStream_t st);
+
 // ---- small device helpers ---------------------------------------------------------------
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16_rn(x)); }
 
@@ -85,66 +96,50 @@ __device__ __forceinline__ float fast_ex2(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// Two-element GELU / GELU' for GEMM epilogues: same Abramowitz-Stegun erf as erf_fast, but packed FFMA2 / FMUL2
-// arithmetic, MUFU.RCP instead of the IEEE reciprocal and one shared exp(-x^2/2) for cdf and pdf: ~10 instructions
-// per element instead of ~35 (the fc1 GELU epilogue measured 34k cycles per 128 x 256 tile against 8k of MMA).
+// Two-lane float arithmetic, each lane rounded to nearest like the scalar operation (sm_90 has no packed fp32 pipe;
+// keeping the pairs lets the callers below read as the vector maths they are).
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+
+// Two-element GELU / GELU' for GEMM epilogues: same Abramowitz-Stegun erf as erf_fast, but MUFU.RCP instead of the
+// IEEE reciprocal and one shared exp(-x^2/2) for cdf and pdf: ~10 instructions per element instead of ~35.
 struct GeluPair { float2 ea; float2 e; };   // erf(|x|/sqrt2) (>= 0) and exp(-x^2/2)
 __device__ __forceinline__ GeluPair gelu_core2(float2 x) {
-  // 1 / (1 + p |x| / sqrt2): |x| folds into the FFMA2 operand modifier
+  // 1 / (1 + p |x| / sqrt2)
   const float2 ax = make_float2(fabsf(x.x), fabsf(x.y));
-  const float2 d = __ffma2_rn(ax, make_float2(0.23164189f, 0.23164189f), make_float2(1.0f, 1.0f));
+  const float2 d = ffma2(ax, make_float2(0.23164189f, 0.23164189f), make_float2(1.0f, 1.0f));
   const float2 t = make_float2(fast_rcp(d.x), fast_rcp(d.y));
-  float2 p = __ffma2_rn(t, make_float2(1.061405429f, 1.061405429f), make_float2(-1.453152027f, -1.453152027f));
-  p = __ffma2_rn(p, t, make_float2(1.421413741f, 1.421413741f));
-  p = __ffma2_rn(p, t, make_float2(-0.284496736f, -0.284496736f));
-  p = __ffma2_rn(p, t, make_float2(0.254829592f, 0.254829592f));
+  float2 p = ffma2(t, make_float2(1.061405429f, 1.061405429f), make_float2(-1.453152027f, -1.453152027f));
+  p = ffma2(p, t, make_float2(1.421413741f, 1.421413741f));
+  p = ffma2(p, t, make_float2(-0.284496736f, -0.284496736f));
+  p = ffma2(p, t, make_float2(0.254829592f, 0.254829592f));
   // exp(-x^2/2) = 2^(-(k x)^2), k = sqrt(log2(e) / 2)
-  const float2 y = __fmul2_rn(x, make_float2(0.84932180028801907f, 0.84932180028801907f));
-  const float2 a = __fmul2_rn(make_float2(-y.x, -y.y), y);
+  const float2 y = fmul2(x, make_float2(0.84932180028801907f, 0.84932180028801907f));
+  const float2 a = fmul2(make_float2(-y.x, -y.y), y);
   GeluPair r;
   r.e = make_float2(fast_ex2(a.x), fast_ex2(a.y));
-  const float2 pt = __fmul2_rn(p, t);
-  r.ea = __ffma2_rn(make_float2(-pt.x, -pt.y), r.e, make_float2(1.0f, 1.0f));
+  const float2 pt = fmul2(p, t);
+  r.ea = ffma2(make_float2(-pt.x, -pt.y), r.e, make_float2(1.0f, 1.0f));
   return r;
 }
 __device__ __forceinline__ float2 gelu_erf2(float2 x) {   // 0.5 x (1 + erf(x / sqrt 2)) = hx + |hx| erf(|x| / sqrt 2)
   const GeluPair g = gelu_core2(x);
-  const float2 hx = __fmul2_rn(x, make_float2(0.5f, 0.5f));
-  return __ffma2_rn(make_float2(fabsf(hx.x), fabsf(hx.y)), g.ea, hx);
+  const float2 hx = fmul2(x, make_float2(0.5f, 0.5f));
+  return ffma2(make_float2(fabsf(hx.x), fabsf(hx.y)), g.ea, hx);
 }
 __device__ __forceinline__ float2 gelu_erf_grad2(float2 x) {   // Phi(x) + x phi(x)
   const GeluPair g = gelu_core2(x);
   const float2 se = make_float2(copysignf(g.ea.x, x.x), copysignf(g.ea.y, x.y));
-  const float2 cdf = __ffma2_rn(se, make_float2(0.5f, 0.5f), make_float2(0.5f, 0.5f));
-  const float2 xp = __fmul2_rn(x, make_float2(0.39894228040143267794f, 0.39894228040143267794f));
-  return __ffma2_rn(xp, g.e, cdf);
+  const float2 cdf = ffma2(se, make_float2(0.5f, 0.5f), make_float2(0.5f, 0.5f));
+  const float2 xp = fmul2(x, make_float2(0.39894228040143267794f, 0.39894228040143267794f));
+  return ffma2(xp, g.e, cdf);
 }
 
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-// 2^x for two values on the FMA / ALU pipes (no MUFU): round-to-nearest split x = j + f, f in [-0.5, 0.5], degree-4
-// polynomial for 2^f (rel. error ~4e-5, far below the bf16 rounding of the consumer), exponent patched with an integer
-// add.  The attention kernels send half of their exponentials here: MUFU.EX2 (16 lanes/clk/SM) is their bottleneck
-// while the FMA pipe (128 lanes/clk/SM) idles.  Inputs below -126 flush to ~1e-38.
-__device__ __forceinline__ float2 exp2_poly2(float2 x) {
-  x.x = fmaxf(x.x, -126.0f);
-  x.y = fmaxf(x.y, -126.0f);
-  const float2 magic = make_float2(12582912.0f, 12582912.0f);        // 1.5 * 2^23: low mantissa bits = round(x)
-  const float2 t = __fadd2_rn(x, magic);
-  const float2 jf = __fadd2_rn(t, make_float2(-12582912.0f, -12582912.0f));
-  const float2 f = __fadd2_rn(x, make_float2(-jf.x, -jf.y));
-  float2 pl = __ffma2_rn(f, make_float2(0.0096181291f, 0.0096181291f), make_float2(0.0555041087f, 0.0555041087f));
-  pl = __ffma2_rn(pl, f, make_float2(0.2402265070f, 0.2402265070f));
-  pl = __ffma2_rn(pl, f, make_float2(0.6931471806f, 0.6931471806f));
-  pl = __ffma2_rn(pl, f, make_float2(1.0f, 1.0f));
-  float2 r;
-  r.x = __int_as_float(__float_as_int(pl.x) + (__float_as_int(t.x) << 23));
-  r.y = __int_as_float(__float_as_int(pl.y) + (__float_as_int(t.y) << 23));
-  return r;
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

@@ -17,7 +17,7 @@ __device__ __forceinline__ MS ms_merge(MS a, MS b) {
   return {m, a.s * __expf(a.m - m) + b.s * __expf(b.m - m)};
 }
 
-// lse[row] = logsumexp(logits[row, :V]);  loss_sum += lse - logits[row, y];  count += 1   (rows with y == ignore skipped)
+// lse[row] = logsumexp(logits[row, :V]);  count += 1   (rows with y == ignore skipped; the counts are exact integers)
 __global__ void __launch_bounds__(256)
 ce_fwd_kernel(const bf16* __restrict__ logits, const int64_t* __restrict__ targets, float* __restrict__ lse,
               float* __restrict__ loss_sum_count, int64_t ld, int V, int64_t ignore_index) {
@@ -61,9 +61,29 @@ ce_fwd_kernel(const bf16* __restrict__ logits, const int64_t* __restrict__ targe
     for (int i = 1; i < (blockDim.x >> 5); ++i) t = ms_merge(t, part[i]);
     const float l = t.m + logf(t.s);
     lse[row] = l;
-    atomicAdd(loss_sum_count, l - __bfloat162float(x[y]));
     atomicAdd(loss_sum_count + 1, 1.0f);
   }
+}
+
+// loss_sum += sum over the counted rows of lse - logits[row, y], in row order: 1024 threads take fixed strided subsets
+// of the rows, then a fixed tree (an atomic per row would make the rounding of the sum change from run to run)
+__global__ void __launch_bounds__(1024)
+ce_loss_sum_kernel(const bf16* __restrict__ logits, const int64_t* __restrict__ targets, const float* __restrict__ lse,
+                   float* __restrict__ loss_sum_count, int64_t rows, int64_t ld, int V, int64_t ignore_index) {
+  __shared__ float red[1024];
+  float t = 0.f;
+  for (int64_t row = threadIdx.x; row < rows; row += 1024) {
+    const int64_t y = targets[row];
+    if (y == ignore_index || y < 0 || y >= V) continue;
+    t += lse[row] - __bfloat162float(logits[row * ld + y]);
+  }
+  red[threadIdx.x] = t;
+  __syncthreads();
+  for (int w = 512; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) loss_sum_count[0] += red[0];
 }
 
 // in place: logits[row, v] <- bf16( g * (exp(logits - lse) - [v == y]) ),  g = grad_out / count  (0 for ignored rows)
@@ -120,6 +140,8 @@ extern "C" int oasr_ce_fwd(const void* logits, const int64_t* targets, float* ls
                            int64_t V, int64_t ld, int64_t ignore_index, void* stream) {
   OASR_REQUIRE(rows > 0 && V > 0 && ld >= V && (ld & 7) == 0, "ce_fwd: bad shape rows=%ld V=%ld ld=%ld", (long)rows, (long)V, (long)ld);
   ce_fwd_kernel<<<(unsigned)rows, 256, 0, (cudaStream_t)stream>>>((const bf16*)logits, targets, lse, loss_sum_count, ld, (int)V, ignore_index);
+  OASR_LAUNCH_CHECK();
+  ce_loss_sum_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>((const bf16*)logits, targets, lse, loss_sum_count, rows, ld, (int)V, ignore_index);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }

@@ -14,7 +14,7 @@
 //     feeds mma.sync.m16n8k16 (fp32 accumulate); the preceding LayerNorm, the bias, GELU, the residual add and the
 //     scatter of new K/V rows into the pre-allocated cache are all fused into it -- 6 of the 10 launches per layer;
 //   * dec_attn_scores / dec_attn_pv: single-query attention that reads every cached K and V element once (16-byte
-//     loads, 8 lanes per key row), key ranges split over CTAs when batch x heads cannot fill 148 SMs;
+//     loads, 8 lanes per key row), key ranges split over CTAs when batch x heads cannot fill the SMs;
 //   * dec_sample: logit filters + argmax + log-prob + eot bookkeeping in one pass over the fp32 logits.
 //
 // Rounding points are the reference's in the activation dtype T (inf_model.py:172-196): q*hd^-0.25 and k*hd^-0.25 rounded
@@ -879,8 +879,8 @@ __global__ void convert_kernel(const TI* __restrict__ src, TO* __restrict__ dst,
 
 // Launch with the programmatic-dependent-launch attribute (see pdl_wait above) when OASR_DEC_PDL=1; plainly otherwise.
 inline bool pdl_enabled() {
-  // measured on B200 (profiles/r02_decode_rtf_pdl_ab.txt): inside a CUDA graph the gaps between these kernels are already
-  // ~0 and holding several waiting grids resident costs more than the early weight prefetch gains -> off by default
+  // off by default: inside a CUDA graph the gaps between these kernels are already small, and holding several waiting
+  // grids resident competes with the running one
   static const int v = [] { const char* e = getenv("OASR_DEC_PDL"); return e ? atoi(e) : 0; }();
   return v != 0;
 }
@@ -941,8 +941,7 @@ int launch_linear_direct(const oasr_dec_linear_args& a, cudaStream_t st) {
 }
 template <typename T>
 int dispatch_linear(const oasr_dec_linear_args& a, cudaStream_t st) {
-  // measured on B200 (profiles/r02_decode_profile_*): the direct form wins up to 32 rows (6.7 vs 8.9 us per launch at 1-8
-  // rows), the staged form from there on (23.5 -> 17 us per launch at 64 rows)
+  // the direct form up to 32 rows (no staging round trip for a handful of rows), the staged form from there on
   if (a.M <= 16) return launch_linear_direct<T, 1>(a, st);
   if (a.M <= 32) return launch_linear_direct<T, 2>(a, st);
   return launch_linear<T, 4>(a, st);

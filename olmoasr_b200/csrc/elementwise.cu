@@ -114,20 +114,54 @@ __global__ void embed_fwd_kernel(const int64_t* __restrict__ ids, const float* _
   }
 }
 // dE[id] += dx (skipping padding_idx), dP[s] += dx   (autograd of the above; nn.Embedding padding_idx, model.py:665-667)
-__global__ void embed_bwd_kernel(const int64_t* __restrict__ ids, const bf16* __restrict__ dx,
-                                 float* __restrict__ demb, float* __restrict__ dpos, int64_t rows, int S, int d,
-                                 int64_t padding_idx, int64_t n_rows_emb) {
+// One block per row, sums taken in row order so that the result does not depend on scheduling: the block of a row
+// with b == 0 writes dP[s] (sum over the batch), the block of the FIRST row carrying an id writes dE[id] (sum over
+// every row with that id, gathered 128 rows at a time).
+constexpr int EMB_COLS = 10;   // columns per thread: 128 threads cover d <= 1280 (every OLMoASR width)
+__global__ void __launch_bounds__(128)
+embed_bwd_kernel(const int64_t* __restrict__ ids, const bf16* __restrict__ dx,
+                 float* __restrict__ demb, float* __restrict__ dpos, int64_t rows, int S, int d,
+                 int64_t padding_idx, int64_t n_rows_emb) {
+  __shared__ int64_t s_rows[128];
+  __shared__ int s_cnt[4];
   const int64_t row = blockIdx.x;
   if (row >= rows) return;
-  const int64_t id = ids[row];
-  const int s = static_cast<int>(row % S);
-  const bool do_emb = (id != padding_idx) && id >= 0 && id < n_rows_emb;
-  const bf16* g = dx + row * d;
-  for (int c = threadIdx.x; c < d; c += blockDim.x) {
-    const float v = __bfloat162float(g[c]);
-    if (do_emb) atomicAdd(demb + id * d + c, v);
-    atomicAdd(dpos + static_cast<int64_t>(s) * d + c, v);
+  const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+  if (row < S) {
+    const int64_t batch = rows / S;
+    for (int c = t; c < d; c += blockDim.x) {
+      float v = 0.f;
+      for (int64_t b = 0; b < batch; ++b) v += __bfloat162float(dx[(b * S + row) * d + c]);
+      dpos[row * d + c] += v;
+    }
   }
+  const int64_t id = ids[row];
+  if (id == padding_idx || id < 0 || id >= n_rows_emb) return;
+  for (int64_t base = 0; base < row; base += blockDim.x)   // an earlier row with this id owns the sum
+    if (__syncthreads_or(base + t < row && ids[base + t] == id)) return;
+  float acc[EMB_COLS];
+#pragma unroll
+  for (int j = 0; j < EMB_COLS; ++j) acc[j] = 0.f;
+  for (int64_t base = row; base < rows; base += blockDim.x) {
+    const bool hit = base + t < rows && ids[base + t] == id;
+    const unsigned bal = __ballot_sync(0xffffffffu, hit);
+    if (lane == 0) s_cnt[warp] = __popc(bal);
+    __syncthreads();
+    int before = 0, total = 0;
+    for (int w = 0; w < 4; ++w) { if (w < warp) before += s_cnt[w]; total += s_cnt[w]; }
+    if (hit) s_rows[before + __popc(bal & ((1u << lane) - 1u))] = base + t;
+    __syncthreads();
+    for (int k = 0; k < total; ++k) {   // matches in row order
+      const bf16* g = dx + s_rows[k] * d;
+#pragma unroll
+      for (int j = 0; j < EMB_COLS; ++j)
+        if (t + j * 128 < d) acc[j] += __bfloat162float(g[t + j * 128]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int j = 0; j < EMB_COLS; ++j)
+    if (t + j * 128 < d) demb[id * d + t + j * 128] += acc[j];
 }
 
 // ------------------------------------------------------------------ conv stem data movement
@@ -225,9 +259,10 @@ __global__ void gelu_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restr
 }
 
 // ------------------------------------------------------------------ bias gradient: db[n] += sum_m dy[m,n]
-// Block = 32 x 8 threads; tile = 256 columns (8 per thread, one 16-byte load) x a slab of rows.
+// Block = 32 x 8 threads; tile = 256 columns (8 per thread, one 16-byte load) x a slab of rows.  Each slab of rows
+// writes its column sums to part[slab][n]; add_partials adds the slabs in order.
 __global__ void __launch_bounds__(256)
-colsum_kernel(const bf16* __restrict__ dy, float* __restrict__ db, int64_t M, int N, int64_t ld, int rows_per_block) {
+colsum_kernel(const bf16* __restrict__ dy, float* __restrict__ part, int64_t M, int N, int64_t ld, int rows_per_block) {
   __shared__ float red[8][256 + 8];
   const int col = blockIdx.x * 256 + threadIdx.x * 8;
   const int64_t r0 = static_cast<int64_t>(blockIdx.y) * rows_per_block;
@@ -266,7 +301,7 @@ colsum_kernel(const bf16* __restrict__ dy, float* __restrict__ db, int64_t M, in
   float a = 0.f;
 #pragma unroll
   for (int j = 0; j < 8; ++j) a += red[j][t];
-  if (blockIdx.x * 256 + t < N) atomicAdd(db + blockIdx.x * 256 + t, a);
+  if (blockIdx.x * 256 + t < N) part[static_cast<int64_t>(blockIdx.y) * N + blockIdx.x * 256 + t] = a;
 }
 
 }  // namespace
@@ -321,7 +356,7 @@ extern "C" int oasr_embed_fwd(const int64_t* ids, const float* emb, const float*
 
 extern "C" int oasr_embed_bwd(const int64_t* ids, const void* dx, float* demb, float* dpos, int64_t batch, int64_t S,
                               int64_t d, int64_t padding_idx, int64_t n_rows_emb, void* stream) {
-  OASR_REQUIRE(batch > 0 && S > 0, "embed_bwd: bad shape");
+  OASR_REQUIRE(batch > 0 && S > 0 && d <= 128 * EMB_COLS, "embed_bwd: bad shape");
   embed_bwd_kernel<<<(unsigned)(batch * S), 128, 0, (cudaStream_t)stream>>>(ids, (const bf16*)dx, demb, dpos, batch * S, (int)S, (int)d,
                                                                            padding_idx, n_rows_emb);
   OASR_LAUNCH_CHECK();
@@ -371,7 +406,12 @@ extern "C" int oasr_colsum_bf16(const void* dy, float* db, int64_t M, int64_t N,
   int row_blocks = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(M, 64), (num_sms() * 6) / col_tiles + 1));
   const int rows_per_block = (int)ceil_div(M, row_blocks);
   row_blocks = (int)ceil_div(M, rows_per_block);
-  colsum_kernel<<<dim3(col_tiles, row_blocks), dim3(32, 8), 0, (cudaStream_t)stream>>>((const bf16*)dy, db, M, (int)N, ld, rows_per_block);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* part = static_cast<float*>(scratch_alloc(sizeof(float) * row_blocks * N, st));
+  if (!part) return OASR_ERR_CUDA;
+  colsum_kernel<<<dim3(col_tiles, row_blocks), dim3(32, 8), 0, st>>>((const bf16*)dy, part, M, (int)N, ld, rows_per_block);
   OASR_LAUNCH_CHECK();
-  return OASR_OK;
+  const int rc = add_partials(part, row_blocks, N, db, st);
+  scratch_free(part, st);
+  return rc;
 }

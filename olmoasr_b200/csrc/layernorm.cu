@@ -70,7 +70,7 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ w, co
 // Backward.  One warp per row (grid-stride), lane l owns the same 8-column vectors l, l+32, ... of every row it visits,
 // so the parameter gradients (column sums of dy*xhat and dy) accumulate in that lane's registers with no shared-memory
 // traffic and no block barrier inside the row loop; the 8 warps of a block are folded through shared memory once at
-// the end, then one atomicAdd per column and block.  x and dy stay packed (bf16) in registers between the statistics
+// the end into this block's partial column sums, which add_partials adds up in block order.  x and dy stay packed (bf16) in registers between the statistics
 // pass and the dx pass and are unpacked twice -- 32 registers instead of 64.  (History: all-fp32-in-registers needed
 // 214 registers -> 23 % of the HBM roofline; staging every row through shared memory with two __syncthreads per 8
 // rows -> 37 %.)
@@ -78,8 +78,8 @@ template <int NV>
 __global__ void __launch_bounds__(256, 2)
 layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ w,
                      const float* __restrict__ mean, const float* __restrict__ rstd,
-                     const bf16* __restrict__ dres, bf16* __restrict__ dx, float* __restrict__ dw,
-                     float* __restrict__ db, int64_t rows, int d) {
+                     const bf16* __restrict__ dres, bf16* __restrict__ dx, float* __restrict__ part,
+                     int64_t rows, int d) {
   extern __shared__ __align__(16) float fold[];  // [8][d], used once at the end
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -131,13 +131,13 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
         const uint32_t gw[4] = {ug[i].x, ug[i].y, ug[i].z, ug[i].w};
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          const float2 xh = __fmul2_rn(__fadd2_rn(unpack_bf16x2(xw[j]), make_float2(-mu, -mu)), rs2);
+          const float2 xh = fmul2(fadd2(unpack_bf16x2(xw[j]), make_float2(-mu, -mu)), rs2);
           const float2 g = unpack_bf16x2(gw[j]);
-          const float2 gwj = __fmul2_rn(g, ww[j]);
-          s1 = __fadd2_rn(s1, gwj);
-          s2 = __ffma2_rn(gwj, xh, s2);
-          acc_w[i][j] = __ffma2_rn(g, xh, acc_w[i][j]);
-          acc_b[i][j] = __fadd2_rn(acc_b[i][j], g);
+          const float2 gwj = fmul2(g, ww[j]);
+          s1 = fadd2(s1, gwj);
+          s2 = ffma2(gwj, xh, s2);
+          acc_w[i][j] = ffma2(g, xh, acc_w[i][j]);
+          acc_b[i][j] = fadd2(acc_b[i][j], g);
         }
       }
     }
@@ -159,14 +159,14 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
         uint32_t ow[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          const float2 xh = __fmul2_rn(__fadd2_rn(unpack_bf16x2(xw[j]), make_float2(-mu, -mu)), rs2);
-          const float2 gwj = __fmul2_rn(unpack_bf16x2(gw[j]), ww[j]);
+          const float2 xh = fmul2(fadd2(unpack_bf16x2(xw[j]), make_float2(-mu, -mu)), rs2);
+          const float2 gwj = fmul2(unpack_bf16x2(gw[j]), ww[j]);
           // rs * (g*w - mean(g*w) - xhat * mean(g*w*xhat))
-          float2 o = __ffma2_rn(xh, make_float2(-m2, -m2), __fadd2_rn(gwj, make_float2(-m1, -m1)));
-          o = __fmul2_rn(o, rs2);
+          float2 o = ffma2(xh, make_float2(-m2, -m2), fadd2(gwj, make_float2(-m1, -m1)));
+          o = fmul2(o, rs2);
           if (rr) {
             const float2 ob = unpack_bf16x2(pack_bf16x2(o.x, o.y));   // bf16(dx_ln) first, like autograd's accumulation
-            o = __fadd2_rn(unpack_bf16x2(rw[j]), ob);
+            o = fadd2(unpack_bf16x2(rw[j]), ob);
           }
           ow[j] = pack_bf16x2(o.x, o.y);
         }
@@ -175,7 +175,7 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
     }
   }
 
-  // fold the 8 warps' accumulators (two passes through one [8][d] buffer), one global atomic per column and block
+  // fold the 8 warps' accumulators (two passes through one [8][d] buffer) into part[pass][block][d]
 #pragma unroll
   for (int pass = 0; pass < 2; ++pass) {
     __syncthreads();
@@ -190,12 +190,12 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
       }
     }
     __syncthreads();
-    float* out = pass == 0 ? dw : db;
+    float* out = part + (static_cast<int64_t>(pass) * gridDim.x + blockIdx.x) * d;
     for (int c = threadIdx.x; c < d; c += 256) {
       float t = 0.f;
 #pragma unroll
       for (int r = 0; r < 8; ++r) t += fold[r * d + c];
-      atomicAdd(out + c, t);
+      out[c] = t;
     }
   }
 }
@@ -241,9 +241,11 @@ extern "C" int oasr_layernorm_bwd(const void* dy, const void* x, const float* we
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int wpb = 8;
   int64_t blocks = ceil_div(rows, wpb);
-  const int64_t cap = static_cast<int64_t>(num_sms()) * 2;  // 2 resident blocks per SM; few blocks => few global atomics
+  const int64_t cap = static_cast<int64_t>(num_sms()) * 2;  // 2 resident blocks per SM; few blocks => few partials
   if (blocks > cap) blocks = cap;
   const size_t smem = 8 * d * sizeof(float);
+  float* part = static_cast<float*>(scratch_alloc(sizeof(float) * 2 * blocks * d, st));
+  if (!part) return OASR_ERR_CUDA;
 #define OASR_LN_BWD(NVv)                                                                                              \
   do {                                                                                                                 \
     static bool attr_set = false;                                                                                      \
@@ -252,7 +254,7 @@ extern "C" int oasr_layernorm_bwd(const void* dy, const void* x, const float* we
       attr_set = true;                                                                                                 \
     }                                                                                                                  \
     layernorm_bwd_kernel<NVv><<<(int)blocks, wpb * 32, smem, st>>>(                                                    \
-        (const bf16*)dy, (const bf16*)x, weight, mean, rstd, (const bf16*)dresidual, (bf16*)dx, dweight, dbias, rows, (int)d); \
+        (const bf16*)dy, (const bf16*)x, weight, mean, rstd, (const bf16*)dresidual, (bf16*)dx, part, rows, (int)d); \
   } while (0)
   switch ((int)ceil_div(d, 256)) {
     case 1: case 2: OASR_LN_BWD(2); break;
@@ -262,5 +264,8 @@ extern "C" int oasr_layernorm_bwd(const void* dy, const void* x, const float* we
   }
 #undef OASR_LN_BWD
   OASR_LAUNCH_CHECK();
-  return OASR_OK;
+  int rc = add_partials(part, (int)blocks, d, dweight, st);
+  if (rc == OASR_OK) rc = add_partials(part + blocks * d, (int)blocks, d, dbias, st);
+  scratch_free(part, st);
+  return rc;
 }

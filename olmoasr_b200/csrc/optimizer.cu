@@ -19,22 +19,22 @@ struct TensorRec {  // one row of the device-side table (6 x int64)
   bf16* shadow;  // optional bf16 copy of p, refreshed by the update itself (nullptr: none)
 };
 
-// sum over the block, one atomic per block.  Callers square UNSCALED values (g * inv_scale) so that a 65536x loss scale
-// cannot overflow the fp32 total.
-__device__ __forceinline__ void block_sum_to(float s, float* out) {
+// sum over the block into this block's partial (added up in block order afterwards: add_partials).  Callers square
+// UNSCALED values (g * inv_scale) so that a 65536x loss scale cannot overflow the fp32 total.
+__device__ __forceinline__ void block_sum_to(float s, float* part) {
   s = warp_sum(s);
-  __shared__ float part[8];
-  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
+  __shared__ float part_w[8];
+  if ((threadIdx.x & 31) == 0) part_w[threadIdx.x >> 5] = s;
   __syncthreads();
   if (threadIdx.x == 0) {
     float t = 0.f;
-    for (int i = 0; i < 8; ++i) t += part[i];
-    atomicAdd(out, t);
+    for (int i = 0; i < 8; ++i) t += part_w[i];
+    part[blockIdx.x] = t;
   }
 }
 
 __global__ void __launch_bounds__(256)
-grad_sqnorm_kernel(const TensorRec* __restrict__ recs, const int2* __restrict__ chunks, float* __restrict__ out,
+grad_sqnorm_kernel(const TensorRec* __restrict__ recs, const int2* __restrict__ chunks, float* __restrict__ part,
                    float inv_scale) {
   const int2 ch = chunks[blockIdx.x];
   const TensorRec r = recs[ch.x];
@@ -54,12 +54,12 @@ grad_sqnorm_kernel(const TensorRec* __restrict__ recs, const int2* __restrict__ 
   } else {
     for (int i = threadIdx.x; i < n; i += blockDim.x) { const float a = g[i] * k; s += a * a; }
   }
-  block_sum_to(s, out);
+  block_sum_to(s, part);
 }
 
 // Same reduction over one flat gradient slab (olmoasr_b200.slab): no table, every block owns CHUNK elements.
 __global__ void __launch_bounds__(256)
-sqnorm_flat_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ out, float inv_scale) {
+sqnorm_flat_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ part, float inv_scale) {
   const int64_t start = static_cast<int64_t>(blockIdx.x) * CHUNK;
   const int m = static_cast<int>(min(n, start + CHUNK) - start);
   g += start;
@@ -71,7 +71,7 @@ sqnorm_flat_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ o
     s += a * a + b * b + c * c + d * d;
   }
   for (int i = (m & ~3) + threadIdx.x; i < m; i += blockDim.x) { const float a = g[i] * k; s += a * a; }
-  block_sum_to(s, out);
+  block_sum_to(s, part);
 }
 
 // One thread: turns the squared norm into the step's scalars.  The step counter lives on the device and advances only
@@ -174,18 +174,29 @@ extern "C" int oasr_optim_chunk_elems(void) { return CHUNK; }
 
 extern "C" int oasr_grad_sqnorm(const void* recs, const void* chunks, int64_t n_chunks, float inv_scale, float* out, void* stream) {
   OASR_REQUIRE(n_chunks > 0, "grad_sqnorm: no chunks");
-  OASR_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float), (cudaStream_t)stream));
-  grad_sqnorm_kernel<<<(unsigned)n_chunks, 256, 0, (cudaStream_t)stream>>>((const TensorRec*)recs, (const int2*)chunks, out, inv_scale);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* part = static_cast<float*>(scratch_alloc(sizeof(float) * n_chunks, st));
+  if (!part) return OASR_ERR_CUDA;
+  OASR_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float), st));
+  grad_sqnorm_kernel<<<(unsigned)n_chunks, 256, 0, st>>>((const TensorRec*)recs, (const int2*)chunks, part, inv_scale);
   OASR_LAUNCH_CHECK();
-  return OASR_OK;
+  const int rc = add_partials(part, (int)n_chunks, 1, out, st);
+  scratch_free(part, st);
+  return rc;
 }
 
 extern "C" int oasr_grad_sqnorm_flat(const float* g, int64_t numel, float inv_scale, float* out, void* stream) {
   OASR_REQUIRE(numel > 0 && ((uintptr_t)g & 15) == 0, "grad_sqnorm_flat: empty or unaligned slab");
-  OASR_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float), (cudaStream_t)stream));
-  sqnorm_flat_kernel<<<(unsigned)ceil_div(numel, CHUNK), 256, 0, (cudaStream_t)stream>>>(g, numel, out, inv_scale);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t blocks = ceil_div(numel, CHUNK);
+  float* part = static_cast<float*>(scratch_alloc(sizeof(float) * blocks, st));
+  if (!part) return OASR_ERR_CUDA;
+  OASR_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(float), st));
+  sqnorm_flat_kernel<<<(unsigned)blocks, 256, 0, st>>>(g, numel, part, inv_scale);
   OASR_LAUNCH_CHECK();
-  return OASR_OK;
+  const int rc = add_partials(part, (int)blocks, 1, out, st);
+  scratch_free(part, st);
+  return rc;
 }
 
 extern "C" int oasr_optim_prepare(const float* norm_sq, float* found_inf, float* state, float inv_scale, float max_norm,

@@ -1,8 +1,7 @@
 """Block-wise gradient all-reduce: a leaner stand-in for DistributedDataParallel on this path (opt-in).
 
 The reference wraps the model in `DDP(model, device_ids=[rank])` (scripts/training/train_timestamps.py:2329-2330): 25 MB
-buckets, one flatten-copy and one divide kernel per parameter (946 + 948 launches per step at medium, 7 ms of device
-time, profiles/r01_step_profile_ddp_2gpu.txt) and 87 all-reduce launches wherever a bucket happens to fill.  Here the
+buckets, one flatten-copy and one divide kernel per parameter (946 + 948 launches per step at medium) and 87 all-reduce launches wherever a bucket happens to fill.  Here the
 gradients stay where the backward kernels wrote them: when the last parameter of a ResidualAttentionBlock has its
 gradient, the block's tensors are summed across ranks by ONE coalesced NCCL call (ncclGroupStart / ncclAllReduce per
 tensor / ncclGroupEnd -- no flattening), and the 1 / world_size average is folded into the fused optimizer's
@@ -14,7 +13,7 @@ tensor / ncclGroupEnd -- no flattening), and the 1 / world_size average is folde
 
 Same collective order on every rank (the autograd graph is the same), same result as DDP up to fp32 summation order.
 
-`SlabGradSync` (below) is the B200-first form and what bench.py uses: gradients already live in ONE flat fp32 slab in
+`SlabGradSync` (below) is the preferred form and what bench.py uses: gradients already live in ONE flat fp32 slab in
 backward-completion order (olmoasr_b200/slab.py), so the sum across ranks is a handful of large contiguous all-reduces
 -- NCCL's bandwidth regime over NVLink 5 / NVSwitch instead of 87 latency-protocol bucket launches -- issued as soon as
 the backward has finished a slab range, with no flatten copies and no per-parameter divides.

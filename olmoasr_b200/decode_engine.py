@@ -9,13 +9,13 @@ What the reference does per step and what replaces it:
   * builds the causal mask on the CPU and copies it over (:341-352)     -> single-query kernels need no mask
   * torch.cat of every self-attention K / V (hooks, :439-445)           -> pre-allocated (L, 2, N, 448, d) cache written
                                                                            in place by the fused QKV projection's epilogue
-  * cross-attention K / V projected once, kept in the hook dict         -> projected once by the tcgen05 GEMM into a static
+  * cross-attention K / V projected once, kept in the hook dict         -> projected once by the wgmma GEMM into a static
                                                                            (L, N*1500, 2d) buffer
   * 4 small matmul / softmax kernels per attention + separate LN, bias,
     GELU, residual kernels                                               -> 8-9 launches per layer (csrc/decode.cu), 100-112 per step (small)
 
 The activation dtype is fp16 (upstream default `fp16=True`) or bf16; the decoder-step kernels reproduce the reference's
-rounding points in that dtype.  The audio encoder and the cross K/V projection run on the bf16 tcgen05 kernels in both
+rounding points in that dtype.  The audio encoder and the cross K/V projection run on the bf16 wgmma kernels in both
 cases (their bf16 outputs are converted to fp16 for an fp16 decoder).
 """
 from __future__ import annotations
@@ -161,8 +161,8 @@ class DecodeEngine:
             _lib.LAUNCH_COUNT -= 1      # an unsplit key range runs as ONE fused kernel (scores + softmax + P V), not two
 
     def cross_splits(self, n: int) -> int:
-        """Key-range splits of the cross-attention so that n x H x splits CTAs cover the 148 SMs about twice (>= 188 keys each)."""
-        return max(1, min(self.max_splits, math.ceil(2 * 148 / (n * self.H))))
+        """Key-range splits of the cross-attention so that n x H x splits CTAs cover the SMs about twice."""
+        return max(1, min(self.max_splits, math.ceil(2 * _lib.lib().oasr_device_sm_count() / (n * self.H))))
 
     def _enqueue_step(self, n: int):
         """One decoder step for sequences [0, n): per layer 6 fused Linear launches, 1 self-attention launch and 1 (unsplit key
@@ -223,7 +223,7 @@ class DecodeEngine:
     @torch.no_grad()
     def prepare(self, audio_features: Tensor):
         """Project the encoder output into every layer's cross-attention K / V once (inf_model.py:164-167: `kv_cache[self.key]`
-        is filled on the first call and only read afterwards) with the tcgen05 GEMM."""
+        is filled on the first call and only read afterwards) with the wgmma GEMM."""
         from ._core import _as_bf16_2d, linear_fwd
 
         self.refresh_weights()

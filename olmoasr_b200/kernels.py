@@ -34,7 +34,7 @@ def _req(cond, msg):
 
 def gemm(a, b, M, N, K, *, a_mn=False, b_mn=False, out=None, out2=None, bias=None, aux=None,
          epi=EPI_BF16, split_k=1, block_n=0):
-    """D[M,N] = epi(sum_k A[m,k] B[n,k]) on tcgen05.  `a` is (M,K) (or (K,M) when a_mn), `b` is (N,K)
+    """D[M,N] = epi(sum_k A[m,k] B[n,k]) on wgmma.  `a` is (M,K) (or (K,M) when a_mn), `b` is (N,K)
     (or (K,N) when b_mn); both bf16 with unit inner stride.  See include/oasr_b200.h."""
     _req(a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16, "gemm: operands must be bf16")
     _req(a.is_cuda and b.is_cuda, "gemm: operands must be CUDA tensors")
@@ -121,16 +121,11 @@ _BWD_PERSISTENT_USER = os.environ.get("OASR_BWD_PERSISTENT")   # an explicit set
 
 
 def _choose_attention_bwd_mode(world_size=None):
-    """The backward attention kernel is persistent (one CTA per SM walking over its share of the work items) unless NCCL
-    collectives are resident next to the backward pass for a large part of it.  A resident all-reduce kernel takes SMs away
-    (its CTAs cannot share an SM with a 224 KB CTA); a statically partitioned persistent grid then runs its displaced CTAs as
-    a second wave -- between the 1-GPU and the 8-GPU profile (side stream on in both) the persistent GEMMs' kernel time grows
-    from 120 to 147 ms (+22 %) where the then one-CTA-per-item attention backward grew from 50.5 to 55.1 ms (+9 %)
-    (profiles/r02_step_profile_sidestream.txt, r02_step_profile_slabsync_8gpu.txt).  One CTA per item degrades in proportion to
-    the SMs it loses (32 of 148: +28 % while a collective is resident, against +100 % for a displaced second wave), so that
-    launch shape is used in jobs of more than 2 GPUs; at 2 GPUs the collectives are resident for 9 ms of a 200 ms step and
-    the persistent shape measured faster (profiles/r02_bench_2gpu_final.json).  Both shapes run the same code and are
-    covered by the parity tests; the forward pass does not overlap the gradient all-reduces and stays persistent."""
+    """Launch-shape policy of the backward attention kernel, published as OASR_BWD_PERSISTENT: a persistent grid (one CTA
+    per SM walking over the work items) up to 2 GPUs, one CTA per work item beyond, where resident NCCL collectives take
+    SMs away and a statically partitioned persistent grid would run its displaced CTAs as a second wave.  The sm_90a
+    kernel (csrc/attention_bwd_sm90.cu) launches one CTA per work item in every job, which is the shape this policy asks
+    for under collectives; an explicit setting of the user always wins."""
     if _BWD_PERSISTENT_USER is not None:
         return
     if world_size is None:
@@ -155,9 +150,8 @@ def attention_bwd(q, k, v, o, dout, lse, B, H, Tq, Tkv, causal=False, kv_len=Non
     if dv is None:
         dv = torch.empty((B * Tkv, H * 64), device=dev, dtype=torch.bfloat16)
     delta = torch.empty((B, H, Tq), device=dev, dtype=torch.float32)
-    dq_accum = torch.empty((B * Tq, H * 64), device=dev, dtype=torch.float32)
     call("oasr_attention_bwd", ptr(q), q.stride(0), ptr(k), k.stride(0), ptr(v), v.stride(0), ptr(o), o.stride(0),
-         ptr(dout), dout.stride(0), ptr(lse), ptr(delta), ptr(dq_accum), ptr(dq), dq.stride(0), ptr(dk), dk.stride(0),
+         ptr(dout), dout.stride(0), ptr(lse), ptr(delta), ptr(dq), dq.stride(0), ptr(dk), dk.stride(0),
          ptr(dv), dv.stride(0), B, H, Tq, Tkv, 64, int(causal), ptr(kv_len), float(scale), stream())
     return dq, dk, dv
 

@@ -8,7 +8,7 @@ layout:
     P  fp32 master weights      (every nn.Parameter is a view into it; state_dict names / shapes are unchanged)
     G  fp32 gradients           (p.grad is a view; wgrad GEMM epilogues accumulate straight into it)
     M, V  fp32 AdamW moments    (optimizer state views, torch.optim.AdamW's names)
-    S  bf16 shadow of P         (what the tcgen05 GEMMs read; rewritten by the AdamW kernel from registers)
+    S  bf16 shadow of P         (what the wgmma GEMMs read; rewritten by the AdamW kernel from registers)
 
 so that the optimizer is three launches over flat memory, zero_grad is one memset, the bf16 weights cost no extra
 pass, and a data-parallel gradient sum is a handful of large contiguous NCCL all-reduces (`SlabGradSync` in ddp.py)

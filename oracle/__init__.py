@@ -17,6 +17,6 @@ Contents
                GreedyDecoder / SuppressBlank / SuppressTokens).  The upstream package is absent here, so
                the LOOP is "parity unpinned"; the model calls inside it are pinned through model.py.
   synth.py     the synthetic batch of SURVEY.md section 8(d).
-  ref_import.py  imports /root/reference/olmoasr/{model,inf_model}.py unmodified behind three stub
-               modules (only works where /root/reference exists, i.e. the build container).
+  ref_import.py  imports olmoasr/{model,inf_model}.py unmodified behind three stub
+               modules (only where OLMOASR_REFERENCE_ROOT names a reference checkout).
 """

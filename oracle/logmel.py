@@ -3,7 +3,7 @@
 Reference call sites: scripts/training/train_timestamps.py:196-214 (int16 -> /32768 -> pad_or_trim ->
 log_mel_spectrogram), scripts/eval/eval.py:157-162, olmoasr/transcribe.py:148; re-exported at
 olmoasr/__init__.py:21.  The arithmetic lives in openai-whisper `whisper/audio.py` (absent from
-/root/reference); this file restates its published algorithm:
+the reference checkout); this file restates its published algorithm:
 
     pad_or_trim(array, 480000)            zero-pad / truncate the last axis
     stft  = torch.stft(audio, 400, 160, window=hann(400), center=True (reflect pad), return_complex)

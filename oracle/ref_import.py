@@ -2,8 +2,8 @@
 
 `import olmoasr` fails in this container (openai-whisper is absent and cannot be installed), but
 olmoasr/model.py and olmoasr/inf_model.py only need `whisper.decoding.{decode,detect_language}` and
-`olmoasr.transcribe.transcribe` as attributes at import time.  /root/reference exists only in the build
-container: everything here is used to VALIDATE oracle/model.py and to GENERATE tests/golden/*, never at
+`olmoasr.transcribe.transcribe` as attributes at import time.  The reference checkout (OLMOASR_REFERENCE_ROOT) is
+only needed where golden data is generated: everything here is used to VALIDATE oracle/model.py and to GENERATE tests/golden/*, never at
 run time on the GPU box.
 """
 from __future__ import annotations
@@ -13,11 +13,11 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("OLMOASR_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("OLMOASR_REFERENCE_ROOT", "")   # a checkout of allenai/OLMoASR
 
 
 def available() -> bool:
-    return os.path.isfile(os.path.join(REFERENCE_ROOT, "olmoasr", "model.py"))
+    return bool(REFERENCE_ROOT) and os.path.isfile(os.path.join(REFERENCE_ROOT, "olmoasr", "model.py"))
 
 
 def _stub(name, **attrs):

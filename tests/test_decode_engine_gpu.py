@@ -136,6 +136,7 @@ def test_greedy_token_ids_match_the_reference_loop(variant, fp16):
     opts = DecodingOptions(language="en", without_timestamps=True, sample_len=n_steps, fp16=fp16)
     task = DecodingTask(m, opts)
     want, margins, sum_lp, nsp = _ref_greedy(OM, sd, dims, xa, dtype, n_steps, task.suppress)
+    want32, _, sum_lp32, _ = _ref_greedy(OM, sd, dims, xa, torch.float32, n_steps, task.suppress)
     res = decode(m, xa, opts)                                        # encoded features are accepted like upstream
     got = [r.tokens for r in res]
     # token ids are compared up to the first step at which the REFERENCE's own top-1 / top-2 margin drops into rounding
@@ -150,7 +151,11 @@ def test_greedy_token_ids_match_the_reference_loop(variant, fp16):
         assert got[k][:n_cmp] == seq[:n_cmp], k
         if n_cmp == len(margins):
             assert got[k] == seq
-            assert abs(res[k].avg_logprob - float(sum_lp[k]) / (len(seq) + 1)) <= 2e-2 * abs(float(sum_lp[k]) / (len(seq) + 1)) + 1e-3
+            # the reference's log-probs come from logits rounded to the activation dtype: besides the fixed tolerance, a
+            # result may sit as far from them as the reference's own rounding moved them off its fp32 run (same tokens)
+            lp_ref = float(sum_lp[k]) / (len(seq) + 1)
+            rounding = abs(lp_ref - float(sum_lp32[k]) / (len(seq) + 1)) if torch.equal(want32[k], want[k]) else 0.0
+            assert abs(res[k].avg_logprob - lp_ref) <= 2e-2 * abs(lp_ref) + 1e-3 + 2.0 * rounding
         assert abs(res[k].no_speech_prob - float(nsp[k])) <= 0.05 * float(nsp[k]) + 1e-6
     eng = m.decode_engine(dtype)
     cross = 1 if eng.cross_splits(xa.shape[0]) == 1 else 2
@@ -175,7 +180,8 @@ def test_batch_size_independence_and_split_paths():
             ref = toks[0]
         assert torch.equal(toks[0], ref), n
         assert all(torch.equal(toks[i], toks[i % 2]) for i in range(n)), n
-        assert eng.cross_splits(n) == max(1, min(eng.max_splits, math.ceil(296 / (n * dims.n_text_head))))
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+        assert eng.cross_splits(n) == max(1, min(eng.max_splits, math.ceil(2 * sms / (n * dims.n_text_head))))
 
 
 def test_sampling_kernel_bookkeeping():

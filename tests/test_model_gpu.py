@@ -122,7 +122,7 @@ def test_no_padding_mask_path_and_error_behaviour(setup):
 
 # =====================================================================================================================
 # The benchmarked variants (BASELINE.json configs 2, 3, 5): real width / head count, so the kernels run the tile shapes,
-# grids and vector widths of the benchmark (N = 1024 / 3072 / 4096 2-CTA tiles, 16 heads, d = 1024 LayerNorm rows,
+# grids and vector widths of the benchmark (N = 1024 / 3072 / 4096 GEMM tiles, 16 heads, d = 1024 LayerNorm rows,
 # K = 3000-row split-K wgrads, the M-fastest logits raster), at depth 2+2 so that the fp32 oracle finishes in seconds.
 # Tolerances, as for tiny: loss within 1e-3 relative (north_star); logits and gradients as close to the fp32 oracle as the
 # REFERENCE'S OWN bf16-autocast run is (yardsticks recorded from the reference in tests/golden/model_<v>_2x2.pt).

@@ -1,13 +1,15 @@
-"""Generate tests/golden/* from the UNMODIFIED reference (run in the build container only).
+"""Generate tests/golden/* from the UNMODIFIED reference.
 
-    python tools/make_golden.py
+    OLMOASR_REFERENCE_ROOT=<checkout of allenai/OLMoASR> python tools/make_golden.py
 
   logmel_hf.npz     transformers.WhisperFeatureExtractor (independent implementation of the upstream
                     whisper log-mel) on seeded waveforms, frame-subsampled.
-  model_tiny.pt     outputs of /root/reference/olmoasr/model.py (tiny, seed 0) on the seeded synthetic batch:
+  model_tiny.pt     outputs of olmoasr/model.py (tiny, seed 0) on the seeded synthetic batch:
                     fp32 and bf16-autocast logits samples, losses, gradient norms; plus per-tensor weight
                     checksums so that the oracle's re-created weights can be pinned on any box.
-  inf_tiny.pt       /root/reference/olmoasr/inf_model.py: full-prefix logits sample and kv-cache step logits.
+  inf_tiny.pt       olmoasr/inf_model.py: full-prefix logits sample and kv-cache step logits.
+  ref_tiny_outputs.pt  the reference's train-model forward (tiny, seed 0) in fp32 and under CPU bf16 autocast: dense
+                    logits samples and whole-tensor sums, what the oracle is compared with element for element.
 """
 import sys
 from pathlib import Path
@@ -106,6 +108,24 @@ def golden_model():
     print("inf_tiny.pt")
 
 
+def golden_ref_outputs():
+    ref_model, ref_inf, ref_dims = ref_import.load()
+    torch.manual_seed(0)
+    rm = ref_model.OLMoASR(ref_dims.VARIANT_TO_DIMS["tiny"])
+    mel = torch.from_numpy(logmel.log_mel_spectrogram(synth.waveforms(2).numpy()))
+    ti, ty, pm, _ = synth.text_batch(2)
+    with torch.no_grad():
+        l32 = rm(mel, ti, pm)
+        with torch.autocast("cpu", dtype=torch.bfloat16):
+            lbf = rm(mel, ti, pm)
+    torch.save({
+        "fp32_sample": l32[:, ::16, ::97].clone(), "fp32_sum": float(l32.double().sum()), "fp32_abs_sum": float(l32.double().abs().sum()),
+        "bf16_sample": lbf[:, ::16, ::97].float().clone(), "bf16_dtype": str(lbf.dtype),
+        "torch_version": torch.__version__,
+    }, OUT / "ref_tiny_outputs.pt")
+    print("ref_tiny_outputs.pt", tuple(l32.shape), lbf.dtype)
+
+
 def golden_grad_noise():
     """Per-tensor relative L2 distance between the reference's bf16-autocast gradients and its fp32 gradients
     (tiny, seed 0, the synthetic batch): the yardstick for gradient parity of any bf16 implementation."""
@@ -178,11 +198,13 @@ def golden_widths(depth=(2, 2)):
 
 
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["logmel", "model", "grad_noise", "widths"]
+    which = sys.argv[1:] or ["logmel", "model", "ref_outputs", "grad_noise", "widths"]
     if "logmel" in which:
         golden_logmel()
     if "model" in which:
         golden_model()
+    if "ref_outputs" in which:
+        golden_ref_outputs()
     if "grad_noise" in which:
         golden_grad_noise()
     if "widths" in which:
