@@ -36,8 +36,12 @@ def _sm_count() -> int:
 
 
 def _pick_block_n(M: int, N: int) -> int:
-    """Tile width for the persistent GEMM: 128 (the widest sm_90a tile, csrc/gemm_sm90.cu) unless N fits a 64-wide tile."""
-    return 64 if N <= 64 else 128
+    """Tile width (256, 128 or 64) for the persistent GEMM (csrc/gemm_sm90.cu): the one that loads the fewest operand
+    rows per SM, i.e. waves of the persistent grid times the 128 + BN rows of A and B one k-block of a tile reads.  Wave
+    quantisation and the padding of N to a whole tile both count; ties go to the wider tile."""
+    sms = _sm_count()
+    tiles_m = math.ceil(M / 128)
+    return min((256, 128, 64), key=lambda bn: math.ceil(tiles_m * math.ceil(N / bn) / sms) * (128 + bn))
 
 
 def _pick_split_k(tiles: int, kblocks: int) -> int:

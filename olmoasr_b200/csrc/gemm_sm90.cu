@@ -5,12 +5,13 @@
 //
 // One CTA per SM (at most gemm_sm_budget() CTAs), walking over 128 x BN output tiles with stride gridDim.x.  384 threads:
 //   warpgroup 0    TMA producer (one thread issues; the ring keeps running across tiles, so the next tile's operands
-//                  arrive while this tile's epilogue runs)
-//   warpgroups 1-2 consumers: warpgroup c owns rows 64c .. 64c+63 of the tile, issues its m64 x BN x 16 wgmmas and runs
-//                  the epilogue for those rows
-// Tile = 128 x BN (BN = 64 or 128), BK = 64 bf16 (= one 128-byte swizzle row).  Both operand majors are supported
-// through the wgmma descriptors and transpose bits, so dgrad (B MN-major) and wgrad (A and B MN-major) need no
-// transposes in HBM.  Reference ops replaced: olmoasr/model.py:97-101 (Linear.forward) and its
+//                  arrive while this tile's epilogue runs).  It gives its registers up (setmaxnreg 40) ...
+//   warpgroups 1-2 ... to the consumers (setmaxnreg 232): warpgroup c owns rows 64c .. 64c+63 of the tile, issues its
+//                  m64 x BN x 16 wgmmas and runs the epilogue for those rows
+// Tile = 128 x BN (BN = 64, 128 or 256; 256 keeps 128 fp32 accumulators per consumer thread), BK = 64 bf16 (= one
+// 128-byte swizzle row).  Both operand majors are supported through the wgmma descriptors and transpose bits, so dgrad
+// (B MN-major) and wgrad (A and B MN-major) need no transposes in HBM.  The epilogue is a template parameter: each
+// kernel carries only its own store code.  Reference ops replaced: olmoasr/model.py:97-101 (Linear.forward) and its
 // autograd, model.py:768-770 (tied logits), model.py:592-593 (Conv1d after im2col).
 #include "common.cuh"
 #include "ptx_sm90.cuh"
@@ -25,6 +26,8 @@ constexpr int BM = 128;
 constexpr int BK = 64;               // 64 bf16 = 128 B = swizzle span
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
 constexpr int THREADS = 384;
+constexpr int PRODUCER_REGS = 40;    // 40 * 128 + 232 * 256 <= 64 K registers of the SM
+constexpr int CONSUMER_REGS = 232;
 
 struct GemmParams {
   void* C;
@@ -36,7 +39,6 @@ struct GemmParams {
   int M, N, K;
   int tiles_m, tiles_n, splits;
   int kblocks_total, kblocks_per_split;
-  int epi;
   int raster_m;  // 1: consecutive tiles walk M first (B tile stays hot in L2) -- used when B is the larger operand
   int64_t split_stride;   // split-K: split s stores its fp32 partial at C + s * split_stride (0: one split)
 };
@@ -63,53 +65,82 @@ __device__ __forceinline__ void decode_tile(int tile, const GemmParams& p, int& 
   split = tile / (p.tiles_n * p.tiles_m);
 }
 
-// two adjacent output columns of one row
-__device__ __forceinline__ void store_pair(const GemmParams& p, int row, int col, int split, float x0, float x1, bool vec_c,
-                                           bool vec_aux) {
-  const bool two = col + 1 < p.N;
-  const int64_t off = static_cast<int64_t>(row) * p.ldc + col + split * p.split_stride;
-  if (p.epi == OASR_EPI_F32) {
-    float* dst = reinterpret_cast<float*>(p.C) + off;
-    if (two && vec_c) *reinterpret_cast<float2*>(dst) = make_float2(x0, x1);
-    else { dst[0] = x0; if (two) dst[1] = x1; }
-    return;
-  }
-  if (p.epi == OASR_EPI_F32_ATOMIC_ADD) {
-    float* dst = reinterpret_cast<float*>(p.C) + off;
-    atomicAdd(dst, x0);
-    if (two) atomicAdd(dst + 1, x1);
-    return;
-  }
-  uint32_t o1 = pack_bf16x2(x0, x1), o2 = 0;
-  if (p.epi == OASR_EPI_BF16_GELU) {   // h = bf16(acc + b), g = bf16(gelu(h))
-    const float2 g = gelu_erf2(unpack_bf16x2(o1));
-    o2 = pack_bf16x2(g.x, g.y);
-  } else if (p.epi == OASR_EPI_BF16_RESIDUAL || p.epi == OASR_EPI_BF16_GELU_BWD) {
-    const bf16* ap = reinterpret_cast<const bf16*>(p.aux) + static_cast<int64_t>(row) * p.ldaux + col;
-    uint32_t aw;
-    if (two && vec_aux) aw = *reinterpret_cast<const uint32_t*>(ap);
-    else aw = pack_bf16x2(__bfloat162float(ap[0]), two ? __bfloat162float(ap[1]) : 0.f);
-    const float2 a = unpack_bf16x2(aw);
-    const float2 y = unpack_bf16x2(o1);   // bf16(acc + b): the matmul output as the reference rounds it
-    if (p.epi == OASR_EPI_BF16_RESIDUAL) {   // C = bf16(aux + bf16(acc + b))
-      const float2 o = fadd2(a, y);
-      o1 = pack_bf16x2(o.x, o.y);
-    } else {                                 // C = bf16(bf16(acc) * gelu'(aux))
-      const float2 o = fmul2(y, gelu_erf_grad2(a));
-      o1 = pack_bf16x2(o.x, o.y);
-    }
-  }
-  bf16* dst = reinterpret_cast<bf16*>(p.C) + off;
-  if (two && vec_c) *reinterpret_cast<uint32_t*>(dst) = o1;
-  else { reinterpret_cast<uint16_t*>(dst)[0] = static_cast<uint16_t>(o1); if (two) reinterpret_cast<uint16_t*>(dst)[1] = static_cast<uint16_t>(o1 >> 16); }
-  if (p.epi == OASR_EPI_BF16_GELU) {
-    bf16* dst2 = reinterpret_cast<bf16*>(p.C2) + off;
-    if (two && vec_c) *reinterpret_cast<uint32_t*>(dst2) = o2;
-    else { reinterpret_cast<uint16_t*>(dst2)[0] = static_cast<uint16_t>(o2); if (two) reinterpret_cast<uint16_t*>(dst2)[1] = static_cast<uint16_t>(o2 >> 16); }
+constexpr bool is_f32_epi(int epi) { return epi == OASR_EPI_F32 || epi == OASR_EPI_F32_ATOMIC_ADD; }
+constexpr bool reads_aux(int epi) { return epi == OASR_EPI_BF16_RESIDUAL || epi == OASR_EPI_BF16_GELU_BWD; }
+
+__device__ __forceinline__ uint32_t pick4(const uint32_t (&w)[4], int i) {
+  return i == 0 ? w[0] : (i == 1 ? w[1] : (i == 2 ? w[2] : w[3]));
+}
+
+// 4 x 4 word transpose inside each quad of lanes: lane q holds w[k] = bf16 columns 8k + 2q, 8k + 2q + 1 (k = 0..3) of
+// one row; afterwards it holds v[k] = columns 8q + 2k, 8q + 2k + 1, i.e. 8 consecutive columns (one 16-byte store).
+__device__ __forceinline__ void quad_transpose(const uint32_t (&w)[4], uint32_t (&v)[4], int lane) {
+  const int q = lane & 3;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {   // round r: lane p sends its w[(p + r) % 4], lane q receives from lane (q - r) % 4
+    const int src = (q - r) & 3;
+    const uint32_t x = __shfl_sync(0xffffffffu, pick4(w, (q + r) & 3), (lane & ~3) | src);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (src == k) v[k] = x;
   }
 }
 
-template <int BN, int A_MN, int B_MN>
+// bf16 epilogues: 8 consecutive columns col .. col+7 of one row, v[k] = bf16(acc + bias) of columns col+2k, col+2k+1
+template <int EPI>
+__device__ __forceinline__ void store_bf16x8(const GemmParams& p, int row, int col, const uint32_t (&v)[4], bool vec_c,
+                                             bool vec_aux) {
+  const bool full = col + 8 <= p.N;
+  uint32_t a[4];
+  if constexpr (reads_aux(EPI)) {   // plain loads: aux may be the output itself (in-place residual)
+    const bf16* ap = reinterpret_cast<const bf16*>(p.aux) + static_cast<int64_t>(row) * p.ldaux + col;
+    if (full && vec_aux) {
+      const uint4 t = *reinterpret_cast<const uint4*>(ap);
+      a[0] = t.x; a[1] = t.y; a[2] = t.z; a[3] = t.w;
+    } else {
+      const uint16_t* ah = reinterpret_cast<const uint16_t*>(ap);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t lo = col + 2 * k < p.N ? ah[2 * k] : 0u;
+        const uint32_t hi = col + 2 * k + 1 < p.N ? ah[2 * k + 1] : 0u;
+        a[k] = lo | (hi << 16);
+      }
+    }
+  }
+  uint32_t o[4], g[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    o[k] = v[k];
+    if constexpr (EPI == OASR_EPI_BF16_GELU) {   // h = bf16(acc + b), g = bf16(gelu(h))
+      const float2 x = gelu_erf2(unpack_bf16x2(v[k]));
+      g[k] = pack_bf16x2(x.x, x.y);
+    } else if constexpr (EPI == OASR_EPI_BF16_RESIDUAL) {   // C = bf16(aux + bf16(acc + b))
+      const float2 x = fadd2(unpack_bf16x2(a[k]), unpack_bf16x2(v[k]));
+      o[k] = pack_bf16x2(x.x, x.y);
+    } else if constexpr (EPI == OASR_EPI_BF16_GELU_BWD) {   // C = bf16(bf16(acc) * gelu'(aux))
+      const float2 x = fmul2(unpack_bf16x2(v[k]), gelu_erf_grad2(unpack_bf16x2(a[k])));
+      o[k] = pack_bf16x2(x.x, x.y);
+    }
+  }
+  const int64_t off = static_cast<int64_t>(row) * p.ldc + col;
+#pragma unroll
+  for (int out = 0; out < (EPI == OASR_EPI_BF16_GELU ? 2 : 1); ++out) {
+    const uint32_t* src = out ? g : o;
+    bf16* dst = reinterpret_cast<bf16*>(out ? p.C2 : p.C) + off;
+    if (full && vec_c) {
+      *reinterpret_cast<uint4*>(dst) = make_uint4(src[0], src[1], src[2], src[3]);
+    } else {
+      uint16_t* dh = reinterpret_cast<uint16_t*>(dst);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        if (col + 2 * k < p.N) dh[2 * k] = static_cast<uint16_t>(src[k]);
+        if (col + 2 * k + 1 < p.N) dh[2 * k + 1] = static_cast<uint16_t>(src[k] >> 16);
+      }
+    }
+  }
+}
+
+template <int BN, int A_MN, int B_MN, int EPI>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   using C = Cfg<BN>;
@@ -139,6 +170,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
   if (wg == 0) {
     // ===================== TMA producer =====================
+    ptx::setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -173,6 +205,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   }
 
   // ===================== consumers =====================
+  ptx::setmaxnreg_inc<CONSUMER_REGS>();
   const int c = wg - 1;                 // row half of the tile
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31;
@@ -182,11 +215,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   constexpr uint32_t b_kstep = B_MN ? 16 * 128 : 16 * 2;
   const uint64_t a_desc0 = ptx::desc_sw128(smem_base + c * 8192, A_MN ? BK * 128 : 16, 1024);
   const uint64_t b_desc0 = ptx::desc_sw128(smem_base + A_STAGE_BYTES, B_MN ? BK * 128 : 16, 1024);
-  const bool c_is_f32 = (p.epi == OASR_EPI_F32 || p.epi == OASR_EPI_F32_ATOMIC_ADD);
-  const bool vec_c = c_is_f32 ? ((p.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 7) == 0)
-                              : ((p.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 3) == 0 &&
-                                 (p.C2 == nullptr || (reinterpret_cast<uintptr_t>(p.C2) & 3) == 0));
-  const bool vec_aux = (p.ldaux & 1) == 0 && (reinterpret_cast<uintptr_t>(p.aux) & 3) == 0;
+  const bool vec_c = is_f32_epi(EPI) ? ((p.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 7) == 0)
+                                     : ((p.ldc & 7) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 15) == 0 &&
+                                        (p.C2 == nullptr || (reinterpret_cast<uintptr_t>(p.C2) & 15) == 0));
+  const bool vec_aux = (p.ldaux & 7) == 0 && (reinterpret_cast<uintptr_t>(p.aux) & 15) == 0;
 
   int stage = 0;
   uint32_t phase = 0;
@@ -205,8 +237,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k) {
         const uint32_t accumulate = (kb > kb0 || k > 0) ? 1u : 0u;
-        if constexpr (BN == 128) ptx::wgmma_m64n128k16_ss<A_MN, B_MN>(acc, ptx::desc_add(ad, k * a_kstep), ptx::desc_add(bd, k * b_kstep), accumulate);
-        else ptx::wgmma_m64n64k16_ss<A_MN, B_MN>(acc, ptx::desc_add(ad, k * a_kstep), ptx::desc_add(bd, k * b_kstep), accumulate);
+        const uint64_t da = ptx::desc_add(ad, k * a_kstep), db = ptx::desc_add(bd, k * b_kstep);
+        if constexpr (BN == 256) ptx::wgmma_m64n256k16_ss<A_MN, B_MN>(acc, da, db, accumulate);
+        else if constexpr (BN == 128) ptx::wgmma_m64n128k16_ss<A_MN, B_MN>(acc, da, db, accumulate);
+        else ptx::wgmma_m64n64k16_ss<A_MN, B_MN>(acc, da, db, accumulate);
       }
       ptx::wgmma_commit();
       ptx::wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot may be refilled
@@ -220,22 +254,62 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
     // ---- epilogue straight from the fragments: row 16*warp + lane/4 (+8), columns 8i + 2*(lane%4) (+1)
     const int row0 = m_blk * BM + c * 64 + warp * 16 + (lane >> 2);
-    const int col0 = n_blk * BN + 2 * (lane & 3);
+    const int ncol0 = n_blk * BN;
+    if constexpr (is_f32_epi(EPI)) {
+      const int col0 = ncol0 + 2 * (lane & 3);
 #pragma unroll
-    for (int i = 0; i < BN / 8; ++i) {
-      const int col = col0 + 8 * i;
-      if (col >= p.N) continue;
-      float b0 = 0.f, b1 = 0.f;
-      if (p.bias != nullptr) {   // rounded to bf16 like bias.to(x.dtype) unless the output is fp32
-        b0 = __ldg(p.bias + col);
-        b1 = col + 1 < p.N ? __ldg(p.bias + col + 1) : 0.f;
-        if (!c_is_f32) { b0 = bf16_round(b0); b1 = bf16_round(b1); }
+      for (int i = 0; i < BN / 8; ++i) {
+        const int col = col0 + 8 * i;
+        if (col >= p.N) continue;
+        const bool two = col + 1 < p.N;
+        float b0 = 0.f, b1 = 0.f;
+        if (p.bias != nullptr) {
+          b0 = __ldg(p.bias + col);
+          b1 = two ? __ldg(p.bias + col + 1) : 0.f;
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          if (row >= p.M) continue;
+          const float x0 = __fadd_rn(acc[4 * i + 2 * h], b0), x1 = __fadd_rn(acc[4 * i + 2 * h + 1], b1);
+          float* dst = reinterpret_cast<float*>(p.C) + static_cast<int64_t>(row) * p.ldc + col + split * p.split_stride;
+          if constexpr (EPI == OASR_EPI_F32_ATOMIC_ADD) {
+            atomicAdd(dst, x0);
+            if (two) atomicAdd(dst + 1, x1);
+          } else if (two && vec_c) {
+            *reinterpret_cast<float2*>(dst) = make_float2(x0, x1);
+          } else {
+            dst[0] = x0;
+            if (two) dst[1] = x1;
+          }
+        }
       }
+    } else {
+      // bf16(acc + bf16(bias)) per column pair, then a quad transpose so that each lane stores 8 consecutive columns
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = row0 + 8 * h;
-        if (row < p.M)
-          store_pair(p, row, col, split, __fadd_rn(acc[4 * i + 2 * h], b0), __fadd_rn(acc[4 * i + 2 * h + 1], b1), vec_c, vec_aux);
+      for (int j = 0; j < BN / 32; ++j) {
+        if (ncol0 + 32 * j >= p.N) break;   // warp-uniform: the quad shuffles below need every lane
+        uint32_t w[2][4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const int i = 4 * j + k;
+          const int col = ncol0 + 8 * i + 2 * (lane & 3);
+          float b0 = 0.f, b1 = 0.f;
+          if (p.bias != nullptr) {   // rounded to bf16 like bias.to(x.dtype)
+            if (col < p.N) b0 = bf16_round(__ldg(p.bias + col));
+            if (col + 1 < p.N) b1 = bf16_round(__ldg(p.bias + col + 1));
+          }
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            w[h][k] = pack_bf16x2(__fadd_rn(acc[4 * i + 2 * h], b0), __fadd_rn(acc[4 * i + 2 * h + 1], b1));
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          uint32_t v[4];
+          quad_transpose(w[h], v, lane);
+          const int row = row0 + 8 * h;
+          if (row < p.M) store_bf16x8<EPI>(p, row, ncol0 + 32 * j + 8 * (lane & 3), v, vec_c, vec_aux);
+        }
       }
     }
   }
@@ -251,10 +325,10 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, int splits, i
   }
 }
 
-template <int BN, int A_MN, int B_MN>
+template <int BN, int A_MN, int B_MN, int EPI>
 int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
   using C = Cfg<BN>;
-  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN>;
+  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EPI>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     OASR_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
@@ -267,12 +341,36 @@ int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, 
   return OASR_OK;
 }
 
+// The (operand majors, epilogue) pairs the library calls; each is compiled for every tile width:
+//   A K-major,  B K-major  (forward Linear / Conv1d, tied logits): BF16, BF16_GELU, BF16_RESIDUAL, BF16_GELU_BWD, F32
+//   A K-major,  B MN-major (dgrad, logits dx):                     BF16, BF16_RESIDUAL, BF16_GELU_BWD, F32
+//   A MN-major, B MN-major (wgrad):                                F32, F32_ATOMIC_ADD
+// (split-K launches store fp32 partials: they run the F32 kernel).  Any other pair is rejected.
 template <int BN>
-int dispatch_major(int a_mn, int b_mn, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
-  if (!a_mn && !b_mn) return launch<BN, 0, 0>(tmA, tmB, p, st);
-  if (!a_mn && b_mn) return launch<BN, 0, 1>(tmA, tmB, p, st);
-  if (a_mn && b_mn) return launch<BN, 1, 1>(tmA, tmB, p, st);
-  return launch<BN, 1, 0>(tmA, tmB, p, st);
+int dispatch(int a_mn, int b_mn, int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
+  if (!a_mn && !b_mn) {
+    switch (epi) {
+      case OASR_EPI_BF16: return launch<BN, 0, 0, OASR_EPI_BF16>(tmA, tmB, p, st);
+      case OASR_EPI_BF16_GELU: return launch<BN, 0, 0, OASR_EPI_BF16_GELU>(tmA, tmB, p, st);
+      case OASR_EPI_BF16_RESIDUAL: return launch<BN, 0, 0, OASR_EPI_BF16_RESIDUAL>(tmA, tmB, p, st);
+      case OASR_EPI_BF16_GELU_BWD: return launch<BN, 0, 0, OASR_EPI_BF16_GELU_BWD>(tmA, tmB, p, st);
+      case OASR_EPI_F32: return launch<BN, 0, 0, OASR_EPI_F32>(tmA, tmB, p, st);
+    }
+  } else if (!a_mn && b_mn) {
+    switch (epi) {
+      case OASR_EPI_BF16: return launch<BN, 0, 1, OASR_EPI_BF16>(tmA, tmB, p, st);
+      case OASR_EPI_BF16_RESIDUAL: return launch<BN, 0, 1, OASR_EPI_BF16_RESIDUAL>(tmA, tmB, p, st);
+      case OASR_EPI_BF16_GELU_BWD: return launch<BN, 0, 1, OASR_EPI_BF16_GELU_BWD>(tmA, tmB, p, st);
+      case OASR_EPI_F32: return launch<BN, 0, 1, OASR_EPI_F32>(tmA, tmB, p, st);
+    }
+  } else if (a_mn && b_mn) {
+    switch (epi) {
+      case OASR_EPI_F32: return launch<BN, 1, 1, OASR_EPI_F32>(tmA, tmB, p, st);
+      case OASR_EPI_F32_ATOMIC_ADD: return launch<BN, 1, 1, OASR_EPI_F32_ATOMIC_ADD>(tmA, tmB, p, st);
+    }
+  }
+  set_last_error("gemm: no kernel for a_layout=%d b_layout=%d epilogue=%d", a_mn, b_mn, epi);
+  return OASR_ERR_UNSUPPORTED;
 }
 
 }  // namespace
@@ -297,11 +395,8 @@ extern "C" int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const vo
     OASR_REQUIRE(aux != nullptr, "gemm: epilogue %d needs aux", epilogue);
   if (split_k < 1) split_k = 1;
   OASR_REQUIRE(split_k == 1 || epilogue == OASR_EPI_F32_ATOMIC_ADD, "gemm: split_k needs the accumulating fp32 epilogue");
-  if (block_n == 0) block_n = (N > 64) ? 128 : 64;
+  if (block_n == 0) block_n = (N > 128) ? 256 : (N > 64 ? 128 : 64);
   OASR_REQUIRE(block_n == 64 || block_n == 128 || block_n == 256, "gemm: block_n must be 64/128/256");
-  // 128 is the widest tile on sm_90a: two consumer warpgroups of 64 x 128 fp32 accumulators each; a 256-wide request
-  // is served by 128-wide tiles (same result, the registers of a 64 x 256 accumulator would spill)
-  if (block_n == 256) block_n = 128;
 
   GemmParams p;
   p.C = Cout; p.C2 = C2; p.bias = bias; p.aux = aux; p.ldc = ldc; p.ldaux = ldaux;
@@ -312,7 +407,6 @@ extern "C" int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const vo
   if (split_k > p.kblocks_total) split_k = p.kblocks_total;
   p.kblocks_per_split = (int)ceil_div(p.kblocks_total, split_k);
   p.splits = (int)ceil_div(p.kblocks_total, p.kblocks_per_split);
-  p.epi = epilogue;
   p.raster_m = (N > M) ? 1 : 0;
   p.split_stride = 0;
 
@@ -334,9 +428,11 @@ extern "C" int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const vo
   if (p.splits > 1) {   // every split stores its partial product; one more launch adds them to C in split order
     ws = static_cast<float*>(scratch_alloc(sizeof(float) * p.splits * M * N, st));
     if (!ws) return OASR_ERR_CUDA;
-    p.C = ws; p.ldc = N; p.epi = OASR_EPI_F32; p.split_stride = M * N;
+    p.C = ws; p.ldc = N; epilogue = OASR_EPI_F32; p.split_stride = M * N;
   }
-  rc = (block_n == 128) ? dispatch_major<128>(a_layout, b_layout, tmA, tmB, p, st) : dispatch_major<64>(a_layout, b_layout, tmA, tmB, p, st);
+  rc = block_n == 256 ? dispatch<256>(a_layout, b_layout, epilogue, tmA, tmB, p, st)
+     : block_n == 128 ? dispatch<128>(a_layout, b_layout, epilogue, tmA, tmB, p, st)
+                      : dispatch<64>(a_layout, b_layout, epilogue, tmA, tmB, p, st);
   if (ws) {
     if (rc == OASR_OK) {
       int64_t blocks = ceil_div(M * N, 256);
