@@ -226,6 +226,9 @@ typedef struct oasr_dec_attn_args {
   int32_t n_seq; int32_t n_head; int32_t n_splits; float scale; int32_t dtype;
 } oasr_dec_attn_args;
 OASR_API int oasr_dec_attention(const oasr_dec_attn_args* args, void* stream);
+/* Same as oasr_dec_attention, but sequence n reads K / V entry n / kv_group (beams of one clip share its cross K / V).
+ * oasr_dec_attention is the kv_group = 1 case: the same launches and the same bits. */
+OASR_API int oasr_dec_attention_grouped(const oasr_dec_attn_args* args, int kv_group, void* stream);
 
 /* Logit filters + greedy choice + bookkeeping (whisper/decoding.py SuppressBlank, SuppressTokens, GreedyDecoder.update,
  * the no-speech probability and the stop test of DecodingTask._main_loop), then *pos += 1.
@@ -241,6 +244,33 @@ typedef struct oasr_dec_sample_args {
   int32_t eot; int32_t no_speech; int32_t n_slices; int32_t reserved;
 } oasr_dec_sample_args;
 OASR_API int oasr_dec_sample(const oasr_dec_sample_args* args, void* stream);
+
+/* Beam search step (whisper/decoding.py BeamSearchDecoder.update with SuppressBlank, SuppressTokens and, when
+ * `timestamps`, ApplyTimestampRules) over n_clips x beam rows (row = clip * beam + j), after the logits head.
+ *   oasr_dec_beam_candidates: per row the top beam + 1 log-probs after every filter -> scratch
+ *                              (n_clips * beam, n_slices, 48) f32; also the raw statistics for the no-speech probability.
+ *   oasr_dec_beam_select:     one CTA per clip ranks the candidates, rewrites the clip's token rows (source prefix + new
+ *                              token at *pos + 1), sum_logprobs and src_rows, appends eot candidates to the finished list
+ *                              (fin_tokens (n_clips, max_candidates, ld_fin) int32 of length fin_len, fin_scores,
+ *                              fin_count) while it has room, writes seq_len = *pos + 2; then *pos += 1 and
+ *                              done_flag = every clip's list is full.  With done_flag already set nothing changes.
+ *   oasr_dec_beam_reorder:    self-attention K / V rows [0, *pos) of every layer: row r <- row src_rows[r] (in place;
+ *                              rows whose source is themselves are skipped).  Caches (n_layers, rows, cache_len, d).
+ * max_initial_timestamp < 0: no initial-timestamp limit.  1 <= beam <= 8, max_candidates <= 32. */
+typedef struct oasr_dec_beam_args {
+  const float* logits; int64_t ld_logits; int32_t* tokens; int64_t ld_tokens; int32_t* pos_ptr;
+  const uint8_t* suppress; float* sum_logprobs; float* no_speech_prob; int32_t* n_unfinished; int32_t* done_flag;
+  float* scratch; int32_t* src_rows;
+  int32_t* fin_tokens; int64_t ld_fin; float* fin_scores; int32_t* fin_len; int32_t* fin_count; int32_t* seq_len;
+  int32_t n_clips; int32_t beam; int32_t max_candidates; int32_t n_vocab; int32_t n_slices; int32_t n_ctx;
+  int32_t sample_begin; int32_t sot_index; int32_t suppress_blank; int32_t blank; int32_t eot; int32_t no_speech;
+  int32_t timestamps; int32_t timestamp_begin; int32_t no_timestamps; int32_t max_initial_timestamp;
+} oasr_dec_beam_args;
+OASR_API int oasr_dec_beam_candidates(const oasr_dec_beam_args* args, void* stream);
+OASR_API int oasr_dec_beam_select(const oasr_dec_beam_args* args, void* stream);
+OASR_API int oasr_dec_beam_reorder(void* k_cache, void* v_cache, int64_t layer_stride, int64_t row_stride, int64_t n_layers,
+                                   const int32_t* src_rows, const int32_t* pos_ptr, int32_t n_clips, int32_t beam, int32_t d,
+                                   int32_t n_pos_blocks, int dtype, void* stream);
 
 /* elementwise dtype conversion (weights fp32 -> T once per engine; bf16 encoder output / cross K,V -> fp16) */
 OASR_API int oasr_convert(const void* src, int src_dtype, void* dst, int dst_dtype, int64_t n, void* stream);

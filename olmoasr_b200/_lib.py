@@ -57,6 +57,18 @@ class DecSampleArgs(ctypes.Structure):  # oasr_dec_sample_args
                 ("blank", c_i32), ("eot", c_i32), ("no_speech", c_i32), ("n_slices", c_i32), ("reserved", c_i32)]
 
 
+class DecBeamArgs(ctypes.Structure):  # oasr_dec_beam_args
+    _fields_ = [("logits", c_void_p), ("ld_logits", c_i64), ("tokens", c_void_p), ("ld_tokens", c_i64), ("pos_ptr", c_void_p),
+                ("suppress", c_void_p), ("sum_logprobs", c_void_p), ("no_speech_prob", c_void_p), ("n_unfinished", c_void_p),
+                ("done_flag", c_void_p), ("scratch", c_void_p), ("src_rows", c_void_p),
+                ("fin_tokens", c_void_p), ("ld_fin", c_i64), ("fin_scores", c_void_p), ("fin_len", c_void_p),
+                ("fin_count", c_void_p), ("seq_len", c_void_p),
+                ("n_clips", c_i32), ("beam", c_i32), ("max_candidates", c_i32), ("n_vocab", c_i32), ("n_slices", c_i32),
+                ("n_ctx", c_i32), ("sample_begin", c_i32), ("sot_index", c_i32), ("suppress_blank", c_i32), ("blank", c_i32),
+                ("eot", c_i32), ("no_speech", c_i32), ("timestamps", c_i32), ("timestamp_begin", c_i32),
+                ("no_timestamps", c_i32), ("max_initial_timestamp", c_i32)]
+
+
 # name -> argtypes (restype is always int unless listed in _RESTYPES)
 _SIGNATURES = {
     "oasr_abi_version": [],
@@ -99,6 +111,11 @@ _SIGNATURES = {
     "oasr_dec_linear": [ctypes.POINTER(DecLinearArgs), c_void_p],
     "oasr_dec_attention": [ctypes.POINTER(DecAttnArgs), c_void_p],
     "oasr_dec_sample": [ctypes.POINTER(DecSampleArgs), c_void_p],
+    "oasr_dec_attention_grouped": [ctypes.POINTER(DecAttnArgs), c_int, c_void_p],
+    "oasr_dec_beam_candidates": [ctypes.POINTER(DecBeamArgs), c_void_p],
+    "oasr_dec_beam_select": [ctypes.POINTER(DecBeamArgs), c_void_p],
+    "oasr_dec_beam_reorder": [c_void_p, c_void_p, c_i64, c_i64, c_i64, c_void_p, c_void_p, c_i32, c_i32, c_i32, c_i32, c_int,
+                              c_void_p],
     "oasr_convert": [c_void_p, c_int, c_void_p, c_int, c_i64, c_void_p],
     "oasr_gemm_bf16": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_void_p, c_i64, c_void_p, c_void_p,
                        c_void_p, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_void_p],
@@ -162,6 +179,7 @@ def stream():
 
 # kernels launched per entry point (memsets not counted) -- bench.py reports the total as `gpu_launches`
 _LAUNCHES_PER_CALL = {"oasr_logmel": 3, "oasr_attention_bwd": 3, "oasr_dec_attention": 2, "oasr_dec_sample": 2,
+                      "oasr_dec_attention_grouped": 2, "oasr_dec_beam_select": 2,
                       "oasr_ce_fwd": 2, "oasr_colsum_bf16": 2, "oasr_layernorm_bwd": 3, "oasr_grad_sqnorm": 2,
                       "oasr_grad_sqnorm_flat": 2}
 LAUNCH_COUNT = 0

@@ -24,6 +24,7 @@
 #include "common.cuh"
 
 #include <cuda_fp16.h>
+#include <limits.h>
 #include <stdlib.h>
 
 namespace oasr {
@@ -528,7 +529,7 @@ __global__ void __launch_bounds__(256, (MT <= 2 ? 2 : 1)) dec_linear_kernel(cons
 // scores[n, h, j] = float(round_T( sum_c round_T(q[c] * hd^-.25) * round_T(k_j[c] * hd^-.25) ))    (inf_model.py:176-181)
 // grid (splits, H, N), 128 threads: 8 lanes per key row (16 bytes = 8 dims each), 16 keys per pass.
 template <typename T>
-__global__ void __launch_bounds__(128) dec_attn_scores_kernel(const oasr_dec_attn_args a) {
+__global__ void __launch_bounds__(128) dec_attn_scores_kernel(const oasr_dec_attn_args a, const int kv_group) {
   pdl_launch_dependents();
   pdl_wait();
   const int s = blockIdx.x, h = blockIdx.y, n = blockIdx.z;
@@ -547,7 +548,7 @@ __global__ void __launch_bounds__(128) dec_attn_scores_kernel(const oasr_dec_att
       qs[2 * i] = rnd<T>(p.x * scale); qs[2 * i + 1] = rnd<T>(p.y * scale);
     }
   }
-  const T* kb = static_cast<const T*>(a.k) + static_cast<int64_t>(n) * a.kv_seq_stride + h * 64 + c8 * 8;
+  const T* kb = static_cast<const T*>(a.k) + static_cast<int64_t>(n / kv_group) * a.kv_seq_stride + h * 64 + c8 * 8;
   float* out = a.scores + (static_cast<int64_t>(n) * gridDim.y + h) * a.scores_ld;
   for (int jb = j0; jb < j1; jb += 128) {   // 8 independent 16-byte loads in flight per thread
     uint4 u[8];
@@ -579,7 +580,7 @@ __global__ void __launch_bounds__(128) dec_attn_scores_kernel(const oasr_dec_att
 // splits in order and rounds once = the single rounding of `w @ v`).  Every CTA first derives the row maximum and the
 // normaliser from ALL scores of its (n, h) (<= 1500 floats, L2-resident), as F.softmax(qk.float()) does.
 template <typename T>
-__global__ void __launch_bounds__(128) dec_attn_pv_kernel(const oasr_dec_attn_args a) {
+__global__ void __launch_bounds__(128) dec_attn_pv_kernel(const oasr_dec_attn_args a, const int kv_group) {
   __shared__ float s_part[4];
   __shared__ float s_o[4][64];
   pdl_launch_dependents();
@@ -606,7 +607,7 @@ __global__ void __launch_bounds__(128) dec_attn_pv_kernel(const oasr_dec_attn_ar
   const float inv_l = 1.0f / l;
 
   const int c8 = threadIdx.x & 7, slot = threadIdx.x >> 3;
-  const T* vb = static_cast<const T*>(a.v) + static_cast<int64_t>(n) * a.kv_seq_stride + h * 64 + c8 * 8;
+  const T* vb = static_cast<const T*>(a.v) + static_cast<int64_t>(n / kv_group) * a.kv_seq_stride + h * 64 + c8 * 8;
   float o[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   for (int jb = j0; jb < j1; jb += 128) {
     uint4 u[8];
@@ -651,7 +652,7 @@ __global__ void __launch_bounds__(128) dec_attn_pv_kernel(const oasr_dec_attn_ar
 // machine): scores stay in shared memory, softmax and P V follow in the same kernel -- one launch and no round trip through
 // global memory instead of two.  Same arithmetic and rounding points as the two-kernel form above.
 template <typename T>
-__global__ void __launch_bounds__(128) dec_attn_fused_kernel(const oasr_dec_attn_args a) {
+__global__ void __launch_bounds__(128) dec_attn_fused_kernel(const oasr_dec_attn_args a, const int kv_group) {
   __shared__ float s_sc[1536];
   __shared__ float s_part[4];
   __shared__ float s_o[4][64];
@@ -672,8 +673,8 @@ __global__ void __launch_bounds__(128) dec_attn_fused_kernel(const oasr_dec_attn
       qs[2 * i] = rnd<T>(p.x * scale); qs[2 * i + 1] = rnd<T>(p.y * scale);
     }
   }
-  const T* kb = static_cast<const T*>(a.k) + static_cast<int64_t>(n) * a.kv_seq_stride + h * 64 + c8 * 8;
-  const T* vb = static_cast<const T*>(a.v) + static_cast<int64_t>(n) * a.kv_seq_stride + h * 64 + c8 * 8;
+  const T* kb = static_cast<const T*>(a.k) + static_cast<int64_t>(n / kv_group) * a.kv_seq_stride + h * 64 + c8 * 8;
+  const T* vb = static_cast<const T*>(a.v) + static_cast<int64_t>(n / kv_group) * a.kv_seq_stride + h * 64 + c8 * 8;
   float m = -INFINITY;
   for (int jb = 0; jb < nkeys; jb += 128) {
     uint4 u[8];
@@ -871,6 +872,373 @@ __global__ void dec_advance_kernel(int32_t* pos_ptr, int32_t* n_unfinished, int3
   *pos_ptr = pos + 1;
 }
 
+// ---------------------------------------------------------------------------------------------------------- beam search
+// whisper/decoding.py BeamSearchDecoder.update on the device.  Three kernels per step after the logits head:
+//   * dec_beam_cand: `n_slices` blocks per row, one pass over the fp32 logits applying every filter as an index test
+//     (SuppressTokens, SuppressBlank, ApplyTimestampRules).  Each slice keeps the online (max, sum exp) and the top
+//     beam + 1 entries separately for the text region [0, timestamp_begin) and the timestamp region, plus the raw
+//     (max, sum exp) for the no-speech probability.  Banned ids enter the top-k lists as -inf (topk includes them).
+//   * dec_beam_select: one CTA per clip.  Merges the slices in slice order, applies "timestamp mass beats every text
+//     token" (lse(ts) > max(text): both sides share one normaliser), ranks the clip's candidates, fills the finished
+//     list and rewrites the clip's token rows, log-prob sums and source rows.  Once every clip's list is full (done flag
+//     set by the previous step) it leaves all state untouched, so extra replays before the host looks are harmless.
+//   * dec_beam_reorder: self-attention K / V rows [0, pos) of every layer gathered from the source beams, in place.
+// Ordering: candidates by (value desc, token id asc); across a clip by (score desc, beam, rank) -- Python's stable sort
+// over dict insertion order.  No float atomics: the result is the same on every run.
+constexpr int BEAM_MAX = 8;
+constexpr int BEAM_K = BEAM_MAX + 1;        // candidates per row: beam + 1
+constexpr int BEAM_SCR = 48;                // floats of scratch per (row, slice)
+constexpr int BEAM_TOK_MAX = 456;           // staged token row length (n_text_ctx + 2 <= this)
+
+__device__ __forceinline__ bool cand_better(float x, int i, float y, int j) { return x > y || (x == y && i < j); }
+
+struct TopK {
+  float v[BEAM_K];
+  int i[BEAM_K];
+  __device__ __forceinline__ void init() {
+#pragma unroll
+    for (int k = 0; k < BEAM_K; ++k) { v[k] = -INFINITY; i[k] = INT_MAX; }
+  }
+  __device__ __forceinline__ void push(float x, int id) {     // sorted insert, registers only (compile-time indices)
+    if (!cand_better(x, id, v[BEAM_K - 1], i[BEAM_K - 1])) return;
+#pragma unroll
+    for (int k = 0; k < BEAM_K; ++k) {
+      if (cand_better(x, id, v[k], i[k])) {
+        const float tv = v[k]; const int ti = i[k];
+        v[k] = x; i[k] = id; x = tv; id = ti;
+      }
+    }
+  }
+  __device__ __forceinline__ void pop() {
+#pragma unroll
+    for (int k = 0; k + 1 < BEAM_K; ++k) { v[k] = v[k + 1]; i[k] = i[k + 1]; }
+    v[BEAM_K - 1] = -INFINITY; i[BEAM_K - 1] = INT_MAX;
+  }
+};
+
+struct Lse {   // online (max, sum exp(x - max)); -inf entries add nothing
+  float m, s;
+  __device__ __forceinline__ void push(float x) {
+    if (x == -INFINITY) return;
+    if (x > m) { s = s * expf(m - x) + 1.f; m = x; }
+    else s += expf(x - m);
+  }
+  __device__ __forceinline__ void merge(float bm, float bs) {
+    const float r = fmaxf(m, bm);
+    s = (r == -INFINITY) ? 0.f : s * expf(m - r) + bs * expf(bm - r);
+    m = r;
+  }
+  __device__ __forceinline__ float lse() const { return m == -INFINITY ? -INFINITY : m + logf(s); }
+};
+
+// Per-row logit filter of one step (every rule an index test).
+struct BeamFilter {
+  const uint8_t* suppress;
+  int first, blank_eot, eot, blank;
+  int ts_on, no_ts, ts_begin;
+  int ban_text, ban_below_eot;     // ban [0, ts_begin) / ban [0, eot)
+  int ts_lo, ts_hi;                // allowed timestamps: [ts_lo, ts_hi)
+  __device__ __forceinline__ bool banned(int v) const {
+    if (suppress[v]) return true;
+    if (blank_eot && (v == blank || v == eot)) return true;
+    if (!ts_on) return false;
+    if (v == no_ts) return true;
+    if (v < ts_begin) return ban_text || (ban_below_eot && v < eot);
+    return v < ts_lo || v >= ts_hi;
+  }
+};
+
+__device__ BeamFilter beam_filter(const oasr_dec_beam_args& a, const int32_t* trow, int pos, int* s_red) {
+  BeamFilter f;
+  f.suppress = a.suppress;
+  f.first = pos == a.sample_begin - 1;
+  f.blank_eot = f.first && a.suppress_blank;
+  f.eot = a.eot; f.blank = a.blank;
+  f.ts_on = a.timestamps; f.no_ts = a.no_timestamps; f.ts_begin = a.timestamp_begin;
+  f.ban_text = 0; f.ban_below_eot = 0; f.ts_lo = a.timestamp_begin; f.ts_hi = a.n_vocab;
+  if (!a.timestamps) return f;
+  // ApplyTimestampRules over seq = tokens[sample_begin .. pos]: the last timestamp (block max over positions)
+  int last = -1;
+  for (int p = a.sample_begin + threadIdx.x; p <= pos; p += blockDim.x)
+    if (trow[p] >= a.timestamp_begin) last = p;
+  last = __reduce_max_sync(0xffffffffu, last);
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = last;
+  __syncthreads();
+  last = -1;
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) last = max(last, s_red[w]);
+  __syncthreads();
+  const int len = pos + 1 - a.sample_begin;
+  const bool last_ts = len >= 1 && trow[pos] >= a.timestamp_begin;
+  const bool penult_ts = len < 2 || trow[pos - 1] >= a.timestamp_begin;
+  if (last_ts) {
+    if (penult_ts) f.ts_lo = a.n_vocab;        // a timestamp pair is closed: text must follow
+    else f.ban_below_eot = 1;                  // an open timestamp: another timestamp or eot
+  }
+  if (last >= 0) {                             // timestamps never decrease (strictly increase after a closed pair)
+    const int t = trow[last];
+    f.ts_lo = max(f.ts_lo, (last_ts && !penult_ts) ? t : t + 1);
+  }
+  if (len == 0) {                              // the first sampled token is a timestamp, within the initial window
+    f.ban_text = 1;
+    if (a.max_initial_timestamp >= 0) f.ts_hi = min(f.ts_hi, a.timestamp_begin + a.max_initial_timestamp + 1);
+  }
+  return f;
+}
+
+__global__ void __launch_bounds__(256) dec_beam_cand_kernel(const oasr_dec_beam_args a) {
+  __shared__ int s_red[8];
+  __shared__ float s_f[8][2];
+  __shared__ int s_i[8];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int slice = blockIdx.x, n = blockIdx.y, S = gridDim.x;
+  const int pos = *a.pos_ptr;
+  const bool sampling = pos >= a.sample_begin - 1 && *a.done_flag == 0;
+  const bool want_raw = pos == a.sot_index;
+  if (!sampling && !want_raw) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const float* row = a.logits + static_cast<int64_t>(n) * a.ld_logits;
+  const int32_t* trow = a.tokens + static_cast<int64_t>(n) * a.ld_tokens;
+  const int V = a.n_vocab, K = a.beam + 1;
+  const BeamFilter f = beam_filter(a, trow, pos, s_red);
+  const int per = ((V + S - 1) / S + 3) & ~3;
+  const int v0 = slice * per, v1 = min(V, v0 + per);
+  Lse raw{-INFINITY, 0.f}, lt{-INFINITY, 0.f}, ls{-INFINITY, 0.f};
+  TopK tt, ts;
+  tt.init(); ts.init();
+  auto visit = [&](float x, int v) {
+    if (want_raw) raw.push(x);
+    if (!sampling) return;
+    const bool ban = f.banned(v);
+    const float y = ban ? -INFINITY : x;
+    if (v < f.ts_begin) { if (!ban) lt.push(y); tt.push(y, v); }
+    else { if (!ban) ls.push(y); ts.push(y, v); }
+  };
+  for (int v = v0 + threadIdx.x * 4; v < v1; v += 256 * 4) {
+    if (v + 4 <= v1) {
+      const float4 x = *reinterpret_cast<const float4*>(row + v);
+      visit(x.x, v); visit(x.y, v + 1); visit(x.z, v + 2); visit(x.w, v + 3);
+    } else {
+      for (int u = v; u < v1; ++u) visit(row[u], u);
+    }
+  }
+  float* out = a.scratch + (static_cast<int64_t>(n) * S + slice) * BEAM_SCR;
+  // (max, sum exp) of the three accumulators: warps, then warp 0 in warp order
+  Lse* accs[3] = {&lt, &ls, &raw};
+  for (int q = 0; q < 3; ++q) {
+    Lse& l = *accs[q];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float bm = __shfl_xor_sync(0xffffffffu, l.m, o), bs = __shfl_xor_sync(0xffffffffu, l.s, o);
+      l.merge(bm, bs);
+    }
+    if (lane == 0) { s_f[warp][0] = l.m; s_f[warp][1] = l.s; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      Lse t{-INFINITY, 0.f};
+      for (int w = 0; w < 8; ++w) t.merge(s_f[w][0], s_f[w][1]);
+      out[2 * q] = t.m; out[2 * q + 1] = t.s;
+    }
+    __syncthreads();
+  }
+  if (!sampling) return;
+  // top-K of the block per region: K rounds of a block-wide best over the threads' list heads
+  TopK* lists[2] = {&tt, &ts};
+  for (int q = 0; q < 2; ++q) {
+    TopK& t = *lists[q];
+    for (int r = 0; r < K; ++r) {
+      float bv = t.v[0];
+      int bi = t.i[0];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (cand_better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+      }
+      if (lane == 0) { s_f[warp][0] = bv; s_i[warp] = bi; }
+      __syncthreads();
+      bv = s_f[0][0]; bi = s_i[0];
+      for (int w = 1; w < 8; ++w)
+        if (cand_better(s_f[w][0], s_i[w], bv, bi)) { bv = s_f[w][0]; bi = s_i[w]; }
+      if (t.i[0] == bi) t.pop();                 // ids are unique (sentinels carry INT_MAX and are never consumed)
+      if (threadIdx.x == 0) { out[6 + q * 2 * BEAM_K + r] = bv; out[6 + q * 2 * BEAM_K + BEAM_K + r] = __int_as_float(bi); }
+      __syncthreads();
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) dec_beam_select_kernel(const oasr_dec_beam_args a) {
+  __shared__ float s_val[BEAM_MAX][2][BEAM_K];
+  __shared__ int s_id[BEAM_MAX][2][BEAM_K];
+  __shared__ float s_m[BEAM_MAX][2], s_l[BEAM_MAX][2];
+  __shared__ float c_lp[BEAM_MAX * BEAM_K];
+  __shared__ int c_tok[BEAM_MAX * BEAM_K];
+  __shared__ float c_score[BEAM_MAX * BEAM_K];
+  __shared__ int c_order[BEAM_MAX * BEAM_K];
+  __shared__ int s_tok[BEAM_MAX][BEAM_TOK_MAX];
+  __shared__ int k_src[BEAM_MAX], k_tok[BEAM_MAX];
+  __shared__ int f_slot[BEAM_MAX], f_src[BEAM_MAX];
+  __shared__ int s_nfin;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int c = blockIdx.x, B = a.beam, K = B + 1, S = a.n_slices;
+  const int row0 = c * B;
+  const int pos = *a.pos_ptr;
+  const bool sampling = pos >= a.sample_begin - 1 && *a.done_flag == 0;
+  const bool first = pos == a.sample_begin - 1;
+  const bool want_raw = pos == a.sot_index;
+  const int tid = threadIdx.x;
+  // 1. merge the slices of every (row, region) in slice order; the raw statistics give the no-speech probability
+  if (tid < 2 * B) {
+    const int j = tid >> 1, q = tid & 1, n = row0 + j;
+    const float* in = a.scratch + static_cast<int64_t>(n) * S * BEAM_SCR;
+    if (q == 0 && want_raw) {
+      Lse r{-INFINITY, 0.f};
+      for (int s = 0; s < S; ++s) r.merge(in[s * BEAM_SCR + 4], in[s * BEAM_SCR + 5]);
+      a.no_speech_prob[n] = expf(a.logits[static_cast<int64_t>(n) * a.ld_logits + a.no_speech] - r.m) / r.s;
+    }
+    if (sampling) {
+      Lse l{-INFINITY, 0.f};
+      TopK t;
+      t.init();
+      for (int s = 0; s < S; ++s) {
+        const float* p = in + s * BEAM_SCR;
+        l.merge(p[2 * q], p[2 * q + 1]);
+        for (int r = 0; r < K; ++r) t.push(p[6 + q * 2 * BEAM_K + r], __float_as_int(p[6 + q * 2 * BEAM_K + BEAM_K + r]));
+      }
+      s_m[j][q] = l.m;
+      s_l[j][q] = l.lse();
+#pragma unroll
+      for (int r = 0; r < BEAM_K; ++r) { s_val[j][q][r] = t.v[r]; s_id[j][q][r] = t.i[r]; }
+    }
+  }
+  __syncthreads();
+  if (!sampling) {                           // teacher-forced step or frozen state: identity sources, nothing else
+    if (tid < B) a.src_rows[row0 + tid] = row0 + tid;
+    return;
+  }
+  // 2. per row: "timestamp mass beats every text token" bans text (then every text id is -inf, lowest ids first);
+  //    the row's normaliser and its top K candidates (log-probs)
+  if (tid < B) {
+    const int j = tid;
+    const bool ban_text = a.timestamps && s_l[j][1] > s_m[j][0];
+    const float lse = ban_text ? s_l[j][1]
+                               : (fmaxf(s_l[j][0], s_l[j][1]) == -INFINITY ? -INFINITY
+                                  : fmaxf(s_l[j][0], s_l[j][1]) + log1pf(expf(fminf(s_l[j][0], s_l[j][1]) - fmaxf(s_l[j][0], s_l[j][1]))));
+    int it = 0, is = 0;
+    for (int r = 0; r < K; ++r) {
+      const float vt = ban_text ? -INFINITY : s_val[j][0][it];
+      const int idt = ban_text ? it : s_id[j][0][it];
+      const float vs = s_val[j][1][is];
+      const int ids = s_id[j][1][is];
+      float v; int id;
+      if (cand_better(vt, idt, vs, ids)) { v = vt; id = idt; ++it; } else { v = vs; id = ids; ++is; }
+      c_lp[j * K + r] = v - lse;
+      c_tok[j * K + r] = id;
+    }
+  }
+  __syncthreads();
+  // 3. scores and their rank: (score desc, candidate index asc); at the first sampled step every beam holds the same
+  //    prefix, so only beam 0's candidates exist (upstream's dict keyed by sequence collapses them)
+  const int n_cand = first ? K : B * K;
+  if (tid < n_cand) c_score[tid] = a.sum_logprobs[row0 + tid / K] + c_lp[tid];
+  for (int idx = tid; idx < B * (pos + 1); idx += blockDim.x) {
+    const int j = idx / (pos + 1), p = idx - j * (pos + 1);
+    s_tok[j][p] = a.tokens[static_cast<int64_t>(row0 + j) * a.ld_tokens + p];
+  }
+  __syncthreads();
+  if (tid < n_cand) {
+    const float me = c_score[tid];
+    int rank = 0;
+    for (int u = 0; u < n_cand; ++u) rank += (c_score[u] > me || (c_score[u] == me && u < tid)) ? 1 : 0;
+    c_order[rank] = tid;
+  }
+  __syncthreads();
+  // 4. the walk: eot -> finished (while the list has room), anything else -> the next beam, until `beam` are kept
+  if (tid == 0) {
+    int kept = 0, nf = 0, count = a.fin_count[c];
+    float sums[BEAM_MAX];
+    for (int i = 0; i < n_cand && kept < B; ++i) {
+      const int t = c_order[i];
+      const int tok = c_tok[t];
+      if (tok == a.eot) {
+        if (count < a.max_candidates) {
+          const int slot = count++;
+          a.fin_scores[c * a.max_candidates + slot] = c_score[t];
+          a.fin_len[c * a.max_candidates + slot] = pos + 2;
+          f_slot[nf] = slot; f_src[nf] = t / K; ++nf;
+        }
+      } else {
+        k_src[kept] = t / K; k_tok[kept] = tok; sums[kept] = c_score[t]; ++kept;
+      }
+    }
+    for (int k = 0; k < B; ++k) a.sum_logprobs[row0 + k] = sums[k];
+    a.fin_count[c] = count;
+    s_nfin = nf;
+    if (count < a.max_candidates) atomicAdd(a.n_unfinished, 1);
+    if (c == 0) *a.seq_len = pos + 2;
+  }
+  __syncthreads();
+  // 5. new token rows (prefix of the source beam + the new token), source rows, finished sequences
+  const int L = pos + 2;
+  for (int idx = tid; idx < B * L; idx += blockDim.x) {
+    const int k = idx / L, p = idx - k * L;
+    a.tokens[static_cast<int64_t>(row0 + k) * a.ld_tokens + p] = (p <= pos) ? s_tok[k_src[k]][p] : k_tok[k];
+  }
+  for (int idx = tid; idx < s_nfin * L; idx += blockDim.x) {
+    const int f = idx / L, p = idx - f * L;
+    a.fin_tokens[(static_cast<int64_t>(c) * a.max_candidates + f_slot[f]) * a.ld_fin + p] = (p <= pos) ? s_tok[f_src[f]][p] : a.eot;
+  }
+  if (tid < B) a.src_rows[row0 + tid] = row0 + k_src[tid];
+}
+
+// K / V rows [0, *pos) of every layer: row r <- row src[r] (rows of one clip, in place).  One CTA iteration owns one
+// (layer, K or V, clip, position) tile of all the clip's beams: every source element is in registers before the
+// barrier and written after it, so cycles and forks are safe.  Rows whose source is themselves are not touched.
+constexpr int REORDER_ITEMS = 5;     // 16-byte items per thread: beam 8 x d 1280 / 8 / 256 threads
+__global__ void __launch_bounds__(256) dec_beam_reorder_kernel(uint16_t* k_cache, uint16_t* v_cache, int64_t layer_stride,
+                                                               int64_t row_stride, const int32_t* src, const int32_t* pos_ptr,
+                                                               int beam, int d) {
+  __shared__ int s_src[BEAM_MAX];
+  __shared__ int s_any;
+  pdl_launch_dependents();
+  pdl_wait();
+  const int c = blockIdx.z, layer = blockIdx.y >> 1;
+  uint16_t* base = ((blockIdx.y & 1) ? v_cache : k_cache) + static_cast<int64_t>(layer) * layer_stride;
+  if (threadIdx.x == 0) s_any = 0;
+  __syncthreads();
+  if (threadIdx.x < beam) {
+    s_src[threadIdx.x] = src[c * beam + threadIdx.x];
+    if (s_src[threadIdx.x] != c * beam + static_cast<int>(threadIdx.x)) s_any = 1;
+  }
+  __syncthreads();
+  if (!s_any) return;
+  const int npos = *pos_ptr;
+  const int vec = d >> 3, items = beam * vec;
+  for (int p = blockIdx.x; p < npos; p += gridDim.x) {
+    uint4 buf[REORDER_ITEMS];
+#pragma unroll
+    for (int q = 0; q < REORDER_ITEMS; ++q) {
+      const int idx = threadIdx.x + 256 * q;
+      if (idx < items) {
+        const int j = idx / vec, v = idx - j * vec;
+        const int s = s_src[j];
+        if (s != c * beam + j) buf[q] = *reinterpret_cast<const uint4*>(base + s * row_stride + static_cast<int64_t>(p) * d + v * 8);
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int q = 0; q < REORDER_ITEMS; ++q) {
+      const int idx = threadIdx.x + 256 * q;
+      if (idx < items) {
+        const int j = idx / vec, v = idx - j * vec;
+        const int r = c * beam + j;
+        if (s_src[j] != r) *reinterpret_cast<uint4*>(base + r * row_stride + static_cast<int64_t>(p) * d + v * 8) = buf[q];
+      }
+    }
+  }
+}
+
 template <typename TI, typename TO>
 __global__ void convert_kernel(const TI* __restrict__ src, TO* __restrict__ dst, int64_t n) {
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<int64_t>(gridDim.x) * blockDim.x)
@@ -983,28 +1351,36 @@ extern "C" int oasr_dec_linear(const oasr_dec_linear_args* a, void* stream) {
   OASR_REQUIRE(false, "dec_linear: unknown dtype %d", a->dtype);
 }
 
-extern "C" int oasr_dec_attention(const oasr_dec_attn_args* a, void* stream) {
+namespace {
+int dec_attention(const oasr_dec_attn_args* a, int kv_group, cudaStream_t st) {
   OASR_REQUIRE(a != nullptr && a->q && a->k && a->v && a->scores && a->out_partial, "dec_attention: null tensor");
   OASR_REQUIRE(a->n_seq >= 1 && a->n_head >= 1 && a->n_splits >= 1, "dec_attention: bad sizes");
+  OASR_REQUIRE(kv_group >= 1, "dec_attention: kv_group must be >= 1 (got %d)", kv_group);
   OASR_REQUIRE(a->pos_ptr != nullptr || a->n_keys >= 1, "dec_attention: key count missing");
   OASR_REQUIRE((a->ldq % 8) == 0 && (a->kv_row_stride % 8) == 0 && (a->kv_seq_stride % 8) == 0, "dec_attention: strides must be multiples of 8");
   dim3 grid((unsigned)a->n_splits, (unsigned)a->n_head, (unsigned)a->n_seq);
-  cudaStream_t st = (cudaStream_t)stream;
   OASR_REQUIRE(a->dtype == OASR_DTYPE_F16 || a->dtype == OASR_DTYPE_BF16, "dec_attention: unknown dtype %d", a->dtype);
   const bool f16 = a->dtype == OASR_DTYPE_F16;
   if (a->n_splits == 1 && (a->pos_ptr != nullptr || a->n_keys <= 1536)) {   // whole key range in one CTA: fused form
-    if (f16) OASR_CUDA_OK(launch_pdl(dec_attn_fused_kernel<__half>, grid, dim3(128), st, *a));
-    else OASR_CUDA_OK(launch_pdl(dec_attn_fused_kernel<bf16>, grid, dim3(128), st, *a));
+    if (f16) OASR_CUDA_OK(launch_pdl(dec_attn_fused_kernel<__half>, grid, dim3(128), st, *a, kv_group));
+    else OASR_CUDA_OK(launch_pdl(dec_attn_fused_kernel<bf16>, grid, dim3(128), st, *a, kv_group));
     return OASR_OK;
   }
   if (f16) {
-    OASR_CUDA_OK(launch_pdl(dec_attn_scores_kernel<__half>, grid, dim3(128), st, *a));
-    OASR_CUDA_OK(launch_pdl(dec_attn_pv_kernel<__half>, grid, dim3(128), st, *a));
+    OASR_CUDA_OK(launch_pdl(dec_attn_scores_kernel<__half>, grid, dim3(128), st, *a, kv_group));
+    OASR_CUDA_OK(launch_pdl(dec_attn_pv_kernel<__half>, grid, dim3(128), st, *a, kv_group));
   } else {
-    OASR_CUDA_OK(launch_pdl(dec_attn_scores_kernel<bf16>, grid, dim3(128), st, *a));
-    OASR_CUDA_OK(launch_pdl(dec_attn_pv_kernel<bf16>, grid, dim3(128), st, *a));
+    OASR_CUDA_OK(launch_pdl(dec_attn_scores_kernel<bf16>, grid, dim3(128), st, *a, kv_group));
+    OASR_CUDA_OK(launch_pdl(dec_attn_pv_kernel<bf16>, grid, dim3(128), st, *a, kv_group));
   }
   return OASR_OK;
+}
+}  // namespace
+
+extern "C" int oasr_dec_attention(const oasr_dec_attn_args* a, void* stream) { return dec_attention(a, 1, (cudaStream_t)stream); }
+
+extern "C" int oasr_dec_attention_grouped(const oasr_dec_attn_args* a, int kv_group, void* stream) {
+  return dec_attention(a, kv_group, (cudaStream_t)stream);
 }
 
 extern "C" int oasr_dec_sample(const oasr_dec_sample_args* a, void* stream) {
@@ -1015,6 +1391,52 @@ extern "C" int oasr_dec_sample(const oasr_dec_sample_args* a, void* stream) {
   OASR_CUDA_OK(launch_pdl(dec_sample_kernel, dim3((unsigned)a->n_slices, (unsigned)a->n_seq), dim3(256), (cudaStream_t)stream, *a));
   OASR_CUDA_OK(launch_pdl(dec_advance_kernel, dim3(1), dim3(1), (cudaStream_t)stream, a->pos_ptr, a->n_unfinished, a->done_flag,
                           (int)a->sample_begin));
+  return OASR_OK;
+}
+
+static int check_beam_args(const oasr_dec_beam_args* a, const char* what) {
+  OASR_REQUIRE(a != nullptr && a->logits && a->tokens && a->pos_ptr && a->suppress && a->sum_logprobs && a->no_speech_prob &&
+                   a->n_unfinished && a->done_flag && a->scratch && a->src_rows && a->fin_tokens && a->fin_scores && a->fin_len &&
+                   a->fin_count && a->seq_len, "%s: null tensor", what);
+  OASR_REQUIRE(a->beam >= 1 && a->beam <= BEAM_MAX, "%s: 1 <= beam <= %d (got %d)", what, BEAM_MAX, a->beam);
+  OASR_REQUIRE(a->max_candidates >= 1 && a->max_candidates <= 32, "%s: 1 <= max_candidates <= 32 (got %d)", what, a->max_candidates);
+  OASR_REQUIRE(a->n_clips >= 1 && a->n_clips * a->beam <= 64, "%s: 1 <= n_clips x beam <= 64", what);
+  OASR_REQUIRE(a->n_slices >= 1 && a->n_slices <= 64 && a->n_vocab >= 1, "%s: 1 <= n_slices <= 64", what);
+  OASR_REQUIRE(a->n_ctx >= 1 && a->n_ctx + 2 <= BEAM_TOK_MAX && a->ld_tokens >= a->n_ctx + 2 && a->ld_fin >= a->n_ctx + 1,
+               "%s: n_ctx + 2 <= %d, ld_tokens >= n_ctx + 2, ld_fin >= n_ctx + 1", what, BEAM_TOK_MAX);
+  OASR_REQUIRE(((uintptr_t)a->logits & 15) == 0 && (a->ld_logits % 4) == 0, "%s: logits rows must be 16-byte aligned", what);
+  OASR_REQUIRE(!a->timestamps || (a->timestamp_begin > a->eot && a->timestamp_begin < a->n_vocab), "%s: bad timestamp_begin", what);
+  return OASR_OK;
+}
+
+extern "C" int oasr_dec_beam_candidates(const oasr_dec_beam_args* a, void* stream) {
+  if (int rc = check_beam_args(a, "dec_beam_candidates")) return rc;
+  OASR_CUDA_OK(launch_pdl(dec_beam_cand_kernel, dim3((unsigned)a->n_slices, (unsigned)(a->n_clips * a->beam)), dim3(256),
+                          (cudaStream_t)stream, *a));
+  return OASR_OK;
+}
+
+extern "C" int oasr_dec_beam_select(const oasr_dec_beam_args* a, void* stream) {
+  if (int rc = check_beam_args(a, "dec_beam_select")) return rc;
+  OASR_CUDA_OK(launch_pdl(dec_beam_select_kernel, dim3((unsigned)a->n_clips), dim3(256), (cudaStream_t)stream, *a));
+  OASR_CUDA_OK(launch_pdl(dec_advance_kernel, dim3(1), dim3(1), (cudaStream_t)stream, a->pos_ptr, a->n_unfinished, a->done_flag,
+                          (int)a->sample_begin));
+  return OASR_OK;
+}
+
+extern "C" int oasr_dec_beam_reorder(void* k_cache, void* v_cache, int64_t layer_stride, int64_t row_stride, int64_t n_layers,
+                                     const int32_t* src_rows, const int32_t* pos_ptr, int32_t n_clips, int32_t beam, int32_t d,
+                                     int32_t n_pos_blocks, int dtype, void* stream) {
+  OASR_REQUIRE(k_cache && v_cache && src_rows && pos_ptr, "dec_beam_reorder: null tensor");
+  OASR_REQUIRE(dtype == OASR_DTYPE_F16 || dtype == OASR_DTYPE_BF16, "dec_beam_reorder: fp16 / bf16 caches only");
+  OASR_REQUIRE(beam >= 1 && beam <= BEAM_MAX && n_clips >= 1 && n_layers >= 1 && n_pos_blocks >= 1, "dec_beam_reorder: bad sizes");
+  OASR_REQUIRE(d % 8 == 0 && beam * (d / 8) <= 256 * REORDER_ITEMS, "dec_beam_reorder: d must be a multiple of 8 and beam x d <= %d",
+               256 * 8 * REORDER_ITEMS);
+  OASR_REQUIRE((row_stride % 8) == 0 && (layer_stride % 8) == 0 && ((uintptr_t)k_cache & 15) == 0 && ((uintptr_t)v_cache & 15) == 0,
+               "dec_beam_reorder: caches must be 16-byte aligned");
+  OASR_CUDA_OK(launch_pdl(dec_beam_reorder_kernel, dim3((unsigned)n_pos_blocks, (unsigned)(2 * n_layers), (unsigned)n_clips), dim3(256),
+                          (cudaStream_t)stream, (uint16_t*)k_cache, (uint16_t*)v_cache, layer_stride, row_stride, src_rows, pos_ptr,
+                          (int)beam, (int)d));
   return OASR_OK;
 }
 

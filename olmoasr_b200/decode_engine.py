@@ -14,6 +14,10 @@ What the reference does per step and what replaces it:
   * 4 small matmul / softmax kernels per attention + separate LN, bias,
     GELU, residual kernels                                               -> 8-9 launches per layer (csrc/decode.cu), 100-112 per step (small)
 
+`beam_search` runs whisper/decoding.py's BeamSearchDecoder (with ApplyTimestampRules when asked) the same way: the step
+graph ends in a candidate kernel, a per-clip ranking kernel that keeps the finished lists on the device, and an in-place
+reorder of the self-attention cache; the beams of one clip share its cross-attention K / V (one projection per clip).
+
 The activation dtype is fp16 (upstream default `fp16=True`) or bf16; the decoder-step kernels reproduce the reference's
 rounding points in that dtype.  The audio encoder and the cross K/V projection run on the bf16 wgmma kernels in both
 cases (their bf16 outputs are converted to fp16 for an fp16 decoder).
@@ -28,11 +32,14 @@ import torch
 from torch import Tensor
 
 from . import _lib
-from ._lib import DTYPE_BF16, DTYPE_F16, DTYPE_F32, DecAttnArgs, DecLinearArgs, DecSampleArgs, call, ptr, stream
+from ._lib import DTYPE_BF16, DTYPE_F16, DTYPE_F32, DecAttnArgs, DecBeamArgs, DecLinearArgs, DecSampleArgs, call, ptr, stream
 
 X_PLAIN, X_LAYERNORM, X_PARTIAL_SUM = 0, 1, 2
 EPI_STORE, EPI_GELU, EPI_RESIDUAL, EPI_LOGITS_F32, EPI_QKV_SCATTER = 0, 1, 2, 3, 4
 _DT = {torch.float16: DTYPE_F16, torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
+TIMESTAMP_BEGIN, NO_TIMESTAMPS = 50363, 50362
+BEAM_MAX, MAX_CANDIDATES = 8, 32
+BEAM_SCRATCH = 48      # floats per (row, slice) of the beam candidate kernel
 
 
 def _convert(src: Tensor, dst: Tensor) -> Tensor:
@@ -84,6 +91,15 @@ class DecodeEngine:
         self.sample_slices = 16          # blocks per sequence in the sampling kernel
         self.sample_scratch = z(N, self.sample_slices, 8, dt=torch.float32)
         self.sample_counters = torch.zeros(N, device=dev, dtype=torch.int32)
+        # beam search state (row = clip * beam + j): candidates per slice, source rows, finished lists per clip
+        self.beam_scratch = z(N, self.sample_slices, BEAM_SCRATCH, dt=torch.float32)
+        self.src_rows = torch.zeros(N, device=dev, dtype=torch.int32)
+        self.fin_tokens = torch.zeros((N, MAX_CANDIDATES, self.n_ctx + 1), device=dev, dtype=torch.int32)
+        self.fin_scores = z(N, MAX_CANDIDATES, dt=torch.float32)
+        self.fin_len = torch.zeros((N, MAX_CANDIDATES), device=dev, dtype=torch.int32)
+        self.fin_count = torch.zeros(N, device=dev, dtype=torch.int32)
+        self.seq_len = torch.zeros(1, device=dev, dtype=torch.int32)
+        self._beam_cfg = None      # (beam, clips, max_candidates, timestamps, max_initial_timestamp_index or -1) while beam searching
         self._w: Optional[dict] = None
         self._w_sig = None
         self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}
@@ -147,7 +163,7 @@ class DecodeEngine:
         a.M, a.N, a.dtype = n, W.shape[0], self.dt
         call("oasr_dec_linear", ctypes.byref(a), stream())
 
-    def _attention(self, n, k, v, seq_stride, row_stride, part, splits, n_keys=None):
+    def _attention(self, n, k, v, seq_stride, row_stride, part, splits, n_keys=None, kv_group=1):
         a = DecAttnArgs()
         a.q, a.ldq = ptr(self.q), self.q.stride(0)
         a.k, a.v, a.kv_seq_stride, a.kv_row_stride = ptr(k), ptr(v), seq_stride, row_stride
@@ -156,7 +172,10 @@ class DecodeEngine:
         a.pos_ptr = None if n_keys is not None else ptr(self.pos)
         a.n_keys = n_keys or 0
         a.n_seq, a.n_head, a.n_splits, a.scale, a.dtype = n, self.H, splits, 64 ** -0.25, self.dt
-        call("oasr_dec_attention", ctypes.byref(a), stream())
+        if kv_group == 1:
+            call("oasr_dec_attention", ctypes.byref(a), stream())
+        else:                           # sequence r reads cross K / V entry r // kv_group (the beams of one clip)
+            call("oasr_dec_attention_grouped", ctypes.byref(a), kv_group, stream())
         if splits == 1:
             _lib.LAUNCH_COUNT -= 1      # an unsplit key range runs as ONE fused kernel (scores + softmax + P V), not two
 
@@ -177,6 +196,7 @@ class DecodeEngine:
         # the attention kernels lay their fp32 partial outputs out as (splits, n, d): views with exactly that geometry
         part_self = self.part_self.view(-1)[: n * d].view(1, n, d)
         part_cross = self.part_cross.view(-1)[: sc * n * d].view(sc, n, d)
+        kv_group = 1 if self._beam_cfg is None else self._beam_cfg[0]
         for l, lw in enumerate(w["layers"]):
             self._linear(n, x, lw["wqkv"], lw["bqkv"], q, x_mode=X_LAYERNORM, ln=lw["ln1"], epi=EPI_QKV_SCATTER,
                          kv=(self.self_k[l], self.self_v[l]))
@@ -184,11 +204,15 @@ class DecodeEngine:
             self._linear(n, part_self, lw["wo"], lw["bo"], x, x_mode=X_PARTIAL_SUM, n_partials=1, epi=EPI_RESIDUAL, res=x)
             self._linear(n, x, lw["wcq"], lw["bcq"], q, x_mode=X_LAYERNORM, ln=lw["lnc"])
             ckv = self.cross_kv[l]
-            self._attention(n, ckv, ckv[:, d:], seq_cross, 2 * d, part_cross, sc, n_keys=self.n_audio_ctx)
+            self._attention(n, ckv, ckv[:, d:], seq_cross, 2 * d, part_cross, sc, n_keys=self.n_audio_ctx, kv_group=kv_group)
             self._linear(n, part_cross, lw["wco"], lw["bco"], x, x_mode=X_PARTIAL_SUM, n_partials=sc, epi=EPI_RESIDUAL, res=x)
             self._linear(n, x, lw["w1"], lw["b1"], h, x_mode=X_LAYERNORM, ln=lw["ln2"], epi=EPI_GELU)
             self._linear(n, h, lw["w2"], lw["b2"], x, epi=EPI_RESIDUAL, res=x)
         self._linear(n, x, w["emb_t"], None, self.logits, x_mode=X_LAYERNORM, ln=w["ln"], epi=EPI_LOGITS_F32)
+        if self._beam_cfg is not None:
+            self._enqueue_beam_select()
+            self.launches_per_step = _lib.LAUNCH_COUNT - c0
+            return
         s = DecSampleArgs()
         s.logits, s.ld_logits = ptr(self.logits), self.logits.stride(0)
         s.tokens, s.ld_tokens, s.pos_ptr = ptr(self.tokens), self.tokens.stride(0), ptr(self.pos)
@@ -202,12 +226,13 @@ class DecodeEngine:
         self.launches_per_step = _lib.LAUNCH_COUNT - c0
 
     def _graph(self, n: int) -> torch.cuda.CUDAGraph:
-        key = (n, self._sample_cfg)
+        key = (n, self._sample_cfg, self._beam_cfg)
         g = self._graphs.get(key)
         if g is None:
             # one eager run first (kernel modules are loaded lazily on first launch, which must not happen under capture),
             # with the device-side decode state saved and restored around it; the capture itself does not execute
-            live = (self.pos, self.tokens, self.sum_logprobs, self.no_speech, self.n_unfinished, self.done, self.sample_counters)
+            live = (self.pos, self.tokens, self.sum_logprobs, self.no_speech, self.n_unfinished, self.done, self.sample_counters,
+                    self.src_rows, self.fin_tokens, self.fin_scores, self.fin_len, self.fin_count, self.seq_len)
             state = [t.clone() for t in live]
             self._enqueue_step(n)
             torch.cuda.synchronize(self.dev)
@@ -260,6 +285,7 @@ class DecodeEngine:
             sup[torch.tensor(ids, dtype=torch.long)] = 1
         self.suppress.copy_(sup)
         self._sample_cfg = (P if sample_begin is None else sample_begin, sot_index, int(bool(suppress_blank)), blank, eot, no_speech)
+        self._beam_cfg = None
 
     def replay(self, n: int):
         """One decoder step for sequences [0, n): feeds the token at the device-side position, leaves the fp32 logits of that
@@ -292,6 +318,109 @@ class DecodeEngine:
                 break
         length = n_init + max(0, replays - (n_init - 1))
         return (self.tokens[:n, :length].to(torch.int64).cpu(), self.sum_logprobs[:n].clone(), self.no_speech[:n].clone(), replays)
+
+    # ---- beam search ------------------------------------------------------------------------------------------------
+    def reset_beam(self, n_clips: int, beam: int, max_candidates: int, timestamps: bool = False,
+                   max_initial_timestamp_index: Optional[int] = None):
+        """Switch the state left by `reset` (n_clips * beam rows) to beam search: empty finished lists, identity sources."""
+        self.fin_count.zero_(); self.fin_len.zero_(); self.seq_len.zero_()
+        self.src_rows.copy_(torch.arange(self.max_batch, device=self.dev, dtype=torch.int32))
+        mi = -1 if max_initial_timestamp_index is None else int(max_initial_timestamp_index)
+        self._beam_cfg = (beam, n_clips, max_candidates, int(bool(timestamps)), mi)
+
+    def beam_args(self) -> DecBeamArgs:
+        """Argument block of the beam candidate / select kernels for the current state."""
+        beam, clips, max_cand, ts, mi = self._beam_cfg
+        sample_begin, sot_index, suppress_blank, blank, eot, no_speech = self._sample_cfg
+        a = DecBeamArgs()
+        a.logits, a.ld_logits = ptr(self.logits), self.logits.stride(0)
+        a.tokens, a.ld_tokens, a.pos_ptr = ptr(self.tokens), self.tokens.stride(0), ptr(self.pos)
+        a.suppress, a.sum_logprobs, a.no_speech_prob = ptr(self.suppress), ptr(self.sum_logprobs), ptr(self.no_speech)
+        a.n_unfinished, a.done_flag = ptr(self.n_unfinished), ptr(self.done)
+        a.scratch, a.src_rows = ptr(self.beam_scratch), ptr(self.src_rows)
+        a.fin_tokens, a.ld_fin = ptr(self.fin_tokens), self.fin_tokens.stride(1)
+        a.fin_scores, a.fin_len, a.fin_count, a.seq_len = ptr(self.fin_scores), ptr(self.fin_len), ptr(self.fin_count), ptr(self.seq_len)
+        a.n_clips, a.beam, a.max_candidates, a.n_vocab, a.n_slices, a.n_ctx = clips, beam, max_cand, self.V, self.sample_slices, self.n_ctx
+        a.sample_begin, a.sot_index, a.suppress_blank, a.blank, a.eot, a.no_speech = sample_begin, sot_index, suppress_blank, blank, eot, no_speech
+        a.timestamps, a.timestamp_begin, a.no_timestamps, a.max_initial_timestamp = ts, TIMESTAMP_BEGIN, NO_TIMESTAMPS, mi
+        return a
+
+    def finished_lists(self, n_clips: int, max_candidates: int):
+        """(count (C,), lengths (C, M), token rows (C, M, n_ctx + 1), scores (C, M)) views of the device finished lists
+        (the kernels lay them out clip-major with max_candidates entries per clip)."""
+        C, M, ld = n_clips, max_candidates, self.fin_tokens.shape[-1]
+        return (self.fin_count[:C], self.fin_len.view(-1)[: C * M].view(C, M),
+                self.fin_tokens.view(-1, ld)[: C * M].view(C, M, ld), self.fin_scores.view(-1)[: C * M].view(C, M))
+
+    def reorder_blocks(self, n_clips: int) -> int:
+        """Position blocks of the kv reorder grid (x 2 L layers-and-K/V x clips): about two CTAs per SM."""
+        return max(1, min(self.n_ctx, math.ceil(2 * _lib.lib().oasr_device_sm_count() / (2 * self.L * n_clips))))
+
+    def reorder_kv(self, n_clips: int, beam: int):
+        call("oasr_dec_beam_reorder", ptr(self.self_k), ptr(self.self_v), self.self_k.stride(0), self.self_k.stride(1), self.L,
+             ptr(self.src_rows), ptr(self.pos), n_clips, beam, self.d, self.reorder_blocks(n_clips), self.dt, stream())
+
+    def _enqueue_beam_select(self):
+        """Candidates, ranking + finished lists + position advance, kv reorder: 1 + 2 + 1 launches."""
+        a = self.beam_args()
+        call("oasr_dec_beam_candidates", ctypes.byref(a), stream())
+        call("oasr_dec_beam_select", ctypes.byref(a), stream())
+        self.reorder_kv(a.n_clips, a.beam)
+
+    @torch.no_grad()
+    def beam_search(self, audio_features: Tensor, initial_tokens: Sequence[int], sample_len: int, beam_size: int,
+                    patience: Optional[float] = None, suppress: Sequence[int] = (), suppress_blank: bool = True,
+                    sot_index: int = 0, timestamps: bool = False, max_initial_timestamp_index: Optional[int] = None,
+                    blank: int = 220, eot: int = 50256, no_speech: int = 50361, check_every: int = 8):
+        """Beam search over the clips of `audio_features` (whisper/decoding.py BeamSearchDecoder, with ApplyTimestampRules
+        when `timestamps`).  Cross K/V is projected once per clip and shared by its beams.  Returns (candidates,
+        no_speech_probs (n_clips,), number of graph replays): candidates[c] is the list of (token ids incl. the initial
+        tokens and the final eot, sum_logprob) of BeamSearchDecoder.finalize, in its order."""
+        import numpy as np
+
+        if not 1 <= beam_size <= BEAM_MAX:
+            raise ValueError(f"beam_size must be in 1 .. {BEAM_MAX} (got {beam_size})")
+        max_cand = round(beam_size * (patience or 1.0))
+        if not 1 <= max_cand <= MAX_CANDIDATES:
+            raise ValueError(f"round(beam_size * patience) must be in 1 .. {MAX_CANDIDATES} (got {max_cand})")
+        C = audio_features.shape[0]
+        if C * beam_size > self.max_batch:
+            raise ValueError(f"beam search: at most {self.max_batch // beam_size} clips per call at beam {beam_size} (got {C})")
+        init = list(initial_tokens)
+        n_init = len(init)
+        if not 1 <= n_init < self.n_ctx:
+            raise ValueError("initial_tokens: need 1 .. n_text_ctx-1 tokens")
+        self.prepare(audio_features)
+        n = C * beam_size
+        self.reset(n, torch.tensor([init], dtype=torch.int32).repeat(n, 1), None, suppress, suppress_blank, sot_index, blank, eot, no_speech)
+        self.reset_beam(C, beam_size, max_cand, timestamps, max_initial_timestamp_index)
+        g = self._graph(n)
+        n_sampling = min(sample_len, self.n_ctx + 1 - n_init)
+        total = (n_init - 1) + n_sampling
+        replays = 0
+        for i in range(total):
+            g.replay()
+            replays += 1
+            sampled = replays - (n_init - 1)
+            if sampled > 0 and sampled % check_every == 0 and i + 1 < total and int(self.done.item()) == 1:
+                break
+        # one copy to the host at the end; BeamSearchDecoder.finalize there
+        seq_len = int(self.seq_len.item())
+        toks = self.tokens[:n, :seq_len].cpu()
+        lps = self.sum_logprobs[:n].cpu()
+        cnt, lens, fin, scores = (t.cpu() for t in self.finished_lists(C, max_cand))
+        nsp = self.no_speech[:n:beam_size].clone()
+        candidates = []
+        for c in range(C):
+            seqs = [(fin[c, i, : int(lens[c, i])].tolist(), float(scores[c, i])) for i in range(int(cnt[c]))]
+            if len(seqs) < beam_size:        # not enough finished: the live beams, best first, each closed by eot
+                lp = lps[c * beam_size:(c + 1) * beam_size]
+                for j in list(np.argsort(lp.numpy()))[::-1]:
+                    seqs.append((toks[c * beam_size + j].tolist() + [eot], float(lp[j])))
+                    if len(seqs) >= beam_size:
+                        break
+            candidates.append(seqs)
+        return candidates, nsp, replays
 
     # ---- roofline bookkeeping --------------------------------------------------------------------------------------
     def step_bytes(self, n: int, t: int) -> int:

@@ -1,12 +1,17 @@
-"""Greedy / temperature decoding with a kv cache -- the `model.decode(mel, DecodingOptions(...))` entry point the
-reference binds to third-party `whisper.decoding.decode` (olmoasr/model.py:9-10,966-968; call sites
+"""Greedy / temperature / best-of / beam-search decoding with a kv cache -- the `model.decode(mel, DecodingOptions(...))`
+entry point the reference binds to third-party `whisper.decoding.decode` (olmoasr/model.py:9-10,966-968; call sites
 scripts/training/train_timestamps.py:1916-1919, scripts/eval/eval.py:1846-1847, olmoasr/transcribe.py:209-210).
 
 openai-whisper is not vendored by the reference and is absent here, so this restates the published algorithm of
 `whisper/decoding.py` for the path OLMoASR uses (English-only `gpt2` vocabulary, n_vocab 51864):
-DecodingTask._main_loop, PyTorchInference (first call = whole prefix, later calls = last token, kv cache through
-`model.install_kv_cache_hooks()`), GreedyDecoder, SuppressBlank, SuppressTokens, ApplyTimestampRules.
-Beam search is not implemented (long-form eval only, out of scope for the hot path).
+DecodingTask._verify_options / _main_loop, PyTorchInference (first call = whole prefix, later calls = last token, kv cache
+through `model.install_kv_cache_hooks()`), GreedyDecoder, BeamSearchDecoder, MaximumLikelihoodRanker, SuppressBlank,
+SuppressTokens, ApplyTimestampRules.
+
+Routes: greedy without timestamps and beam search (with or without timestamps) run on the device decoder
+(olmoasr_b200/decode_engine.py) as replays of one CUDA graph per step; greedy with timestamps and temperature sampling
+(best_of samples per clip, ranked like upstream) run on the hook loop below.  Beam search needs the device decoder: a
+model without `decode_engine`, or OASR_DECODE_ENGINE=0, raises NotImplementedError for `beam_size`.
 
 Token ids are the contract: text<->id conversion needs the `gpt2.tiktoken` vocabulary, which is not available offline;
 pass `tokenizer=` (an object with `.decode(list[int])`) to get text, otherwise `DecodingResult.text` is empty.
@@ -123,13 +128,53 @@ class _TimestampRules:
                 logits[k, :TIMESTAMP_BEGIN] = -np.inf
 
 
+class MaximumLikelihoodRanker:
+    """whisper/decoding.py MaximumLikelihoodRanker: per clip the candidate with the highest sum_logprob / penalty,
+    penalty = length without a length_penalty, else the Google NMT ((5 + length) / 6) ** length_penalty."""
+
+    def __init__(self, length_penalty: Optional[float]):
+        self.length_penalty = length_penalty
+
+    def rank(self, tokens: List[List[List[int]]], sum_logprobs: List[List[float]]) -> List[int]:
+        def scores(logprobs, lengths):
+            result = []
+            for logprob, length in zip(logprobs, lengths):
+                penalty = length if self.length_penalty is None else ((5 + length) / 6) ** self.length_penalty
+                result.append(logprob / penalty)
+            return result
+
+        lengths = [[len(t) for t in s] for s in tokens]
+        return [int(np.argmax(scores(p, l))) for p, l in zip(sum_logprobs, lengths)]
+
+
+def verify_options(options: DecodingOptions):
+    """DecodingTask._verify_options (the checks that apply to the English-only models)."""
+    if options.beam_size is not None and options.best_of is not None:
+        raise ValueError("beam_size and best_of can't be given together")
+    if options.temperature == 0 and options.best_of is not None:
+        raise ValueError("best_of with greedy sampling (T=0) is not compatible")
+    if options.patience is not None and options.beam_size is None:
+        raise ValueError("patience requires beam_size to be given")
+    if options.length_penalty is not None and not 0 <= options.length_penalty <= 1:
+        raise ValueError("length_penalty (alpha) should be a value between 0 and 1")
+
+
 class DecodingTask:
     def __init__(self, model: "OLMoASRBase", options: DecodingOptions):
-        if options.beam_size is not None or (options.best_of or 1) > 1:
-            raise NotImplementedError("beam search / best_of sampling are not part of the hot path (greedy only)")
+        verify_options(options)
+        if options.beam_size is not None:
+            if not (USE_ENGINE and hasattr(model, "decode_engine")):
+                raise NotImplementedError("beam search runs on the device decoder only (model.decode_engine)")
+            from .decode_engine import BEAM_MAX, MAX_CANDIDATES
+            if not 1 <= options.beam_size <= BEAM_MAX:
+                raise ValueError(f"beam_size must be in 1 .. {BEAM_MAX}")
+            if not 1 <= round(options.beam_size * (options.patience or 1.0)) <= MAX_CANDIDATES:
+                raise ValueError(f"round(beam_size * patience) must be in 1 .. {MAX_CANDIDATES}")
         if model.is_multilingual:
             raise NotImplementedError("only the English-only vocabulary of the OLMoASR checkpoints is supported")
         self.model, self.options = model, options
+        self.n_group = options.beam_size or options.best_of or 1
+        self.ranker = MaximumLikelihoodRanker(options.length_penalty)
         self.n_ctx = model.dims.n_text_ctx
         self.sample_len = options.sample_len or model.dims.n_text_ctx // 2
         sot_seq = [SOT] + ([NO_TIMESTAMPS] if options.without_timestamps else [])
@@ -159,17 +204,22 @@ class DecodingTask:
             audio_features = model.encoder(mel)
         n_audio = audio_features.shape[0]
         dev = audio_features.device
+        if opt.beam_size is not None:
+            return self._run_beam_on_device(audio_features, tokenizer)
         if opt.temperature == 0 and self.ts_rules is None and USE_ENGINE and hasattr(model, "decode_engine"):
             return self._run_on_device(audio_features, tokenizer)
-        tokens = torch.tensor([self.initial_tokens], device=dev).repeat(n_audio, 1)
-        sum_logprobs = torch.zeros(n_audio, device=dev)
-        no_speech_probs = [np.nan] * n_audio
+        G = self.n_group                           # best_of samples per clip (temperature > 0), rows clip-major
+        xa = audio_features.repeat_interleave(G, dim=0) if G > 1 else audio_features
+        n_rows = n_audio * G
+        tokens = torch.tensor([self.initial_tokens], device=dev).repeat(n_rows, 1)
+        sum_logprobs = torch.zeros(n_rows, device=dev)
+        no_speech_probs = [np.nan] * n_rows
         suppress = torch.tensor(self.suppress, device=dev, dtype=torch.long) if self.suppress else None
         cache, hooks = model.install_kv_cache_hooks()
         try:
             for i in range(self.sample_len):
                 inp = tokens if tokens.shape[-1] <= len(self.initial_tokens) else tokens[:, -1:]
-                logits = model.decoder(inp, audio_features, kv_cache=cache)
+                logits = model.decoder(inp, xa, kv_cache=cache)
                 if i == 0:
                     probs_at_sot = logits[:, self.sot_index].float().softmax(dim=-1)
                     no_speech_probs = probs_at_sot[:, NO_SPEECH].tolist()
@@ -186,7 +236,7 @@ class DecodingTask:
                 else:
                     next_tokens = torch.distributions.Categorical(logits=logits / opt.temperature).sample()
                 logprobs = F.log_softmax(logits.float(), dim=-1)
-                current = logprobs[torch.arange(n_audio, device=dev), next_tokens]
+                current = logprobs[torch.arange(n_rows, device=dev), next_tokens]
                 sum_logprobs += current * (tokens[:, -1] != EOT)
                 next_tokens[tokens[:, -1] == EOT] = EOT
                 tokens = torch.cat([tokens, next_tokens[:, None]], dim=-1)
@@ -196,7 +246,50 @@ class DecodingTask:
             for h in hooks:
                 h.remove()
         tokens = F.pad(tokens, (0, 1), value=EOT)  # GreedyDecoder.finalize
-        return self._results(audio_features, tokens, sum_logprobs.tolist(), no_speech_probs, tokenizer)
+        if G == 1:
+            return self._results(audio_features, tokens, sum_logprobs.tolist(), no_speech_probs, tokenizer)
+        rows, lps = tokens.tolist(), sum_logprobs.tolist()
+        candidates = [[(rows[k * G + j], lps[k * G + j]) for j in range(G)] for k in range(n_audio)]
+        return self._ranked(audio_features, candidates, no_speech_probs[::G], tokenizer)
+
+    def _run_beam_on_device(self, audio_features: Tensor, tokenizer):
+        """Beam search (the long-form eval configuration, scripts/eval/eval.py:2077-2084) on the device decoder: one CUDA
+        graph replay per step, candidates / ranking / kv reorder in kernels, up to 64 // beam_size clips per call."""
+        opt = self.options
+        eng = self.model.decode_engine(torch.float16 if opt.fp16 else torch.bfloat16)
+        per = eng.max_batch // opt.beam_size
+        ts = self.ts_rules is not None
+        mi = self.ts_rules.max_initial_timestamp_index if ts else None
+        candidates, nsp = [], []
+        for s in range(0, audio_features.shape[0], per):
+            c, ns, _ = eng.beam_search(audio_features[s:s + per], self.initial_tokens, self.sample_len, opt.beam_size, opt.patience,
+                                       self.suppress, opt.suppress_blank, self.sot_index, timestamps=ts,
+                                       max_initial_timestamp_index=mi)
+            candidates += c
+            nsp += ns.tolist()
+        return self._ranked(audio_features, candidates, nsp, tokenizer)
+
+    def _ranked(self, audio_features, candidates, no_speech_probs, tokenizer) -> List[DecodingResult]:
+        """DecodingTask.run after finalize: candidates[k] = [(full token row ending in eot, sum_logprob), ...]; each is cut
+        to the sampled tokens before the first eot and the ranker picks one per clip."""
+        opt = self.options
+        tokens, sum_logprobs = [], []
+        for cands in candidates:
+            seqs = []
+            for row, _ in cands:
+                seq = row[self.sample_begin:]
+                seqs.append(seq[: seq.index(EOT)] if EOT in seq else seq)
+            tokens.append(seqs)
+            sum_logprobs.append([lp for _, lp in cands])
+        selected = self.ranker.rank(tokens, sum_logprobs)
+        results = []
+        for k, i in enumerate(selected):
+            ids, lp = tokens[k][i], sum_logprobs[k][i]
+            text = tokenizer.decode([t for t in ids if t < EOT]).strip() if tokenizer is not None else ""
+            results.append(DecodingResult(audio_features=audio_features[k], language="en", tokens=ids, text=text,
+                                          avg_logprob=lp / (len(ids) + 1), no_speech_prob=no_speech_probs[k],
+                                          temperature=opt.temperature))
+        return results
 
     def _run_on_device(self, audio_features: Tensor, tokenizer):
         """Greedy decoding without timestamp rules (the short-form eval configuration, scripts/eval/eval.py:1846-1847): the

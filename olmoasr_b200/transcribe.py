@@ -2,9 +2,12 @@
 519-523; README.md:199-246): `transcribe(model, audio, **opts) -> {"text", "segments", "language"}`.
 
 Caller of the hot path, kept so that `model.transcribe(...)` stays callable: GPU log-mel of the whole recording, a
-30 s window loop, greedy decode with temperature fallback (transcribe.py:193-233), timestamp-token driven seek advance
-(:348-408).  Like the reference, previous-text prompt conditioning is disabled (transcribe.py:297-302).  Not implemented
-(raises): word_timestamps (needs alignment heads OLMoASR never sets, __init__.py:145), beam search.
+30 s window loop, decode with temperature fallback (transcribe.py:193-233), timestamp-token driven seek advance
+(:348-408).  As in the reference (transcribe.py:199-207), `beam_size` / `patience` apply at temperature 0 (beam search on
+the device decoder) and `best_of` at the fallback temperatures (best-of-n sampling), so the long-form eval options
+`without_timestamps=False, beam_size=5, best_of=5` (scripts/eval/eval.py:2077-2084) work as given.  Like the reference,
+previous-text prompt conditioning is disabled (transcribe.py:297-302).  Not implemented (raises): word_timestamps (needs
+alignment heads OLMoASR never sets, __init__.py:145).
 
 Text needs a tokenizer: pass `tokenizer=` (object with `.decode(list[int]) -> str`); without one, segments carry token
 ids and empty text (the `gpt2.tiktoken` vocabulary cannot be fetched offline).
@@ -36,8 +39,6 @@ def transcribe(model, audio: Union[str, np.ndarray, torch.Tensor], *, verbose: O
                tokenizer=None, **decode_options):
     if word_timestamps:
         raise NotImplementedError("word_timestamps needs alignment heads, which OLMoASR checkpoints do not define")
-    if decode_options.get("beam_size") is not None:
-        raise NotImplementedError("beam search is outside the accelerated path (greedy + temperature fallback only)")
     decode_options.pop("fp16", None)
     decode_options.setdefault("language", "en")
     mel = log_mel_spectrogram(audio, model.dims.n_mels, padding=N_SAMPLES, device=model.device)
@@ -49,7 +50,9 @@ def transcribe(model, audio: Union[str, np.ndarray, torch.Tensor], *, verbose: O
     def decode_with_fallback(segment: torch.Tensor) -> DecodingResult:
         result = None
         for t in temps:
-            kw = {k: v for k, v in decode_options.items() if not (t > 0 and k in ("beam_size", "patience"))}
+            # beam search at t == 0, best-of-n sampling at t > 0 (transcribe.py:199-207)
+            drop = ("beam_size", "patience") if t > 0 else ("best_of",)
+            kw = {k: v for k, v in decode_options.items() if k not in drop}
             result = decode(model, segment, DecodingOptions(**kw, temperature=t), tokenizer=tokenizer)
             result = _with_ratio(result)
             retry = False

@@ -50,6 +50,10 @@ def main():
         for n in (3, 40):
             xa = torch.randn(n, 1500, 64, device=dev).bfloat16()
             eng.greedy(xa, [50257, 50362], 3, suppress=(7, 9))
+        # beam search: candidates, select, kv reorder, grouped cross-attention; with and without timestamp rules
+        xa = torch.randn(3, 1500, 64, device=dev).bfloat16()
+        eng.beam_search(xa, [50257, 50362], 4, 5, suppress=(7, 9))
+        eng.beam_search(xa[:2], [50257], 4, 3, patience=2.0, suppress=(7, 9), timestamps=True, max_initial_timestamp_index=50)
     torch.cuda.synchronize()
     print("sanitize run complete; loss", float(loss))
 
