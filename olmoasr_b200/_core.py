@@ -8,8 +8,8 @@ reference under `torch.autocast("cuda", torch.bfloat16)` (scripts/training/train
 its rounding points reproduced (Linear outputs, GELU, residual adds, LayerNorm casts, bf16 logits).
 
 Training fast path: one autograd.Function per ResidualAttentionBlock (+ stem, embedding and loss head) whose
-backward is a hand-sequenced list of kernels -- dgrad / wgrad GEMMs read the saved activations through
-MN-major UMMA descriptors, so nothing is transposed in HBM.
+backward is a hand-sequenced list of kernels -- dgrad / wgrad GEMMs read the saved activations MN-major through
+the wgmma shared-memory descriptors, so nothing is transposed in HBM.
 """
 from __future__ import annotations
 
@@ -94,38 +94,97 @@ def linear_wgrad(dy: Tensor, x: Tensor, n_valid: Optional[int] = None, side=None
     return side.run(launch) if side is not None else launch()
 
 
-class _ZeroPool:
-    """One zero-fill per backward instead of one per small gradient vector (each fill is a separate ~4 us launch;
-    ~700 of them per step otherwise).  Slices are 64-element aligned so every view stays 256-byte aligned."""
+# Projections of a block whose weight gradients one GEMM computes, stacked in this order (d rows each), and whose bias
+# gradients one column sum covers.  The key projections have no bias (model.py:259): their rows of the fused [bq; 0; bv]
+# bias are a gap of the slab that no gradient may ever be written to.
+_FUSED = {"attn.qkv": ("attn.query", "attn.key", "attn.value"), "cross_attn.kv": ("cross_attn.key", "cross_attn.value")}
 
-    def __init__(self, n_total: int, device):
-        self.buf = torch.zeros(n_total, device=device, dtype=torch.float32)
-        self.off = 0
 
-    def take(self, n: int) -> Tensor:
-        m = (n + 63) // 64 * 64
-        if self.off + m > self.buf.numel():  # defensive: never hand out overlapping storage
-            return torch.zeros(n, device=self.buf.device, dtype=torch.float32)
-        v = self.buf[self.off:self.off + n]
-        self.off += m
+class _GradDest:
+    """Where the parameter gradients of one backward go, decided once from `owner`, the module that holds them.
+
+    Direct mode (`use_slabs()` with `direct_grads`): every kernel ACCUMULATES into its parameter's slice of the gradient
+    slab, autograd is handed None, and `done()` fires the owner's `_bwd_done_cb` (olmoasr_b200.ddp.SlabGradSync).
+    Hand-over mode (no slabs, or `direct_grads=False` for torch DDP; FSDP's parameter views): fresh tensors are returned
+    to autograd, so wrappers that hook gradient accumulation and foreign optimizers keep working.  With `pool_size`, its
+    zeroed vectors are slices of one zero fill (each fill is a separate ~4 us launch; ~700 of them per step otherwise).
+    Weight and bias gradients are launched through `side` when given."""
+
+    def __init__(self, owner, device=None, side: Optional["_Side"] = None, pool_size: int = 0):
+        direct = owner is not None and owner._direct is not None and owner._slabs.direct_grads
+        self.owner, self.device, self.side = owner, device, side
+        self.slab: Optional[Dict[str, Tensor]] = owner._direct if direct else None
+        self.pool = torch.zeros(pool_size, device=device, dtype=torch.float32) if (pool_size and not direct) else None
+        self.used = 0
+        self.grads: Dict[str, Tensor] = {}
+
+    def out(self, key: str) -> Optional[Tensor]:
+        """The slab view a kernel accumulates `key`'s gradient into, or None: the kernel allocates the gradient."""
+        return None if self.slab is None else self.slab[key]
+
+    def keep(self, key: str, g: Tensor) -> Tensor:
+        self.grads[key] = g
+        return g
+
+    def _zeros(self, shape) -> Tensor:
+        """The next slice of the pool, 64-element aligned so that every view stays 256-byte aligned, else its own fill."""
+        if self.pool is None or self.used + (shape + 63) // 64 * 64 > self.pool.numel():
+            return torch.zeros(shape, device=self.device, dtype=torch.float32)
+        v = self.pool[self.used:self.used + shape]
+        self.used += (shape + 63) // 64 * 64
         return v
 
+    def vec(self, key: str, shape) -> Tensor:
+        """Zero-initialised accumulation target of `key`'s gradient (LayerNorm, embedding and bias vectors)."""
+        return self.slab[key] if self.slab is not None else self.keep(key, self._zeros(shape))
 
-def bias_grad(dy: Tensor, n: Optional[int] = None, pool: Optional[_ZeroPool] = None, side=None, out: Optional[Tensor] = None) -> Tensor:
-    """Column sums of dy (M, >= n) bf16, accumulated into `out` (a gradient-slab view) or a fresh zeroed vector."""
-    n = dy.shape[1] if n is None else n
-    db = out if out is not None else (pool.take(n) if pool is not None else torch.zeros(n, device=dy.device, dtype=torch.float32))
-    if side is not None:
-        return side.run(lambda: K.colsum_(dy, db, n))
-    return K.colsum_(dy, db, n)
+    def _launch(self, fn):
+        return self.side.run(fn) if self.side is not None else fn()
+
+    def weight(self, key: str, dy: Tensor, x: Tensor, n_valid: Optional[int] = None) -> Tensor:
+        return self.keep(key, linear_wgrad(dy, x, n_valid, side=self.side, out=self.out(key)))
+
+    def bias(self, key: str, dy: Tensor):
+        """Column sums of dy (M, n) bf16 into the bias gradient `key`."""
+        db = self.vec(key, dy.shape[1])
+        self._launch(lambda: K.colsum_(dy, db, dy.shape[1]))
+
+    def linear(self, name: str, dy: Tensor, x: Tensor):
+        """Weight and bias gradients of the Linear `name`, or of the projections `_FUSED[name]`, from the output
+        gradient dy and the input x."""
+        dw = self.weight(name + ".weight", dy, x)
+        members = _FUSED.get(name)
+        if members is None:
+            return self.bias(name + ".bias", dy)
+        d = dw.shape[0] // len(members)
+        if self.slab is not None:      # one column sum per member that has a bias, so no gap of the slab is written
+            for i, m in enumerate(members):
+                if m + ".bias" in self.slab:
+                    self.bias(m + ".bias", dy[:, i * d:(i + 1) * d])
+            return
+        self.bias(name + ".bias", dy)  # one column sum over the whole fused width; every member takes its rows
+        for i, m in enumerate(members):
+            for kind in (".weight", ".bias"):
+                self.grads[m + kind] = self.grads[name + kind][i * d:(i + 1) * d]
+
+    def grads_for(self, names: Iterable[str]) -> tuple:
+        """What autograd receives for these parameters: all None in direct mode, where the slab already holds them."""
+        if self.slab is not None:
+            return tuple(None for _ in names)
+        return tuple(self.grads[n] for n in names)
+
+    def done(self):
+        """Direct mode: tell the owner's gradient synchronisation hook that its slab range is final."""
+        if self.slab is not None and self.owner._bwd_done_cb is not None:
+            self.owner._bwd_done_cb()
 
 
 # ----------------------------------------------------------------------------------------------------
 # Weight / bias gradients of a block are leaves of the backward graph: nothing downstream in the same backward reads
-# them.  They are enqueued on a second CUDA stream so that their CTAs fill the tail waves (and launch gaps) of the
-# dgrad / attention / LayerNorm chain on the main stream -- e.g. the decoder's 14336 x 1024 x 1024 GEMMs are 3.03
-# waves of 256 x 256 tiles on 74 SM pairs, i.e. a quarter of their time runs on 2 pairs.  Every block joins the side
-# stream before its backward returns, so gradients are complete in main-stream order (DDP hooks, optimizer).
+# them.  They are enqueued on a second CUDA stream so that their CTAs fill the SMs that the dgrad / attention /
+# LayerNorm chain on the main stream leaves idle: the partial last wave of tiles of each persistent wgmma GEMM
+# (csrc/gemm_sm90.cu), and the gaps between launches.  Every block joins the side stream before its backward returns,
+# so gradients are complete in main-stream order (DDP hooks, optimizer).
 SIDE_STREAM = os.environ.get("OASR_SIDE_STREAM", "1") != "0"
 _side_streams: Dict[int, "torch.cuda.Stream"] = {}
 
@@ -457,51 +516,26 @@ class _BlockFn(torch.autograd.Function):
             x2 = x1
             mean2, rstd2, ln2, h, g = sv[8:13]
         dx3 = dx3.contiguous()
-        dev = x.device
-        # Where the parameter gradients go.  Slab mode (OLMoASRBase.use_slabs + direct_grads): every kernel ACCUMULATES into
-        # its parameter's slice of the flat gradient slab and autograd is handed None.  Otherwise: fresh tensors returned
-        # to autograd (DistributedDataParallel / any foreign optimizer keep working).
-        D = blk._direct if (blk._direct is not None and blk._slabs.direct_grads) else None
-        grads: Dict[str, Tensor] = {}
-        pool = None if D is not None else _ZeroPool(32 * d + 4096, dev)   # all bias / LayerNorm gradient vectors (<= 26 d)
-        side = _Side(dev)
-
-        def wg(key, dy, xin):
-            return linear_wgrad(dy, xin, side=side, out=None if D is None else D[key])
-
-        def bg(key, dy, n=None):
-            return bias_grad(dy, n, pool=pool, side=side, out=None if D is None else D[key])
-
-        def vec(key):
-            return D[key] if D is not None else pool.take(d)
-
+        side = _Side(x.device)
+        # hand-over mode takes all bias / LayerNorm gradient vectors (<= 26 d) from one zero fill
+        grads = _GradDest(blk, x.device, side, pool_size=32 * d + 4096)
         # ---- MLP: x3 = x2 + fc2(gelu(fc1(ln(x2))))
-        grads["mlp.2.weight"] = wg("mlp.2.weight", dx3, g)
-        grads["mlp.2.bias"] = bg("mlp.2.bias", dx3)
+        grads.linear("mlp.2", dx3, g)
         dh = linear_dgrad(dx3, sh["w2"], epi=K.EPI_BF16_GELU_BWD, aux=h)
-        grads["mlp.0.weight"] = wg("mlp.0.weight", dh, ln2)
-        grads["mlp.0.bias"] = bg("mlp.0.bias", dh)
+        grads.linear("mlp.0", dh, ln2)
         dln2 = linear_dgrad(dh, sh["w1"])
-        grads["mlp_ln.weight"], grads["mlp_ln.bias"] = vec("mlp_ln.weight"), vec("mlp_ln.bias")
-        dx2 = K.layernorm_bwd(dln2, x2, sh["ln2w"], mean2, rstd2, grads["mlp_ln.weight"], grads["mlp_ln.bias"],
+        dx2 = K.layernorm_bwd(dln2, x2, sh["ln2w"], mean2, rstd2, grads.vec("mlp_ln.weight", d), grads.vec("mlp_ln.bias", d),
                               dresidual=dx3)
         dxa = None
         if cross:
             # ---- cross attention: x2 = x1 + out(attn(q(ln(x1)), kv(xa)))
-            grads["cross_attn.out.weight"] = wg("cross_attn.out.weight", dx2, co)
-            grads["cross_attn.out.bias"] = bg("cross_attn.out.bias", dx2)
+            grads.linear("cross_attn.out", dx2, co)
             dco = linear_dgrad(dx2, sh["wco"])
             dqc = torch.empty_like(qc)
             dkvc = torch.empty_like(kvc)
             K.attention_bwd(qc, kvc[:, :d], kvc[:, d:], co, dco, lsec, B, H, T, Ta, dq=dqc, dk=dkvc[:, :d], dv=dkvc[:, d:])
-            grads["cross_attn.query.weight"] = wg("cross_attn.query.weight", dqc, lnc)
-            grads["cross_attn.query.bias"] = bg("cross_attn.query.bias", dqc)
-            dwkv = wg("cross_attn.kv.weight", dkvc, xa)     # [dWk; dWv] in one GEMM
-            if D is None:
-                grads["cross_attn.key.weight"], grads["cross_attn.value.weight"] = dwkv[:d], dwkv[d:]
-                grads["cross_attn.value.bias"] = bias_grad(dkvc, pool=pool, side=side)[d:]
-            else:
-                bias_grad(dkvc[:, d:], d, side=side, out=D["cross_attn.value.bias"])
+            grads.linear("cross_attn.query", dqc, lnc)
+            grads.linear("cross_attn.kv", dkvc, xa)         # [dWk; dWv] in one GEMM
             # d(loss)/d(xa): every decoder layer contributes one (B*1500, d) term.  Instead of 24 separate tensors that
             # autograd adds pairwise (23 elementwise kernels over 98 MB each at medium), the layers accumulate into ONE buffer
             # through the GEMM's residual epilogue (bf16(buf + bf16(acc)), the rounding autograd's bf16 adds would apply);
@@ -522,36 +556,23 @@ class _BlockFn(torch.autograd.Function):
                 st["left"] -= 1
                 dxa = buf if st["left"] == 0 else None
             dlnc = linear_dgrad(dqc, sh["wcq"])
-            grads["cross_attn_ln.weight"], grads["cross_attn_ln.bias"] = vec("cross_attn_ln.weight"), vec("cross_attn_ln.bias")
-            dx1 = K.layernorm_bwd(dlnc, x1, sh["lncw"], meanc, rstdc, grads["cross_attn_ln.weight"],
-                                  grads["cross_attn_ln.bias"], dresidual=dx2)
+            dx1 = K.layernorm_bwd(dlnc, x1, sh["lncw"], meanc, rstdc, grads.vec("cross_attn_ln.weight", d),
+                                  grads.vec("cross_attn_ln.bias", d), dresidual=dx2)
         else:
             dx1 = dx2
         # ---- self attention: x1 = x + out(attn(qkv(ln(x))))
-        grads["attn.out.weight"] = wg("attn.out.weight", dx1, ao)
-        grads["attn.out.bias"] = bg("attn.out.bias", dx1)
+        grads.linear("attn.out", dx1, ao)
         dao = linear_dgrad(dx1, sh["wo"])
         dqkv = torch.empty_like(qkv)
         K.attention_bwd(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ao, dao, lse, B, H, T, T, causal=causal, kv_len=kv_len,
                         dq=dqkv[:, :d], dk=dqkv[:, d:2 * d], dv=dqkv[:, 2 * d:])
-        dw = wg("attn.qkv.weight", dqkv, ln1)               # [dWq; dWk; dWv] in one GEMM
-        if D is None:
-            grads["attn.query.weight"], grads["attn.key.weight"], grads["attn.value.weight"] = dw[:d], dw[d:2 * d], dw[2 * d:]
-            db = bias_grad(dqkv, pool=pool, side=side)
-            grads["attn.query.bias"], grads["attn.value.bias"] = db[:d], db[2 * d:]
-        else:   # the key projection has no bias (model.py:259): its slot in the fused [bq; 0; bv] vector must stay zero
-            bias_grad(dqkv[:, :d], d, side=side, out=D["attn.query.bias"])
-            bias_grad(dqkv[:, 2 * d:], d, side=side, out=D["attn.value.bias"])
+        grads.linear("attn.qkv", dqkv, ln1)                 # [dWq; dWk; dWv] in one GEMM
         dln1 = linear_dgrad(dqkv, sh["wqkv"])
-        grads["attn_ln.weight"], grads["attn_ln.bias"] = vec("attn_ln.weight"), vec("attn_ln.bias")
-        dx = K.layernorm_bwd(dln1, x, sh["ln1w"], mean1, rstd1, grads["attn_ln.weight"], grads["attn_ln.bias"],
+        dx = K.layernorm_bwd(dln1, x, sh["ln1w"], mean1, rstd1, grads.vec("attn_ln.weight", d), grads.vec("attn_ln.bias", d),
                              dresidual=dx1)
         side.join()
-        if D is not None:
-            if blk._bwd_done_cb is not None:
-                blk._bwd_done_cb()      # gradient synchronisation hook: this block's slab range is final
-            return (None, None, None, None, None, None, None, dx, dxa, *([None] * len(blk._param_names)))
-        return (None, None, None, None, None, None, None, dx, dxa, *[grads[n] for n in blk._param_names])
+        grads.done()
+        return (None, None, None, None, None, None, None, dx, dxa, *grads.grads_for(blk._param_names))
 
 
 class ResidualAttentionBlock(nn.Module):
@@ -657,19 +678,16 @@ class _StemFn(torch.autograd.Function):
         A1, pre1, A2, pre2 = ctx.saved_tensors
         enc = ctx.enc
         B, C, T, T2, d = ctx.dims
-        D = enc._direct if (enc._direct is not None and enc._slabs.direct_grads) else None
+        grads = _GradDest(enc, dx0.device)
         dpre2 = K.gelu_bwd(dx0.contiguous(), pre2)
-        dw2 = K.unpermute_conv_wgrad(linear_wgrad(dpre2, A2), d, d, out=None if D is None else D["conv2.weight"])
-        db2 = bias_grad(dpre2, out=None if D is None else D["conv2.bias"])
+        grads.keep("conv2.weight", K.unpermute_conv_wgrad(linear_wgrad(dpre2, A2), d, d, out=grads.out("conv2.weight")))
+        grads.bias("conv2.bias", dpre2)
         dA2 = linear_dgrad(dpre2, enc.conv2.weight_bf16())
         dpre1 = K.col2im_conv2_gelu_bwd(dA2, pre1, B, T, T2, d)
-        dw1 = K.unpermute_conv_wgrad(linear_wgrad(dpre1, A1), d, C, out=None if D is None else D["conv1.weight"])
-        db1 = bias_grad(dpre1, out=None if D is None else D["conv1.bias"])
-        if D is not None:
-            if enc._bwd_done_cb is not None:
-                enc._bwd_done_cb()     # last gradients of the whole backward pass
-            return None, None, None, None, None, None
-        return None, None, dw1, db1, dw2, db2
+        grads.keep("conv1.weight", K.unpermute_conv_wgrad(linear_wgrad(dpre1, A1), d, C, out=grads.out("conv1.weight")))
+        grads.bias("conv1.bias", dpre1)
+        grads.done()     # last gradients of the whole backward pass
+        return (None, None, *grads.grads_for(("conv1.weight", "conv1.bias", "conv2.weight", "conv2.bias")))
 
 
 class AudioEncoder(nn.Module):
@@ -703,11 +721,10 @@ class AudioEncoder(nn.Module):
 
 
 class _LayerNormFn(torch.autograd.Function):
-    """Final LayerNorm of the encoder / decoder.  `owner._direct[key + ".weight" / ".bias"]` are the gradient-slab targets
-    in slab mode."""
+    """Final LayerNorm of the encoder / decoder, whose parameters are `owner`'s `key + ".weight"` / `key + ".bias"`."""
 
     @staticmethod
-    def forward(ctx, x, w, b, eps, owner=None, key=None):
+    def forward(ctx, x, w, b, eps, owner, key):
         y, mean, rstd = K.layernorm_fwd(x, _f32(w), _f32(b), eps)
         ctx.save_for_backward(x, w, mean, rstd)
         ctx.owner, ctx.key = owner, key
@@ -717,15 +734,10 @@ class _LayerNormFn(torch.autograd.Function):
     def backward(ctx, dy):
         x, w, mean, rstd = ctx.saved_tensors
         w = _f32(w)
-        owner = ctx.owner
-        D = owner._direct if (owner is not None and owner._direct is not None and owner._slabs.direct_grads) else None
-        if D is not None:
-            dx = K.layernorm_bwd(dy.contiguous(), x, w, mean, rstd, D[ctx.key + ".weight"], D[ctx.key + ".bias"])
-            return dx, None, None, None, None, None
-        dw = torch.zeros(w.shape, device=w.device, dtype=torch.float32)
-        db = torch.zeros(w.shape, device=w.device, dtype=torch.float32)
+        grads, names = _GradDest(ctx.owner, w.device), (ctx.key + ".weight", ctx.key + ".bias")
+        dw, db = grads.vec(names[0], w.shape), grads.vec(names[1], w.shape)
         dx = K.layernorm_bwd(dy.contiguous(), x, w, mean, rstd, dw, db)
-        return dx, dw, db, None, None, None
+        return (dx, *grads.grads_for(names), None, None, None)
 
 
 # =====================================================================================================
@@ -746,25 +758,13 @@ class _EmbedFn(torch.autograd.Function):
     def backward(ctx, dx):
         (ids,) = ctx.saved_tensors
         eshape, pshape, offset, padding_idx = ctx.meta
-        dec = ctx.dec
         pad = -1 if padding_idx is None else padding_idx
-        D = dec._direct if (dec is not None and dec._direct is not None and dec._slabs.direct_grads) else None
-        if D is not None:   # scatter-add straight into the slab (the tied logits wgrad already accumulated there)
-            K.embed_bwd(ids.contiguous(), dx.contiguous(), D["token_embedding.weight"], D["positional_embedding"][offset:], pad)
-            if dec._bwd_done_cb is not None:
-                dec._bwd_done_cb()     # decoder gradients (incl. the tied embedding) are final
-            return None, None, None, None, None, None
-        demb = torch.zeros(eshape, device=dx.device, dtype=torch.float32)
-        dpos = torch.zeros(pshape, device=dx.device, dtype=torch.float32)
+        grads, names = _GradDest(ctx.dec, dx.device), ("token_embedding.weight", "positional_embedding")
+        # in direct mode a scatter-add straight into the slab, where the tied logits wgrad has already accumulated
+        demb, dpos = grads.vec(names[0], eshape), grads.vec(names[1], pshape)
         K.embed_bwd(ids.contiguous(), dx.contiguous(), demb, dpos[offset:], pad)
-        return None, demb, dpos, None, None, None
-
-
-def _direct_of(mod):
-    """Gradient-slab targets of a module when the model runs in slab mode with direct gradients, else None."""
-    if mod is not None and mod._direct is not None and mod._slabs.direct_grads:
-        return mod._direct
-    return None
+        grads.done()     # decoder gradients (incl. the tied embedding) are final
+        return (None, *grads.grads_for(names), None, None, None)
 
 
 def _logits_ld(V: int) -> int:
@@ -792,9 +792,9 @@ class _LogitsFn(torch.autograd.Function):
         buf = torch.empty((M, _logits_ld(V)), device=x.device, dtype=torch.bfloat16)
         buf[:, :V].copy_(dlogits)  # `.float()` backward: the gradient enters the matmul as bf16
         dx = K.gemm(buf[:, :V], emb_bf16, M, d, V, b_mn=True, block_n=_pick_block_n(M, d))
-        D = _direct_of(ctx.dec)
-        demb = linear_wgrad(buf, x, n_valid=V, out=None if D is None else D["token_embedding.weight"])
-        return dx, (None if D is not None else demb), None, None
+        grads = _GradDest(ctx.dec)
+        grads.weight("token_embedding.weight", buf, x, n_valid=V)
+        return (dx, *grads.grads_for(("token_embedding.weight",)), None, None)
 
 
 class _LossHeadFn(torch.autograd.Function):
@@ -827,9 +827,9 @@ class _LossHeadFn(torch.autograd.Function):
         ctx.consumed[0] = True
         K.ce_bwd_(buf, t, lse, lsc, dloss.reshape(1).float().contiguous(), V, ignore_index)
         dx = K.gemm(buf[:, :V], emb_bf16, M, d, V, b_mn=True, block_n=_pick_block_n(M, d))
-        D = _direct_of(ctx.dec)
-        demb = linear_wgrad(buf, x, n_valid=V, out=None if D is None else D["token_embedding.weight"])
-        return dx, (None if D is not None else demb), None, None, None, None
+        grads = _GradDest(ctx.dec)
+        grads.weight("token_embedding.weight", buf, x, n_valid=V)
+        return (dx, *grads.grads_for(("token_embedding.weight",)), None, None, None, None)
 
 
 class TextDecoder(nn.Module):
@@ -951,41 +951,32 @@ class OLMoASRBase(nn.Module):
         sl = ParamSlabs(self, layout)
         sl.direct_grads = direct_grads
 
-        def install_mha(a: "MultiHeadAttention", direct: Dict[str, Tensor], prefix: str, cross: bool):
+        def install_mha(a: "MultiHeadAttention"):
             d = a.query.weight.shape[0]
             assert sl.adjacent(a.query.weight, a.key.weight, a.value.weight)
             assert sl.offset[id(a.value.bias)] == sl.offset[id(a.query.bias)] + 2 * d
             a._slab_fused = (sl.span("S", a.query.weight, 3 * d * d).view(3 * d, d), sl.span("P", a.query.bias, 3 * d))
             for lin in (a.query, a.key, a.value, a.out):
                 lin._slab_view = sl.shadow(lin.weight)
-            direct[prefix + ".out.weight"], direct[prefix + ".out.bias"] = sl.grad(a.out.weight), sl.grad(a.out.bias)
-            direct[prefix + ".query.bias"], direct[prefix + ".value.bias"] = sl.grad(a.query.bias), sl.grad(a.value.bias)
-            if cross:
-                direct[prefix + ".query.weight"] = sl.grad(a.query.weight)
-                direct[prefix + ".kv.weight"] = sl.span("G", a.key.weight, 2 * d * d).view(2 * d, d)
-            else:
-                direct[prefix + ".qkv.weight"] = sl.span("G", a.query.weight, 3 * d * d).view(3 * d, d)
+
+        def grad_views(mod: nn.Module) -> Dict[str, Tensor]:   # the gradients its own backward writes, by name
+            return {n: sl.grad(p) for n, p in mod.named_parameters() if not n.startswith("blocks.")}
 
         for b in list(enc.blocks) + list(dec.blocks):
-            direct: Dict[str, Tensor] = {}
-            install_mha(b.attn, direct, "attn", cross=False)
+            install_mha(b.attn)
             if b.cross_attn is not None:
-                install_mha(b.cross_attn, direct, "cross_attn", cross=True)
-            for name, lin in (("mlp.0", b.mlp[0]), ("mlp.2", b.mlp[2])):
+                install_mha(b.cross_attn)
+            for lin in (b.mlp[0], b.mlp[2]):
                 lin._slab_view = sl.shadow(lin.weight)
-                direct[name + ".weight"], direct[name + ".bias"] = sl.grad(lin.weight), sl.grad(lin.bias)
-            for name, ln in (("attn_ln", b.attn_ln), ("cross_attn_ln", b.cross_attn_ln), ("mlp_ln", b.mlp_ln)):
-                if ln is not None:
-                    direct[name + ".weight"], direct[name + ".bias"] = sl.grad(ln.weight), sl.grad(ln.bias)
+            direct = grad_views(b)
+            for name, members in _FUSED.items():     # a fused weight gradient is the slab span of its adjacent members
+                if members[0] + ".weight" in direct:
+                    w = _attr_by_path(b, members[0]).weight
+                    direct[name + ".weight"] = sl.span("G", w, len(members) * w.numel()).view(len(members) * w.shape[0], -1)
             sh = b._build_shadows()      # slab views throughout: bf16 weights from S, fp32 vectors from P
             b._slabs, b._slab_sh, b._direct = sl, sh, direct
         enc._slabs, dec._slabs = sl, sl
-        enc._direct = {"conv1.weight": sl.grad(enc.conv1.weight), "conv1.bias": sl.grad(enc.conv1.bias),
-                       "conv2.weight": sl.grad(enc.conv2.weight), "conv2.bias": sl.grad(enc.conv2.bias),
-                       "ln_post.weight": sl.grad(enc.ln_post.weight), "ln_post.bias": sl.grad(enc.ln_post.bias)}
-        dec._direct = {"token_embedding.weight": sl.grad(dec.token_embedding.weight),
-                       "positional_embedding": sl.grad(dec.positional_embedding),
-                       "ln.weight": sl.grad(dec.ln.weight), "ln.bias": sl.grad(dec.ln.bias)}
+        enc._direct, dec._direct = grad_views(enc), grad_views(dec)
         dec._emb_slab_view = sl.shadow(dec.token_embedding.weight)
         self._slabs = sl
         if sl.device.type == "cuda":

@@ -5,8 +5,6 @@ kernel is launched; the kernels themselves never allocate.
 """
 from __future__ import annotations
 
-import os
-
 import torch
 
 from . import _lib
@@ -117,29 +115,9 @@ def attention_fwd(q, k, v, B, H, Tq, Tkv, causal=False, kv_len=None, scale=None,
     return out, lse
 
 
-_BWD_PERSISTENT_USER = os.environ.get("OASR_BWD_PERSISTENT")   # an explicit setting of the user always wins
-
-
-def _choose_attention_bwd_mode(world_size=None):
-    """Launch-shape policy of the backward attention kernel, published as OASR_BWD_PERSISTENT: a persistent grid (one CTA
-    per SM walking over the work items) up to 2 GPUs, one CTA per work item beyond, where resident NCCL collectives take
-    SMs away and a statically partitioned persistent grid would run its displaced CTAs as a second wave.  The sm_90a
-    kernel (csrc/attention_bwd_sm90.cu) launches one CTA per work item in every job, which is the shape this policy asks
-    for under collectives; an explicit setting of the user always wins."""
-    if _BWD_PERSISTENT_USER is not None:
-        return
-    if world_size is None:
-        d = torch.distributed
-        world_size = d.get_world_size() if (d.is_available() and d.is_initialized()) else 1
-    want = "0" if world_size > 2 else "1"
-    if os.environ.get("OASR_BWD_PERSISTENT") != want:
-        os.environ["OASR_BWD_PERSISTENT"] = want
-
-
 def attention_bwd(q, k, v, o, dout, lse, B, H, Tq, Tkv, causal=False, kv_len=None, scale=None, dq=None, dk=None, dv=None):
     for t, n in ((q, "q"), (k, "k"), (v, "v"), (o, "o"), (dout, "dout")):
         _bf16_2d(t, n)
-    _choose_attention_bwd_mode()
     if scale is None:
         scale = 64 ** -0.5
     dev = q.device

@@ -194,17 +194,8 @@ def _ddp_worker(rank, world, port, out):
     dist.all_gather(gathered, g)
     t = torch.tensor([float(rank + 1) * 10.0])
     dist.all_reduce(t, op=dist.ReduceOp.MAX)   # bench.py: max-over-ranks step time
-    # the backward attention kernel's launch shape follows the size of the job (kernels.py explains why): persistent up to
-    # 2 ranks, one CTA per work item beyond
-    from olmoasr_b200 import kernels as K
-    os.environ.pop("OASR_BWD_PERSISTENT", None)
-    K._BWD_PERSISTENT_USER = None
-    K._choose_attention_bwd_mode()
-    bwd_mode = os.environ.get("OASR_BWD_PERSISTENT")
-    K._choose_attention_bwd_mode(world_size=8)
-    bwd_mode += os.environ.get("OASR_BWD_PERSISTENT")
     if rank == 0:
-        torch.save({"grads": gathered, "lens": lens, "tmax": float(t), "bwd_mode": bwd_mode}, out)
+        torch.save({"grads": gathered, "lens": lens, "tmax": float(t)}, out)
     dist.barrier()
     dist.destroy_process_group()
 
@@ -216,23 +207,6 @@ def test_data_parallel_semantics_world2_gloo(tmp_path):
     r = torch.load(out, weights_only=False)
     assert torch.allclose(r["grads"][0], r["grads"][1])           # gradients are averaged across ranks
     assert r["tmax"] == 20.0
-    assert r["bwd_mode"] == "10"      # 2 ranks: persistent; 8 ranks: one CTA per item
-    from olmoasr_b200 import kernels as K          # ... and persistent in a single-process job, unless the user said otherwise
-    saved, user = os.environ.pop("OASR_BWD_PERSISTENT", None), K._BWD_PERSISTENT_USER
-    try:
-        K._BWD_PERSISTENT_USER = None
-        K._choose_attention_bwd_mode()
-        assert os.environ["OASR_BWD_PERSISTENT"] == "1"
-        K._BWD_PERSISTENT_USER = "0"
-        os.environ["OASR_BWD_PERSISTENT"] = "0"
-        K._choose_attention_bwd_mode()
-        assert os.environ["OASR_BWD_PERSISTENT"] == "0"
-    finally:
-        K._BWD_PERSISTENT_USER = user
-        if saved is None:
-            os.environ.pop("OASR_BWD_PERSISTENT", None)
-        else:
-            os.environ["OASR_BWD_PERSISTENT"] = saved
     # ranks draw different shards
     a = synthetic.text_batch(3, rank=0)[0]
     b = synthetic.text_batch(3, rank=1)[0]
