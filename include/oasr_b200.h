@@ -245,6 +245,26 @@ typedef struct oasr_dec_sample_args {
 } oasr_dec_sample_args;
 OASR_API int oasr_dec_sample(const oasr_dec_sample_args* args, void* stream);
 
+/* The same step with ApplyTimestampRules and temperature sampling (whisper/decoding.py GreedyDecoder.update at any
+ * temperature with SuppressBlank, SuppressTokens and, when `timestamps`, ApplyTimestampRules; replaces the hook loop's
+ * per-row Python rules and `Categorical(logits=logits / temperature).sample()`), then *pos += 1.
+ * temperature: NULL for greedy (argmax), else a device scalar; at > 0 the next token is the Gumbel-max draw
+ * argmax_v logits_v / T + g_v over the allowed ids, with g_v from Philox4x32-10 keyed on row_keys[n] (device, one
+ * uint64 per row) and counted with (v / 4, *pos): a sample of softmax(filtered logits / T) that depends on (row key,
+ * position) only.  sum_logprobs collects log_softmax(filtered logits)[next] at temperature 1.  Temperature and keys are
+ * read on the device at every launch, so one captured graph serves every temperature and seed.
+ * scratch: (n_seq, n_slices, 48) f32; counters as for oasr_dec_sample.  max_initial_timestamp < 0: no initial limit.
+ * n_seq <= 64. */
+typedef struct oasr_dec_sample_rules_args {
+  const float* logits; int64_t ld_logits; int32_t* tokens; int64_t ld_tokens; int32_t* pos_ptr;
+  const uint8_t* suppress; float* sum_logprobs; float* no_speech_prob; int32_t* n_unfinished; int32_t* done_flag;
+  float* scratch; int32_t* counters; const float* temperature; const uint64_t* row_keys;
+  int32_t n_seq; int32_t n_vocab; int32_t sample_begin; int32_t sot_index; int32_t suppress_blank; int32_t blank;
+  int32_t eot; int32_t no_speech; int32_t n_slices;
+  int32_t timestamps; int32_t timestamp_begin; int32_t no_timestamps; int32_t max_initial_timestamp; int32_t reserved;
+} oasr_dec_sample_rules_args;
+OASR_API int oasr_dec_sample_rules(const oasr_dec_sample_rules_args* args, void* stream);
+
 /* Beam search step (whisper/decoding.py BeamSearchDecoder.update with SuppressBlank, SuppressTokens and, when
  * `timestamps`, ApplyTimestampRules) over n_clips x beam rows (row = clip * beam + j), after the logits head.
  *   oasr_dec_beam_candidates: per row the top beam + 1 log-probs after every filter -> scratch

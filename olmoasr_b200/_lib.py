@@ -57,6 +57,17 @@ class DecSampleArgs(ctypes.Structure):  # oasr_dec_sample_args
                 ("blank", c_i32), ("eot", c_i32), ("no_speech", c_i32), ("n_slices", c_i32), ("reserved", c_i32)]
 
 
+class DecSampleRulesArgs(ctypes.Structure):  # oasr_dec_sample_rules_args
+    _fields_ = [("logits", c_void_p), ("ld_logits", c_i64), ("tokens", c_void_p), ("ld_tokens", c_i64), ("pos_ptr", c_void_p),
+                ("suppress", c_void_p), ("sum_logprobs", c_void_p), ("no_speech_prob", c_void_p), ("n_unfinished", c_void_p),
+                ("done_flag", c_void_p), ("scratch", c_void_p), ("counters", c_void_p), ("temperature", c_void_p),
+                ("row_keys", c_void_p),
+                ("n_seq", c_i32), ("n_vocab", c_i32), ("sample_begin", c_i32), ("sot_index", c_i32), ("suppress_blank", c_i32),
+                ("blank", c_i32), ("eot", c_i32), ("no_speech", c_i32), ("n_slices", c_i32),
+                ("timestamps", c_i32), ("timestamp_begin", c_i32), ("no_timestamps", c_i32), ("max_initial_timestamp", c_i32),
+                ("reserved", c_i32)]
+
+
 class DecBeamArgs(ctypes.Structure):  # oasr_dec_beam_args
     _fields_ = [("logits", c_void_p), ("ld_logits", c_i64), ("tokens", c_void_p), ("ld_tokens", c_i64), ("pos_ptr", c_void_p),
                 ("suppress", c_void_p), ("sum_logprobs", c_void_p), ("no_speech_prob", c_void_p), ("n_unfinished", c_void_p),
@@ -111,6 +122,7 @@ _SIGNATURES = {
     "oasr_dec_linear": [ctypes.POINTER(DecLinearArgs), c_void_p],
     "oasr_dec_attention": [ctypes.POINTER(DecAttnArgs), c_void_p],
     "oasr_dec_sample": [ctypes.POINTER(DecSampleArgs), c_void_p],
+    "oasr_dec_sample_rules": [ctypes.POINTER(DecSampleRulesArgs), c_void_p],
     "oasr_dec_attention_grouped": [ctypes.POINTER(DecAttnArgs), c_int, c_void_p],
     "oasr_dec_beam_candidates": [ctypes.POINTER(DecBeamArgs), c_void_p],
     "oasr_dec_beam_select": [ctypes.POINTER(DecBeamArgs), c_void_p],
@@ -179,7 +191,7 @@ def stream():
 
 # kernels launched per entry point (memsets not counted) -- bench.py reports the total as `gpu_launches`
 _LAUNCHES_PER_CALL = {"oasr_logmel": 3, "oasr_attention_bwd": 3, "oasr_dec_attention": 2, "oasr_dec_sample": 2,
-                      "oasr_dec_attention_grouped": 2, "oasr_dec_beam_select": 2,
+                      "oasr_dec_sample_rules": 2, "oasr_dec_attention_grouped": 2, "oasr_dec_beam_select": 2,
                       "oasr_ce_fwd": 2, "oasr_colsum_bf16": 2, "oasr_layernorm_bwd": 3, "oasr_grad_sqnorm": 2,
                       "oasr_grad_sqnorm_flat": 2}
 LAUNCH_COUNT = 0

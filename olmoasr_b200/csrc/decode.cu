@@ -755,108 +755,293 @@ __global__ void __launch_bounds__(128) dec_attn_fused_kernel(const oasr_dec_attn
 }
 
 // ---------------------------------------------------------------------------------------------------------- sampling
+constexpr int BEAM_SCR = 48;                // floats of scratch per (row, slice): rule-aware sampling and beam candidates
+
+// Per-row logit filter of one step (every rule an index test): SuppressTokens, SuppressBlank and, with `ts_on`,
+// ApplyTimestampRules.  Used by the sampling step and by beam search.
+struct BeamFilter {
+  const uint8_t* suppress;
+  int first, blank_eot, eot, blank;
+  int ts_on, no_ts, ts_begin;
+  int ban_text, ban_below_eot;     // ban [0, ts_begin) / ban [0, eot)
+  int ts_lo, ts_hi;                // allowed timestamps: [ts_lo, ts_hi)
+  __device__ __forceinline__ bool banned(int v) const {
+    if (suppress[v]) return true;
+    if (blank_eot && (v == blank || v == eot)) return true;
+    if (!ts_on) return false;
+    if (v == no_ts) return true;
+    if (v < ts_begin) return ban_text || (ban_below_eot && v < eot);
+    return v < ts_lo || v >= ts_hi;
+  }
+};
+
+// The filter of row `trow` at position `pos`.  With timestamps on, every thread of the block must call it (block-wide
+// reduction over the row's history; s_red holds one int per warp).
+__device__ BeamFilter beam_filter(const uint8_t* suppress, const int32_t* trow, int pos, int sample_begin, int suppress_blank,
+                                  int blank, int eot, int timestamps, int timestamp_begin, int no_timestamps,
+                                  int max_initial_timestamp, int n_vocab, int* s_red) {
+  BeamFilter f;
+  f.suppress = suppress;
+  f.first = pos == sample_begin - 1;
+  f.blank_eot = f.first && suppress_blank;
+  f.eot = eot; f.blank = blank;
+  f.ts_on = timestamps; f.no_ts = no_timestamps; f.ts_begin = timestamp_begin;
+  f.ban_text = 0; f.ban_below_eot = 0; f.ts_lo = timestamp_begin; f.ts_hi = n_vocab;
+  if (!timestamps) return f;
+  // ApplyTimestampRules over seq = tokens[sample_begin .. pos]: the last timestamp (block max over positions)
+  int last = -1;
+  for (int p = sample_begin + threadIdx.x; p <= pos; p += blockDim.x)
+    if (trow[p] >= timestamp_begin) last = p;
+  last = __reduce_max_sync(0xffffffffu, last);
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = last;
+  __syncthreads();
+  last = -1;
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) last = max(last, s_red[w]);
+  __syncthreads();
+  const int len = pos + 1 - sample_begin;
+  const bool last_ts = len >= 1 && trow[pos] >= timestamp_begin;
+  const bool penult_ts = len < 2 || trow[pos - 1] >= timestamp_begin;
+  if (last_ts) {
+    if (penult_ts) f.ts_lo = n_vocab;          // a timestamp pair is closed: text must follow
+    else f.ban_below_eot = 1;                  // an open timestamp: another timestamp or eot
+  }
+  if (last >= 0) {                             // timestamps never decrease (strictly increase after a closed pair)
+    const int t = trow[last];
+    f.ts_lo = max(f.ts_lo, (last_ts && !penult_ts) ? t : t + 1);
+  }
+  if (len == 0) {                              // the first sampled token is a timestamp, within the initial window
+    f.ban_text = 1;
+    if (max_initial_timestamp >= 0) f.ts_hi = min(f.ts_hi, timestamp_begin + max_initial_timestamp + 1);
+  }
+  return f;
+}
+
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011): 4 x 32 random bits per
+// (counter, key).  The sampler keys it on the row's 64-bit stream key and counts with (vocabulary id / 4, position).
+__device__ __forceinline__ uint4 philox4x32_10(uint32_t c0, uint32_t c1, uint32_t k0, uint32_t k1) {
+  uint32_t c2 = 0, c3 = 0;
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r > 0) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
+    c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+  }
+  return make_uint4(c0, c1, c2, c3);
+}
+__device__ __forceinline__ uint32_t word_of(const uint4& r, int i) { return i == 0 ? r.x : i == 1 ? r.y : i == 2 ? r.z : r.w; }
+// Gumbel(0, 1) from 23 random bits: u = (k + 1/2) / 2^23 lies in (0, 1) and is exact in fp32; g = -log(-log u)
+__device__ __forceinline__ float gumbel(uint32_t bits) {
+  const float u = (__uint2float_rn(bits >> 9) + 0.5f) * 0x1p-23f;
+  return -logf(-logf(u));
+}
+
 // `n_slices` blocks per sequence, each over a contiguous slice of its fp32 logits row, one online pass with 16-byte loads
-// (whisper/decoding.py: SuppressBlank, SuppressTokens, GreedyDecoder.update); the block that arrives last at the sequence's
-// counter merges the slices in slice order (deterministic) and does the bookkeeping:
+// (whisper/decoding.py: SuppressBlank, SuppressTokens, ApplyTimestampRules, GreedyDecoder.update); the block that arrives
+// last at the sequence's counter merges the slices in slice order (deterministic) and does the bookkeeping:
 //   * at pos == sot_index: no_speech_prob = softmax(raw logits)[no_speech]                       (DecodingTask._main_loop)
 //   * suppress[v] != 0 -> -inf; at the first sampled position also `blank` and `eot`            (SuppressTokens / SuppressBlank)
-//   * next = argmax (lowest index on ties); logprob = logit[next] - logsumexp(filtered row)
+//   * TS: every timestamp rule as an index test (BeamFilter), and "timestamp mass beats every text token": the text
+//     region [0, timestamp_begin) and the timestamp region keep separate statistics, so lse(ts) > max(text) (both
+//     sides share one normaliser: raw logits compare) is decided after the merge, without a second pass
+//   * next = argmax (lowest index on ties), or with SAMPLING and *temperature > 0 the Gumbel-max draw
+//     argmax_v x_v / T + g_v (lowest index on ties), a sample of softmax(filtered / T) (Categorical(logits / T).sample())
+//   * logprob = logit[next] - logsumexp(filtered row) at temperature 1 (GreedyDecoder.update)
 //   * sum_logprobs += logprob unless the previous token is eot; rows whose previous token is eot keep emitting eot
-// Positions before sample_begin - 1 are teacher-forced: nothing is written there.
-struct SampleAcc {          // online (max, sum exp) of the raw and the filtered row + filtered argmax
-  float mraw, sraw, mf, sf;
-  int arg;
+// Positions before sample_begin - 1 are teacher-forced: nothing is written there.  The draw of row n at position p is a
+// function of (row_keys[n], p, vocabulary id) only: not of the slice split, the block order or the row's batch slot.
+struct RegionAcc {          // one vocabulary region: online (max, sum exp) of the filtered row, its argmax, best Gumbel draw
+  float m, s, g;
+  int arg, gid;
 };
-__device__ __forceinline__ void acc_raw(SampleAcc& s, float x) {
+template <int NR>
+struct SampleAcc {          // raw (max, sum exp) + the regions (the whole row, or text | timestamps)
+  float mraw, sraw;
+  RegionAcc r[NR];
+};
+template <int NR>
+__device__ __forceinline__ void acc_init(SampleAcc<NR>& s, int V) {
+  s.mraw = -INFINITY; s.sraw = 0.f;
+#pragma unroll
+  for (int q = 0; q < NR; ++q) s.r[q] = RegionAcc{-INFINITY, 0.f, -INFINITY, V, V};
+}
+template <int NR>
+__device__ __forceinline__ void acc_raw(SampleAcc<NR>& s, float x) {
   if (x > s.mraw) { s.sraw = s.sraw * expf(s.mraw - x) + 1.f; s.mraw = x; }
   else s.sraw += expf(x - s.mraw);
 }
-__device__ __forceinline__ void acc_filt(SampleAcc& s, float x, int v) {
-  if (x > s.mf) { s.sf = s.sf * expf(s.mf - x) + 1.f; s.mf = x; s.arg = v; }
-  else { s.sf += expf(x - s.mf); if (x == s.mf && v < s.arg) s.arg = v; }
+__device__ __forceinline__ void acc_filt(RegionAcc& s, float x, int v) {
+  if (x > s.m) { s.s = s.s * expf(s.m - x) + 1.f; s.m = x; s.arg = v; }
+  else { s.s += expf(x - s.m); if (x == s.m && v < s.arg) s.arg = v; }
 }
-__device__ __forceinline__ SampleAcc acc_merge(const SampleAcc& a, const SampleAcc& b) {
-  SampleAcc r;
-  r.mraw = fmaxf(a.mraw, b.mraw);
-  r.sraw = (r.mraw == -INFINITY) ? 0.f : a.sraw * expf(a.mraw - r.mraw) + b.sraw * expf(b.mraw - r.mraw);
-  r.mf = fmaxf(a.mf, b.mf);
-  r.sf = (r.mf == -INFINITY) ? 0.f : a.sf * expf(a.mf - r.mf) + b.sf * expf(b.mf - r.mf);
-  r.arg = (a.mf > b.mf || (a.mf == b.mf && a.arg < b.arg)) ? a.arg : b.arg;
+__device__ __forceinline__ void acc_draw(RegionAcc& s, float y, int v) {
+  if (y > s.g || (y == s.g && v < s.gid)) { s.g = y; s.gid = v; }
+}
+template <bool SAMPLING>
+__device__ __forceinline__ RegionAcc region_merge(const RegionAcc& a, const RegionAcc& b) {
+  RegionAcc r;
+  r.m = fmaxf(a.m, b.m);
+  r.s = (r.m == -INFINITY) ? 0.f : a.s * expf(a.m - r.m) + b.s * expf(b.m - r.m);
+  r.arg = (a.m > b.m || (a.m == b.m && a.arg < b.arg)) ? a.arg : b.arg;
+  if constexpr (SAMPLING) {
+    const bool ta = a.g > b.g || (a.g == b.g && a.gid < b.gid);
+    r.g = ta ? a.g : b.g; r.gid = ta ? a.gid : b.gid;
+  } else {
+    r.g = -INFINITY; r.gid = a.gid;
+  }
   return r;
 }
+template <int NR, bool SAMPLING>
+__device__ __forceinline__ SampleAcc<NR> acc_merge(const SampleAcc<NR>& a, const SampleAcc<NR>& b) {
+  SampleAcc<NR> r;
+  r.mraw = fmaxf(a.mraw, b.mraw);
+  r.sraw = (r.mraw == -INFINITY) ? 0.f : a.sraw * expf(a.mraw - r.mraw) + b.sraw * expf(b.mraw - r.mraw);
+#pragma unroll
+  for (int q = 0; q < NR; ++q) r.r[q] = region_merge<SAMPLING>(a.r[q], b.r[q]);
+  return r;
+}
+template <bool SAMPLING>
+constexpr int region_floats() { return SAMPLING ? 5 : 3; }
+template <int NR, bool SAMPLING>
+__device__ __forceinline__ void acc_store(const SampleAcc<NR>& s, float* out) {   // [mraw, sraw, per region m, s, arg (, g, gid)]
+  out[0] = s.mraw; out[1] = s.sraw;
+#pragma unroll
+  for (int q = 0; q < NR; ++q) {
+    float* o = out + 2 + q * region_floats<SAMPLING>();
+    o[0] = s.r[q].m; o[1] = s.r[q].s; o[2] = __int_as_float(s.r[q].arg);
+    if constexpr (SAMPLING) { o[3] = s.r[q].g; o[4] = __int_as_float(s.r[q].gid); }
+  }
+}
+template <int NR, bool SAMPLING>
+__device__ __forceinline__ SampleAcc<NR> acc_load(const volatile float* in, int V) {
+  SampleAcc<NR> s;
+  acc_init(s, V);
+  s.mraw = in[0]; s.sraw = in[1];
+#pragma unroll
+  for (int q = 0; q < NR; ++q) {
+    const volatile float* p = in + 2 + q * region_floats<SAMPLING>();
+    s.r[q].m = p[0]; s.r[q].s = p[1]; s.r[q].arg = __float_as_int(p[2]);
+    if constexpr (SAMPLING) { s.r[q].g = p[3]; s.r[q].gid = __float_as_int(p[4]); }
+  }
+  return s;
+}
+template <int NR, bool SAMPLING>
+__device__ __forceinline__ SampleAcc<NR> acc_shfl(const SampleAcc<NR>& s, int o) {
+  SampleAcc<NR> t;
+  t.mraw = __shfl_xor_sync(0xffffffffu, s.mraw, o); t.sraw = __shfl_xor_sync(0xffffffffu, s.sraw, o);
+#pragma unroll
+  for (int q = 0; q < NR; ++q) {
+    t.r[q].m = __shfl_xor_sync(0xffffffffu, s.r[q].m, o); t.r[q].s = __shfl_xor_sync(0xffffffffu, s.r[q].s, o);
+    t.r[q].arg = __shfl_xor_sync(0xffffffffu, s.r[q].arg, o);
+    if constexpr (SAMPLING) {
+      t.r[q].g = __shfl_xor_sync(0xffffffffu, s.r[q].g, o); t.r[q].gid = __shfl_xor_sync(0xffffffffu, s.r[q].gid, o);
+    } else {
+      t.r[q].g = -INFINITY; t.r[q].gid = s.r[q].gid;
+    }
+  }
+  return t;
+}
 
-__global__ void __launch_bounds__(256) dec_sample_kernel(const oasr_dec_sample_args a) {
-  __shared__ SampleAcc s_acc[8];
+// <false, false> is greedy decoding without timestamps (oasr_dec_sample, 8 floats of scratch per slice); the other
+// instantiations serve oasr_dec_sample_rules (BEAM_SCR floats per slice).
+template <bool TS, bool SAMPLING>
+__global__ void __launch_bounds__(256) dec_sample_kernel(const oasr_dec_sample_rules_args a) {
+  constexpr int NR = TS ? 2 : 1;
+  constexpr int SCR = (TS || SAMPLING) ? BEAM_SCR : 8;
+  static_assert(2 + NR * region_floats<SAMPLING>() <= SCR, "sampling scratch");
+  __shared__ SampleAcc<NR> s_acc[8];
   __shared__ int s_last;
+  __shared__ int s_red[8];
   pdl_launch_dependents();
   pdl_wait();
   const int slice = blockIdx.x, n = blockIdx.y, S = gridDim.x;
   const int pos = *a.pos_ptr;
   const float* row = a.logits + static_cast<int64_t>(n) * a.ld_logits;
+  const int32_t* trow = a.tokens + static_cast<int64_t>(n) * a.ld_tokens;
   const int V = a.n_vocab;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const bool first = (pos == a.sample_begin - 1);
   const bool sampling = pos >= a.sample_begin - 1;
   const bool want_raw = (pos == a.sot_index);
   if (!sampling && !want_raw) return;
+  const BeamFilter f = beam_filter(a.suppress, trow, pos, a.sample_begin, a.suppress_blank, a.blank, a.eot, TS ? 1 : 0,
+                                   a.timestamp_begin, a.no_timestamps, a.max_initial_timestamp, V, s_red);
+  float temp = 0.f;
+  uint32_t k0 = 0, k1 = 0;
+  if constexpr (SAMPLING) {
+    temp = *a.temperature;
+    const uint64_t key = a.row_keys[n];
+    k0 = static_cast<uint32_t>(key); k1 = static_cast<uint32_t>(key >> 32);
+  }
+  const bool draw = SAMPLING && temp > 0.f;
 
   const int per = ((V + S - 1) / S + 3) & ~3;                  // slice length, a multiple of 4 (16-byte loads)
   const int v0 = slice * per, v1 = min(V, v0 + per);
-  SampleAcc acc{-INFINITY, 0.f, -INFINITY, 0.f, V};
+  SampleAcc<NR> acc;
+  acc_init(acc, V);
   const bool vec_ok = ((reinterpret_cast<uintptr_t>(row) & 15) == 0);
-  auto visit = [&](float x, int v) {
-    acc_raw(acc, x);
-    const bool sup = a.suppress[v] != 0 || (first && a.suppress_blank && (v == a.blank || v == a.eot));
-    if (!sup) acc_filt(acc, x, v);
+  auto visit = [&](float x, int v, uint32_t bits) {
+    if (want_raw) acc_raw(acc, x);
+    if (!sampling || f.banned(v)) return;
+    auto add = [&](RegionAcc& r) {
+      acc_filt(r, x, v);
+      if constexpr (SAMPLING) { if (draw) acc_draw(r, x / temp + gumbel(bits), v); }
+    };
+    if constexpr (TS) { if (v >= f.ts_begin) { add(acc.r[NR - 1]); return; } }   // compile-time indices: registers
+    add(acc.r[0]);
+  };
+  auto bits_of = [&](int v) -> uint4 {      // the random words of the 4-id group holding v (only drawn when sampling)
+    return draw ? philox4x32_10(static_cast<uint32_t>(v >> 2), static_cast<uint32_t>(pos), k0, k1) : make_uint4(0, 0, 0, 0);
   };
   if (vec_ok) {
     for (int v = v0 + threadIdx.x * 4; v < v1; v += 256 * 4) {
       if (v + 4 <= v1) {
         const float4 x = *reinterpret_cast<const float4*>(row + v);
-        visit(x.x, v); visit(x.y, v + 1); visit(x.z, v + 2); visit(x.w, v + 3);
+        const uint4 b = bits_of(v);
+        visit(x.x, v, b.x); visit(x.y, v + 1, b.y); visit(x.z, v + 2, b.z); visit(x.w, v + 3, b.w);
       } else {
-        for (int u = v; u < v1; ++u) visit(row[u], u);
+        for (int u = v; u < v1; ++u) visit(row[u], u, word_of(bits_of(u), u & 3));
       }
     }
   } else {
-    for (int v = v0 + threadIdx.x; v < v1; v += 256) visit(row[v], v);
+    for (int v = v0 + threadIdx.x; v < v1; v += 256) visit(row[v], v, word_of(bits_of(v), v & 3));
   }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    SampleAcc other;
-    other.mraw = __shfl_xor_sync(0xffffffffu, acc.mraw, o); other.sraw = __shfl_xor_sync(0xffffffffu, acc.sraw, o);
-    other.mf = __shfl_xor_sync(0xffffffffu, acc.mf, o); other.sf = __shfl_xor_sync(0xffffffffu, acc.sf, o);
-    other.arg = __shfl_xor_sync(0xffffffffu, acc.arg, o);
-    acc = acc_merge(acc, other);
-  }
+  for (int o = 16; o > 0; o >>= 1) acc = acc_merge<NR, SAMPLING>(acc, acc_shfl<NR, SAMPLING>(acc, o));
   if (lane == 0) s_acc[warp] = acc;
   __syncthreads();
   if (threadIdx.x == 0) {
-    SampleAcc t = s_acc[0];
-    for (int w = 1; w < 8; ++w) t = acc_merge(t, s_acc[w]);
-    float* out = a.scratch + (static_cast<int64_t>(n) * S + slice) * 8;
-    out[0] = t.mraw; out[1] = t.sraw; out[2] = t.mf; out[3] = t.sf; out[4] = __int_as_float(t.arg);
+    SampleAcc<NR> t = s_acc[0];
+    for (int w = 1; w < 8; ++w) t = acc_merge<NR, SAMPLING>(t, s_acc[w]);
+    acc_store<NR, SAMPLING>(t, a.scratch + (static_cast<int64_t>(n) * S + slice) * SCR);
     __threadfence();
     s_last = (atomicAdd(a.counters + n, 1) == S - 1) ? 1 : 0;
   }
   __syncthreads();
   if (!s_last || threadIdx.x != 0) return;
   __threadfence();
-  SampleAcc t{-INFINITY, 0.f, -INFINITY, 0.f, V};
-  for (int sl = 0; sl < S; ++sl) {       // slice order: the result does not depend on which block arrived last
-    const volatile float* in = a.scratch + (static_cast<int64_t>(n) * S + sl) * 8;
-    SampleAcc p;
-    p.mraw = in[0]; p.sraw = in[1]; p.mf = in[2]; p.sf = in[3]; p.arg = __float_as_int(in[4]);
-    t = acc_merge(t, p);
-  }
+  SampleAcc<NR> t;
+  acc_init(t, V);
+  for (int sl = 0; sl < S; ++sl)         // slice order: the result does not depend on which block arrived last
+    t = acc_merge<NR, SAMPLING>(t, acc_load<NR, SAMPLING>(a.scratch + (static_cast<int64_t>(n) * S + sl) * SCR, V));
   a.counters[n] = 0;                     // re-armed for the next step
   if (want_raw) a.no_speech_prob[n] = expf(row[a.no_speech] - t.mraw) / t.sraw;
   if (sampling) {
-    const int prev = a.tokens[static_cast<int64_t>(n) * a.ld_tokens + pos];
+    RegionAcc c = t.r[0];
+    if constexpr (TS) {                  // timestamp mass beats every text token: only timestamps remain
+      const RegionAcc& ts = t.r[1];
+      const float lse_ts = ts.m == -INFINITY ? -INFINITY : ts.m + logf(ts.s);
+      c = (lse_ts > t.r[0].m) ? ts : region_merge<SAMPLING>(t.r[0], ts);
+    }
+    int pick = c.arg;
+    float logprob = -logf(c.s);          // logit[arg] - (m + log sum exp(x - m)), logit[arg] == m
+    if (draw && c.gid < V) {
+      pick = c.gid;
+      logprob = (row[pick] - c.m) - logf(c.s);
+    }
+    const int prev = trow[pos];
     const bool finished = (prev == a.eot);
-    const float logprob = -logf(t.sf);            // logit[arg] - (mf + log sum exp(x - mf)), logit[arg] == mf
     if (!finished) a.sum_logprobs[n] += logprob;
-    const int next = finished ? a.eot : t.arg;
+    const int next = finished ? a.eot : pick;
     a.tokens[static_cast<int64_t>(n) * a.ld_tokens + pos + 1] = next;
     if (next != a.eot) atomicAdd(a.n_unfinished, 1);
   }
@@ -887,7 +1072,6 @@ __global__ void dec_advance_kernel(int32_t* pos_ptr, int32_t* n_unfinished, int3
 // over dict insertion order.  No float atomics: the result is the same on every run.
 constexpr int BEAM_MAX = 8;
 constexpr int BEAM_K = BEAM_MAX + 1;        // candidates per row: beam + 1
-constexpr int BEAM_SCR = 48;                // floats of scratch per (row, slice)
 constexpr int BEAM_TOK_MAX = 456;           // staged token row length (n_text_ctx + 2 <= this)
 
 __device__ __forceinline__ bool cand_better(float x, int i, float y, int j) { return x > y || (x == y && i < j); }
@@ -931,60 +1115,6 @@ struct Lse {   // online (max, sum exp(x - max)); -inf entries add nothing
   __device__ __forceinline__ float lse() const { return m == -INFINITY ? -INFINITY : m + logf(s); }
 };
 
-// Per-row logit filter of one step (every rule an index test).
-struct BeamFilter {
-  const uint8_t* suppress;
-  int first, blank_eot, eot, blank;
-  int ts_on, no_ts, ts_begin;
-  int ban_text, ban_below_eot;     // ban [0, ts_begin) / ban [0, eot)
-  int ts_lo, ts_hi;                // allowed timestamps: [ts_lo, ts_hi)
-  __device__ __forceinline__ bool banned(int v) const {
-    if (suppress[v]) return true;
-    if (blank_eot && (v == blank || v == eot)) return true;
-    if (!ts_on) return false;
-    if (v == no_ts) return true;
-    if (v < ts_begin) return ban_text || (ban_below_eot && v < eot);
-    return v < ts_lo || v >= ts_hi;
-  }
-};
-
-__device__ BeamFilter beam_filter(const oasr_dec_beam_args& a, const int32_t* trow, int pos, int* s_red) {
-  BeamFilter f;
-  f.suppress = a.suppress;
-  f.first = pos == a.sample_begin - 1;
-  f.blank_eot = f.first && a.suppress_blank;
-  f.eot = a.eot; f.blank = a.blank;
-  f.ts_on = a.timestamps; f.no_ts = a.no_timestamps; f.ts_begin = a.timestamp_begin;
-  f.ban_text = 0; f.ban_below_eot = 0; f.ts_lo = a.timestamp_begin; f.ts_hi = a.n_vocab;
-  if (!a.timestamps) return f;
-  // ApplyTimestampRules over seq = tokens[sample_begin .. pos]: the last timestamp (block max over positions)
-  int last = -1;
-  for (int p = a.sample_begin + threadIdx.x; p <= pos; p += blockDim.x)
-    if (trow[p] >= a.timestamp_begin) last = p;
-  last = __reduce_max_sync(0xffffffffu, last);
-  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = last;
-  __syncthreads();
-  last = -1;
-  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) last = max(last, s_red[w]);
-  __syncthreads();
-  const int len = pos + 1 - a.sample_begin;
-  const bool last_ts = len >= 1 && trow[pos] >= a.timestamp_begin;
-  const bool penult_ts = len < 2 || trow[pos - 1] >= a.timestamp_begin;
-  if (last_ts) {
-    if (penult_ts) f.ts_lo = a.n_vocab;        // a timestamp pair is closed: text must follow
-    else f.ban_below_eot = 1;                  // an open timestamp: another timestamp or eot
-  }
-  if (last >= 0) {                             // timestamps never decrease (strictly increase after a closed pair)
-    const int t = trow[last];
-    f.ts_lo = max(f.ts_lo, (last_ts && !penult_ts) ? t : t + 1);
-  }
-  if (len == 0) {                              // the first sampled token is a timestamp, within the initial window
-    f.ban_text = 1;
-    if (a.max_initial_timestamp >= 0) f.ts_hi = min(f.ts_hi, a.timestamp_begin + a.max_initial_timestamp + 1);
-  }
-  return f;
-}
-
 __global__ void __launch_bounds__(256) dec_beam_cand_kernel(const oasr_dec_beam_args a) {
   __shared__ int s_red[8];
   __shared__ float s_f[8][2];
@@ -1000,7 +1130,8 @@ __global__ void __launch_bounds__(256) dec_beam_cand_kernel(const oasr_dec_beam_
   const float* row = a.logits + static_cast<int64_t>(n) * a.ld_logits;
   const int32_t* trow = a.tokens + static_cast<int64_t>(n) * a.ld_tokens;
   const int V = a.n_vocab, K = a.beam + 1;
-  const BeamFilter f = beam_filter(a, trow, pos, s_red);
+  const BeamFilter f = beam_filter(a.suppress, trow, pos, a.sample_begin, a.suppress_blank, a.blank, a.eot, a.timestamps,
+                                   a.timestamp_begin, a.no_timestamps, a.max_initial_timestamp, a.n_vocab, s_red);
   const int per = ((V + S - 1) / S + 3) & ~3;
   const int v0 = slice * per, v1 = min(V, v0 + per);
   Lse raw{-INFINITY, 0.f}, lt{-INFINITY, 0.f}, ls{-INFINITY, 0.f};
@@ -1388,9 +1519,37 @@ extern "C" int oasr_dec_sample(const oasr_dec_sample_args* a, void* stream) {
                    a->n_unfinished && a->done_flag, "dec_sample: null tensor");
   OASR_REQUIRE(a->n_seq >= 1 && a->n_vocab >= 1, "dec_sample: bad sizes");
   OASR_REQUIRE(a->scratch && a->counters && a->n_slices >= 1 && a->n_slices <= 64, "dec_sample: scratch / counters / 1 <= n_slices <= 64");
-  OASR_CUDA_OK(launch_pdl(dec_sample_kernel, dim3((unsigned)a->n_slices, (unsigned)a->n_seq), dim3(256), (cudaStream_t)stream, *a));
+  oasr_dec_sample_rules_args r = {};       // the rule-free, temperature-0 case of the rule-aware sampler
+  r.logits = a->logits; r.ld_logits = a->ld_logits; r.tokens = a->tokens; r.ld_tokens = a->ld_tokens; r.pos_ptr = a->pos_ptr;
+  r.suppress = a->suppress; r.sum_logprobs = a->sum_logprobs; r.no_speech_prob = a->no_speech_prob;
+  r.n_unfinished = a->n_unfinished; r.done_flag = a->done_flag; r.scratch = a->scratch; r.counters = a->counters;
+  r.n_seq = a->n_seq; r.n_vocab = a->n_vocab; r.sample_begin = a->sample_begin; r.sot_index = a->sot_index;
+  r.suppress_blank = a->suppress_blank; r.blank = a->blank; r.eot = a->eot; r.no_speech = a->no_speech; r.n_slices = a->n_slices;
+  OASR_CUDA_OK(launch_pdl(dec_sample_kernel<false, false>, dim3((unsigned)a->n_slices, (unsigned)a->n_seq), dim3(256),
+                          (cudaStream_t)stream, r));
   OASR_CUDA_OK(launch_pdl(dec_advance_kernel, dim3(1), dim3(1), (cudaStream_t)stream, a->pos_ptr, a->n_unfinished, a->done_flag,
                           (int)a->sample_begin));
+  return OASR_OK;
+}
+
+extern "C" int oasr_dec_sample_rules(const oasr_dec_sample_rules_args* a, void* stream) {
+  OASR_REQUIRE(a != nullptr && a->logits && a->tokens && a->pos_ptr && a->suppress && a->sum_logprobs && a->no_speech_prob &&
+                   a->n_unfinished && a->done_flag && a->scratch && a->counters, "dec_sample_rules: null tensor");
+  OASR_REQUIRE(a->n_seq >= 1 && a->n_seq <= 64 && a->n_vocab >= 1, "dec_sample_rules: 1 <= n_seq <= 64 (got %d)", a->n_seq);
+  OASR_REQUIRE(a->n_slices >= 1 && a->n_slices <= 64, "dec_sample_rules: 1 <= n_slices <= 64 (got %d)", a->n_slices);
+  OASR_REQUIRE(((uintptr_t)a->logits & 15) == 0 && (a->ld_logits % 4) == 0, "dec_sample_rules: logits rows must be 16-byte aligned");
+  OASR_REQUIRE(a->ld_tokens >= 1 && a->sample_begin >= 1, "dec_sample_rules: bad token layout");
+  OASR_REQUIRE(!a->timestamps || (a->timestamp_begin > a->eot && a->timestamp_begin < a->n_vocab),
+               "dec_sample_rules: bad timestamp_begin");
+  OASR_REQUIRE(a->temperature == nullptr || a->row_keys != nullptr, "dec_sample_rules: sampling needs row_keys");
+  const dim3 grid((unsigned)a->n_slices, (unsigned)a->n_seq);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool ts = a->timestamps != 0, draw = a->temperature != nullptr;
+  if (ts && draw) OASR_CUDA_OK(launch_pdl(dec_sample_kernel<true, true>, grid, dim3(256), st, *a));
+  else if (ts) OASR_CUDA_OK(launch_pdl(dec_sample_kernel<true, false>, grid, dim3(256), st, *a));
+  else if (draw) OASR_CUDA_OK(launch_pdl(dec_sample_kernel<false, true>, grid, dim3(256), st, *a));
+  else OASR_CUDA_OK(launch_pdl(dec_sample_kernel<false, false>, grid, dim3(256), st, *a));
+  OASR_CUDA_OK(launch_pdl(dec_advance_kernel, dim3(1), dim3(1), st, a->pos_ptr, a->n_unfinished, a->done_flag, (int)a->sample_begin));
   return OASR_OK;
 }
 

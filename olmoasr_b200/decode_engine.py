@@ -14,9 +14,13 @@ What the reference does per step and what replaces it:
   * 4 small matmul / softmax kernels per attention + separate LN, bias,
     GELU, residual kernels                                               -> 8-9 launches per layer (csrc/decode.cu), 100-112 per step (small)
 
-`beam_search` runs whisper/decoding.py's BeamSearchDecoder (with ApplyTimestampRules when asked) the same way: the step
-graph ends in a candidate kernel, a per-clip ranking kernel that keeps the finished lists on the device, and an in-place
-reorder of the self-attention cache; the beams of one clip share its cross-attention K / V (one projection per clip).
+`greedy(timestamps=True)` and `sample` (temperature sampling, best_of samples per clip) end the step graph in the
+rule-aware sampling kernel instead: ApplyTimestampRules as index tests and a Gumbel-max draw keyed per row, with the
+temperature and the keys read from device memory, so one graph per (rows, group size, timestamps) serves every
+temperature and seed.  `beam_search` runs whisper/decoding.py's BeamSearchDecoder (with ApplyTimestampRules when asked)
+the same way: the step graph ends in a candidate kernel, a per-clip ranking kernel that keeps the finished lists on the
+device, and an in-place reorder of the self-attention cache.  The beams (or the best_of samples) of one clip share its
+cross-attention K / V: one projection per clip.
 
 The activation dtype is fp16 (upstream default `fp16=True`) or bf16; the decoder-step kernels reproduce the reference's
 rounding points in that dtype.  The audio encoder and the cross K/V projection run on the bf16 wgmma kernels in both
@@ -32,14 +36,32 @@ import torch
 from torch import Tensor
 
 from . import _lib
-from ._lib import DTYPE_BF16, DTYPE_F16, DTYPE_F32, DecAttnArgs, DecBeamArgs, DecLinearArgs, DecSampleArgs, call, ptr, stream
+from ._lib import (DTYPE_BF16, DTYPE_F16, DTYPE_F32, DecAttnArgs, DecBeamArgs, DecLinearArgs, DecSampleArgs, DecSampleRulesArgs,
+                   call, ptr, stream)
 
 X_PLAIN, X_LAYERNORM, X_PARTIAL_SUM = 0, 1, 2
 EPI_STORE, EPI_GELU, EPI_RESIDUAL, EPI_LOGITS_F32, EPI_QKV_SCATTER = 0, 1, 2, 3, 4
 _DT = {torch.float16: DTYPE_F16, torch.bfloat16: DTYPE_BF16, torch.float32: DTYPE_F32}
 TIMESTAMP_BEGIN, NO_TIMESTAMPS = 50363, 50362
 BEAM_MAX, MAX_CANDIDATES = 8, 32
-BEAM_SCRATCH = 48      # floats per (row, slice) of the beam candidate kernel
+BEAM_SCRATCH = 48      # floats per (row, slice) of the beam candidate and rule-aware sampling kernels
+
+
+_M64 = (1 << 64) - 1
+
+
+def _mix64(x: int) -> int:
+    """splitmix64 (Steele, Lea, Flood: "Fast splittable pseudorandom number generators", OOPSLA 2014)."""
+    x = (x + 0x9E3779B97F4A7C15) & _M64
+    x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & _M64
+    return x ^ (x >> 31)
+
+
+def sample_row_key(seed: int, clip: int, sample: int) -> int:
+    """The 64-bit Philox key of sample `sample` of clip `clip` (counted over the whole decode() call) under `seed`: a
+    clip's draws do not depend on how the call is split into engine batches."""
+    return _mix64(_mix64(_mix64(seed & _M64) ^ clip) ^ sample)
 
 
 def _convert(src: Tensor, dst: Tensor) -> Tensor:
@@ -99,6 +121,11 @@ class DecodeEngine:
         self.fin_len = torch.zeros((N, MAX_CANDIDATES), device=dev, dtype=torch.int32)
         self.fin_count = torch.zeros(N, device=dev, dtype=torch.int32)
         self.seq_len = torch.zeros(1, device=dev, dtype=torch.int32)
+        # temperature sampling: read by the kernel at every replay (not baked into the graphs)
+        self.temperature = z(1, dt=torch.float32)
+        self.row_keys = torch.zeros(N, device=dev, dtype=torch.int64)
+        self._rules_cfg = None     # (timestamps, max_initial_timestamp_index or -1, sampling) for the rule-aware sampler
+        self._group = 1            # rows per clip that share one cross-attention K / V (beam size or best_of)
         self._beam_cfg = None      # (beam, clips, max_candidates, timestamps, max_initial_timestamp_index or -1) while beam searching
         self._w: Optional[dict] = None
         self._w_sig = None
@@ -196,7 +223,7 @@ class DecodeEngine:
         # the attention kernels lay their fp32 partial outputs out as (splits, n, d): views with exactly that geometry
         part_self = self.part_self.view(-1)[: n * d].view(1, n, d)
         part_cross = self.part_cross.view(-1)[: sc * n * d].view(sc, n, d)
-        kv_group = 1 if self._beam_cfg is None else self._beam_cfg[0]
+        kv_group = self._group
         for l, lw in enumerate(w["layers"]):
             self._linear(n, x, lw["wqkv"], lw["bqkv"], q, x_mode=X_LAYERNORM, ln=lw["ln1"], epi=EPI_QKV_SCATTER,
                          kv=(self.self_k[l], self.self_v[l]))
@@ -213,6 +240,10 @@ class DecodeEngine:
             self._enqueue_beam_select()
             self.launches_per_step = _lib.LAUNCH_COUNT - c0
             return
+        if self._rules_cfg is not None:
+            self._enqueue_sample_rules(n)
+            self.launches_per_step = _lib.LAUNCH_COUNT - c0
+            return
         s = DecSampleArgs()
         s.logits, s.ld_logits = ptr(self.logits), self.logits.stride(0)
         s.tokens, s.ld_tokens, s.pos_ptr = ptr(self.tokens), self.tokens.stride(0), ptr(self.pos)
@@ -225,14 +256,31 @@ class DecodeEngine:
         call("oasr_dec_sample", ctypes.byref(s), stream())
         self.launches_per_step = _lib.LAUNCH_COUNT - c0
 
+    def _enqueue_sample_rules(self, n: int):
+        """The rule-aware sampling step (timestamp rules and / or temperature sampling) + position advance: 2 launches."""
+        ts, mi, sampling = self._rules_cfg
+        s = DecSampleRulesArgs()
+        s.logits, s.ld_logits = ptr(self.logits), self.logits.stride(0)
+        s.tokens, s.ld_tokens, s.pos_ptr = ptr(self.tokens), self.tokens.stride(0), ptr(self.pos)
+        s.suppress, s.sum_logprobs, s.no_speech_prob = ptr(self.suppress), ptr(self.sum_logprobs), ptr(self.no_speech)
+        s.n_unfinished, s.done_flag = ptr(self.n_unfinished), ptr(self.done)
+        s.scratch, s.counters, s.n_slices = ptr(self.beam_scratch), ptr(self.sample_counters), self.sample_slices
+        if sampling:
+            s.temperature, s.row_keys = ptr(self.temperature), ptr(self.row_keys)
+        s.n_seq, s.n_vocab = n, self.V
+        s.sample_begin, s.sot_index, s.suppress_blank, s.blank, s.eot, s.no_speech = self._sample_cfg
+        s.timestamps, s.timestamp_begin, s.no_timestamps, s.max_initial_timestamp = ts, TIMESTAMP_BEGIN, NO_TIMESTAMPS, mi
+        call("oasr_dec_sample_rules", ctypes.byref(s), stream())
+
     def _graph(self, n: int) -> torch.cuda.CUDAGraph:
-        key = (n, self._sample_cfg, self._beam_cfg)
+        key = (n, self._sample_cfg, self._beam_cfg, self._rules_cfg, self._group)
         g = self._graphs.get(key)
         if g is None:
             # one eager run first (kernel modules are loaded lazily on first launch, which must not happen under capture),
             # with the device-side decode state saved and restored around it; the capture itself does not execute
             live = (self.pos, self.tokens, self.sum_logprobs, self.no_speech, self.n_unfinished, self.done, self.sample_counters,
-                    self.src_rows, self.fin_tokens, self.fin_scores, self.fin_len, self.fin_count, self.seq_len)
+                    self.src_rows, self.fin_tokens, self.fin_scores, self.fin_len, self.fin_count, self.seq_len,
+                    self.temperature, self.row_keys)
             state = [t.clone() for t in live]
             self._enqueue_step(n)
             torch.cuda.synchronize(self.dev)
@@ -286,6 +334,8 @@ class DecodeEngine:
         self.suppress.copy_(sup)
         self._sample_cfg = (P if sample_begin is None else sample_begin, sot_index, int(bool(suppress_blank)), blank, eot, no_speech)
         self._beam_cfg = None
+        self._rules_cfg = None
+        self._group = 1
 
     def replay(self, n: int):
         """One decoder step for sequences [0, n): feeds the token at the device-side position, leaves the fp32 logits of that
@@ -295,15 +345,24 @@ class DecodeEngine:
     @torch.no_grad()
     def greedy(self, audio_features: Tensor, initial_tokens: Sequence[int], sample_len: int, suppress: Sequence[int] = (),
                suppress_blank: bool = True, sot_index: int = 0, blank: int = 220, eot: int = 50256, no_speech: int = 50361,
-               check_every: int = 8) -> Tuple[Tensor, Tensor, Tensor, int]:
+               check_every: int = 8, timestamps: bool = False,
+               max_initial_timestamp_index: Optional[int] = None) -> Tuple[Tensor, Tensor, Tensor, int]:
         """Returns (tokens (N, len) int64 on the host incl. the initial tokens, sum_logprobs (N,), no_speech_probs (N,),
-        number of graph replays).  Semantics of DecodingTask._main_loop for temperature 0 without timestamp rules."""
+        number of graph replays).  Semantics of DecodingTask._main_loop for temperature 0, with ApplyTimestampRules when
+        `timestamps`."""
         n = self.prepare(audio_features)
         init = list(initial_tokens)
         n_init = len(init)
         if not 1 <= n_init < self.n_ctx:
             raise ValueError("initial_tokens: need 1 .. n_text_ctx-1 tokens")
         self.reset(n, torch.tensor([init], dtype=torch.int32).repeat(n, 1), None, suppress, suppress_blank, sot_index, blank, eot, no_speech)
+        if timestamps:
+            self._rules_cfg = (1, -1 if max_initial_timestamp_index is None else int(max_initial_timestamp_index), 0)
+        return self._run(n, n_init, sample_len, check_every)
+
+    def _run(self, n: int, n_init: int, sample_len: int, check_every: int) -> Tuple[Tensor, Tensor, Tensor, int]:
+        """Replay the step graph of the configured decode until every row has ended (looked at every `check_every` sampled
+        tokens) or the length limit; (tokens, sum_logprobs, no_speech_probs, replays) as `greedy` returns them."""
         g = self._graph(n)
         # positions 0 .. n_init-2 are teacher-forced; every replay from position n_init-1 on samples one token; the loop
         # of the reference also ends when the sequence would exceed n_text_ctx (whisper/decoding.py: tokens.shape[-1] > n_ctx)
@@ -319,6 +378,40 @@ class DecodeEngine:
         length = n_init + max(0, replays - (n_init - 1))
         return (self.tokens[:n, :length].to(torch.int64).cpu(), self.sum_logprobs[:n].clone(), self.no_speech[:n].clone(), replays)
 
+    @torch.no_grad()
+    def sample(self, audio_features: Tensor, initial_tokens: Sequence[int], sample_len: int, temperature: float,
+               best_of: int = 1, seed: int = 0, clip_offset: int = 0, suppress: Sequence[int] = (), suppress_blank: bool = True,
+               sot_index: int = 0, timestamps: bool = False, max_initial_timestamp_index: Optional[int] = None,
+               blank: int = 220, eot: int = 50256, no_speech: int = 50361, check_every: int = 8):
+        """Temperature sampling with `best_of` samples per clip (DecodingTask._main_loop with GreedyDecoder at temperature
+        > 0, and ApplyTimestampRules when `timestamps`).  Row c * best_of + j draws with the key sample_row_key(seed,
+        clip_offset + c, j).  Cross K/V is projected once per clip and shared by its samples.  Returns (candidates,
+        no_speech_probs (n_clips,), number of graph replays): candidates[c] is the list of best_of (token ids incl. the
+        initial tokens and the final eot, sum_logprob), as `beam_search` returns them."""
+        G = int(best_of)
+        C = audio_features.shape[0]
+        if not temperature > 0:
+            raise ValueError(f"sample: temperature must be > 0 (got {temperature}); use greedy() for temperature 0")
+        if not 1 <= G <= self.max_batch or C * G > self.max_batch:
+            raise ValueError(f"sample: at most {self.max_batch // max(G, 1)} clips per call at best_of {G} (got {C})")
+        init = list(initial_tokens)
+        n_init = len(init)
+        if not 1 <= n_init < self.n_ctx:
+            raise ValueError("initial_tokens: need 1 .. n_text_ctx-1 tokens")
+        self.prepare(audio_features)
+        n = C * G
+        self.reset(n, torch.tensor([init], dtype=torch.int32).repeat(n, 1), None, suppress, suppress_blank, sot_index, blank, eot, no_speech)
+        mi = -1 if max_initial_timestamp_index is None else int(max_initial_timestamp_index)
+        self._rules_cfg = (int(bool(timestamps)), mi, 1)
+        self._group = G
+        keys = [sample_row_key(seed, clip_offset + c, j) for c in range(C) for j in range(G)]
+        self.row_keys[:n] = torch.tensor([k - (1 << 64) if k >> 63 else k for k in keys], dtype=torch.int64)
+        self.temperature.fill_(float(temperature))
+        toks, lps, nsp, replays = self._run(n, n_init, sample_len, check_every)
+        rows, lps = toks.tolist(), lps.tolist()
+        candidates = [[(rows[c * G + j] + [eot], lps[c * G + j]) for j in range(G)] for c in range(C)]
+        return candidates, nsp[::G], replays
+
     # ---- beam search ------------------------------------------------------------------------------------------------
     def reset_beam(self, n_clips: int, beam: int, max_candidates: int, timestamps: bool = False,
                    max_initial_timestamp_index: Optional[int] = None):
@@ -327,6 +420,7 @@ class DecodeEngine:
         self.src_rows.copy_(torch.arange(self.max_batch, device=self.dev, dtype=torch.int32))
         mi = -1 if max_initial_timestamp_index is None else int(max_initial_timestamp_index)
         self._beam_cfg = (beam, n_clips, max_candidates, int(bool(timestamps)), mi)
+        self._group = beam
 
     def beam_args(self) -> DecBeamArgs:
         """Argument block of the beam candidate / select kernels for the current state."""

@@ -8,10 +8,12 @@ DecodingTask._verify_options / _main_loop, PyTorchInference (first call = whole 
 through `model.install_kv_cache_hooks()`), GreedyDecoder, BeamSearchDecoder, MaximumLikelihoodRanker, SuppressBlank,
 SuppressTokens, ApplyTimestampRules.
 
-Routes: greedy without timestamps and beam search (with or without timestamps) run on the device decoder
-(olmoasr_b200/decode_engine.py) as replays of one CUDA graph per step; greedy with timestamps and temperature sampling
-(best_of samples per clip, ranked like upstream) run on the hook loop below.  Beam search needs the device decoder: a
-model without `decode_engine`, or OASR_DECODE_ENGINE=0, raises NotImplementedError for `beam_size`.
+Routes: every configuration runs on the device decoder (olmoasr_b200/decode_engine.py) as replays of one CUDA graph per
+step: greedy decoding with or without timestamp rules, temperature sampling (best_of samples per clip sharing the clip's
+cross-attention K/V, ranked like upstream) and beam search.  The hook loop below remains for OASR_DECODE_ENGINE=0, models
+without `decode_engine` and best_of above the engine's batch (64 rows).  Beam search needs the device decoder: without
+it, `beam_size` raises NotImplementedError.  Sampled ids follow softmax(logits / T) like upstream's
+`Categorical(...).sample()` but from the engine's own keyed random stream (reproducible under `torch.manual_seed`).
 
 Token ids are the contract: text<->id conversion needs the `gpt2.tiktoken` vocabulary, which is not available offline;
 pass `tokenizer=` (an object with `.decode(list[int])`) to get text, otherwise `DecodingResult.text` is empty.
@@ -206,8 +208,12 @@ class DecodingTask:
         dev = audio_features.device
         if opt.beam_size is not None:
             return self._run_beam_on_device(audio_features, tokenizer)
-        if opt.temperature == 0 and self.ts_rules is None and USE_ENGINE and hasattr(model, "decode_engine"):
-            return self._run_on_device(audio_features, tokenizer)
+        if USE_ENGINE and hasattr(model, "decode_engine"):
+            eng = model.decode_engine(torch.float16 if opt.fp16 else torch.bfloat16)
+            if opt.temperature == 0:
+                return self._run_on_device(audio_features, tokenizer, eng)
+            if self.n_group <= eng.max_batch:
+                return self._run_sampling_on_device(audio_features, tokenizer, eng)
         G = self.n_group                           # best_of samples per clip (temperature > 0), rows clip-major
         xa = audio_features.repeat_interleave(G, dim=0) if G > 1 else audio_features
         n_rows = n_audio * G
@@ -291,16 +297,35 @@ class DecodingTask:
                                           temperature=opt.temperature))
         return results
 
-    def _run_on_device(self, audio_features: Tensor, tokenizer):
-        """Greedy decoding without timestamp rules (the short-form eval configuration, scripts/eval/eval.py:1846-1847): the
-        whole loop runs as replays of one CUDA graph (olmoasr_b200/decode_engine.py)."""
+    def _run_sampling_on_device(self, audio_features: Tensor, tokenizer, eng):
+        """Temperature sampling, best_of samples per clip (every fallback temperature of transcribe()), on the device
+        decoder: up to max_batch // best_of clips per call, ranked like the hook loop.  One seed per decode() call from
+        torch's default generator; each clip's draws depend on it and on the clip's index in this call only."""
+        opt, G = self.options, self.n_group
+        per = eng.max_batch // G
+        ts = self.ts_rules is not None
+        mi = self.ts_rules.max_initial_timestamp_index if ts else None
+        seed = int(torch.randint(2 ** 62, (1,)))
+        candidates, nsp = [], []
+        for s in range(0, audio_features.shape[0], per):
+            c, ns, _ = eng.sample(audio_features[s:s + per], self.initial_tokens, self.sample_len, opt.temperature, G, seed, s,
+                                  self.suppress, opt.suppress_blank, self.sot_index, timestamps=ts, max_initial_timestamp_index=mi)
+            candidates += c
+            nsp += ns.tolist()
+        return self._ranked(audio_features, candidates, nsp, tokenizer)
+
+    def _run_on_device(self, audio_features: Tensor, tokenizer, eng):
+        """Greedy decoding (the short-form eval configuration, scripts/eval/eval.py:1846-1847, and the temperature-0 step of
+        transcribe() with timestamp rules): the whole loop runs as replays of one CUDA graph (olmoasr_b200/decode_engine.py),
+        up to 64 clips per call."""
         from .decode_engine import DecodeEngine
 
-        eng = self.model.decode_engine(torch.float16 if self.options.fp16 else torch.bfloat16)
+        ts = self.ts_rules is not None
+        mi = self.ts_rules.max_initial_timestamp_index if ts else None
         toks, lps, nsp = [], [], []
         for s in range(0, audio_features.shape[0], DecodeEngine.MAX_BATCH):
             t, lp, ns, _ = eng.greedy(audio_features[s:s + DecodeEngine.MAX_BATCH], self.initial_tokens, self.sample_len, self.suppress,
-                                      self.options.suppress_blank, self.sot_index)
+                                      self.options.suppress_blank, self.sot_index, timestamps=ts, max_initial_timestamp_index=mi)
             toks.append(t); lps += lp.tolist(); nsp += ns.tolist()
         width = max(t.shape[1] for t in toks)
         tokens = torch.cat([F.pad(t, (0, width - t.shape[1]), value=EOT) for t in toks], dim=0)

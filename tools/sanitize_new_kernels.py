@@ -54,6 +54,11 @@ def main():
         xa = torch.randn(3, 1500, 64, device=dev).bfloat16()
         eng.beam_search(xa, [50257, 50362], 4, 5, suppress=(7, 9))
         eng.beam_search(xa[:2], [50257], 4, 3, patience=2.0, suppress=(7, 9), timestamps=True, max_initial_timestamp_index=50)
+        # rule-aware sampling: greedy with timestamp rules, best-of sampling (grouped cross-attention) with and without them
+        eng.greedy(xa, [50257], 4, suppress=(7, 9), timestamps=True, max_initial_timestamp_index=50)
+        eng.sample(xa, [50257, 50362], 4, 0.6, best_of=5, seed=1, suppress=(7, 9))
+        eng.sample(xa[:2], [50257], 4, 1.0, best_of=3, seed=2, clip_offset=5, suppress=(7, 9), timestamps=True,
+                   max_initial_timestamp_index=50)
     torch.cuda.synchronize()
     print("sanitize run complete; loss", float(loss))
 
