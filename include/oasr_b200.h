@@ -295,6 +295,63 @@ OASR_API int oasr_dec_beam_reorder(void* k_cache, void* v_cache, int64_t layer_s
 /* elementwise dtype conversion (weights fp32 -> T once per engine; bf16 encoder output / cross K,V -> fp16) */
 OASR_API int oasr_convert(const void* src, int src_dtype, void* dst, int dst_dtype, int64_t n, void* stream);
 
+/* ---- training kernels with a selectable 16-bit activation type -------------------------------------------------
+ * The same kernels as the bf16 entry points above, for the reference's step under torch.autocast(dtype=float16)
+ * (train_timestamps.py:1414, precision="float16" at :2128): `dtype` is OASR_DTYPE_BF16 (then each call is exactly its
+ * bf16 twin: oasr_gemm16 = oasr_gemm_bf16, oasr_colsum16 = oasr_colsum_bf16, ...) or OASR_DTYPE_F16, which reads
+ * and writes every 16-bit operand, activation and gradient as IEEE fp16 with the bf16 path's rounding points (the
+ * wgmma GEMMs and attention MMAs run .f16 with fp32 accumulators; statistics, lse, delta, biases and weight gradients
+ * stay fp32).  fp16 results outside +-65504 become +-inf, like torch's fp16 ops, so GradScaler sees an overflow.
+ * oasr_im2col_conv2 is a copy and serves both types; the fp32 -> fp16 weight cast is oasr_convert. */
+OASR_API int oasr_gemm16(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, int b_layout, void* C,
+                         int64_t ldc, void* C2, const float* bias, const void* aux, int64_t ldaux, int64_t M, int64_t N,
+                         int64_t K, int epilogue, int split_k, int block_n, int dtype, void* stream);
+OASR_API int oasr_layernorm_fwd16(const void* x, const float* weight, const float* bias, void* y, float* mean,
+                                  float* rstd, int64_t rows, int64_t d, float eps, int dtype, void* stream);
+OASR_API int oasr_layernorm_bwd16(const void* dy, const void* x, const float* weight, const float* mean,
+                                  const float* rstd, const void* dresidual, void* dx, float* dweight, float* dbias,
+                                  int64_t rows, int64_t d, int dtype, void* stream);
+OASR_API int oasr_attention_fwd16(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                  void* o, int64_t ldo, float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
+                                  int64_t head_dim, int causal, const int32_t* kv_len, float scale, int dtype, void* stream);
+OASR_API int oasr_attention_bwd16(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                  const void* o, int64_t ldo, const void* dout, int64_t lddo, const float* lse,
+                                  float* delta, void* dq, int64_t lddq, void* dk, int64_t lddk,
+                                  void* dv, int64_t lddv, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
+                                  int64_t head_dim, int causal, const int32_t* kv_len, float scale, int dtype, void* stream);
+OASR_API int oasr_ce_fwd16(const void* logits, const int64_t* targets, float* lse, float* loss_sum_count,
+                           int64_t rows, int64_t V, int64_t ld, int64_t ignore_index, int dtype, void* stream);
+OASR_API int oasr_ce_bwd16(void* logits, const int64_t* targets, const float* lse, const float* loss_sum_count,
+                           const float* grad_out, int64_t rows, int64_t V, int64_t ld, int64_t ignore_index, int dtype,
+                           void* stream);
+OASR_API int oasr_logits_to_f32_16(const void* src, float* dst, int64_t rows, int64_t V, int64_t ld, int dtype,
+                                   void* stream);
+OASR_API int oasr_embed_fwd16(const int64_t* ids, const float* emb, const float* pos, void* out, int64_t batch,
+                              int64_t S, int64_t d, int64_t pos_offset, int64_t n_rows_emb, int dtype, void* stream);
+OASR_API int oasr_embed_bwd16(const int64_t* ids, const void* dx, float* demb, float* dpos, int64_t batch, int64_t S,
+                              int64_t d, int64_t padding_idx, int64_t n_rows_emb, int dtype, void* stream);
+OASR_API int oasr_cast_conv_weight16(const float* src, void* dst, int64_t c_out, int64_t c_in, int dtype, void* stream);
+OASR_API int oasr_im2col_conv1_16(const float* mel, void* A, int64_t batch, int64_t C, int64_t T, int64_t kpad, int dtype,
+                                  void* stream);
+OASR_API int oasr_col2im_conv2_gelu_bwd16(const void* dA, const void* pre1, void* dpre1, int64_t batch, int64_t T_in,
+                                          int64_t T_out, int64_t d, int dtype, void* stream);
+OASR_API int oasr_add_pos16(const void* x, const float* pos, void* out, int64_t rows, int64_t T, int64_t d, int dtype,
+                            void* stream);
+OASR_API int oasr_gelu_bwd16(const void* dy, const void* pre, void* out, int64_t n, int dtype, void* stream);
+OASR_API int oasr_colsum16(const void* dy, float* db, int64_t M, int64_t N, int64_t ld, int dtype, void* stream);
+/* The flat AdamW update refreshing a shadow slab of type `dtype` (bf16 or fp16; see oasr_adamw_flat). */
+OASR_API int oasr_adamw_flat16(float* p, const float* g, float* m, float* v, void* shadow, int64_t numel,
+                               const float* state, float lr, float beta1, float beta2, float eps, float weight_decay,
+                               int dtype, void* stream);
+/* oasr_optim_prepare for torch.amp.GradScaler (train_timestamps.py:2349, :1509-1521) without a host read: loss_scale
+ * (nullable) is GradScaler's scale S on the device and ext_found_inf (nullable) its found-inf flag.  norm_sq is the
+ * squared norm of g * inv_scale with the gradients still scaled by S; the step multiplies every gradient by
+ * inv_scale / S, clips against sqrt(norm_sq) / S, and is skipped (not counted) when *ext_found_inf != 0 or that norm
+ * is not finite. */
+OASR_API int oasr_optim_prepare_amp(const float* norm_sq, float* found_inf, float* state, const float* loss_scale,
+                                    const float* ext_found_inf, float inv_scale, float max_norm, float beta1, float beta2,
+                                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif

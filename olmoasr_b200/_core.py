@@ -3,9 +3,11 @@
 The module tree, parameter names / shapes and initialisation follow the reference exactly
 (olmoasr/model.py:14-968, olmoasr/inf_model.py) so that `state_dict()`s are interchangeable and DDP / FSDP /
 AdamW / checkpoint code written for the reference keeps working.  Every tensor operation is a call into
-liboasr_b200.so; computation is bf16 with fp32 master weights and fp32 statistics, i.e. the numerics of the
-reference under `torch.autocast("cuda", torch.bfloat16)` (scripts/training/train_timestamps.py:1414) with
-its rounding points reproduced (Linear outputs, GELU, residual adds, LayerNorm casts, bf16 logits).
+liboasr_b200.so; computation is 16-bit with fp32 master weights and fp32 statistics, i.e. the numerics of the
+reference under `torch.autocast("cuda", dtype)` (scripts/training/train_timestamps.py:1414) with its rounding points
+reproduced (Linear outputs, GELU, residual adds, LayerNorm casts, 16-bit logits).  dtype is fp16 when the call is made
+under `torch.autocast("cuda", torch.float16)` (the reference trainer's default precision, :2128) and bf16 otherwise;
+each top-level call resolves it once (`compute_dtype`) and the tensors carry it through every kernel.
 
 Training fast path: one autograd.Function per ResidualAttentionBlock (+ stem, embedding and loss head) whose
 backward is a hand-sequenced list of kernels -- dgrad / wgrad GEMMs read the saved activations MN-major through
@@ -13,6 +15,7 @@ the wgmma shared-memory descriptors, so nothing is transposed in HBM.
 """
 from __future__ import annotations
 
+import contextlib
 import math
 import os
 from typing import Dict, Iterable, Optional
@@ -54,6 +57,41 @@ def _pick_split_k(tiles: int, kblocks: int) -> int:
         if best_cost is None or cost < best_cost - 1e-9:
             best, best_cost = s, cost
     return best
+
+
+_bf16_pinned = 0   # > 0 inside bf16_compute()
+
+
+def compute_dtype() -> torch.dtype:
+    """The 16-bit type of a top-level call: fp16 under torch.autocast("cuda", torch.float16), bf16 otherwise (also under
+    bf16 autocast, with no autocast at all, and inside `bf16_compute()`)."""
+    if _bf16_pinned == 0 and torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.float16:
+        return torch.float16
+    return torch.bfloat16
+
+
+@contextlib.contextmanager
+def bf16_compute():
+    """Run the model in bf16 whatever the autocast state: decode() and transcribe() keep their bf16 encoder and hook
+    path when they are called inside an fp16 autocast region."""
+    global _bf16_pinned
+    _bf16_pinned += 1
+    try:
+        yield
+    finally:
+        _bf16_pinned -= 1
+
+
+def _f16_kw(dtype: torch.dtype) -> dict:
+    """`dtype=` for the kernels whose inputs are all fp32; bf16 calls keep the argument lists they always had."""
+    return {} if dtype == torch.bfloat16 else {"dtype": dtype}
+
+
+def _cast16(src: Tensor, dtype: torch.dtype, *dst: Tensor) -> Tensor:
+    """fp32 master -> 16-bit weight shadow, into `dst` when given (the bf16 cast keeps its own entry point)."""
+    if dtype == torch.bfloat16:
+        return K.cast_bf16(src, *dst)
+    return K.convert(src, *dst, dtype=dtype)
 
 
 def linear_fwd(x: Tensor, w_bf16: Tensor, bias: Optional[Tensor], *, epi=K.EPI_BF16, aux=None, out=None):
@@ -278,14 +316,14 @@ def kv_len_from_padding_mask(padding_mask: Tensor) -> Tensor:
 
 
 class _ShadowCache:
-    """bf16 copies of fp32 master weights (+ fused biases), rebuilt only when a master changed."""
+    """16-bit copies of fp32 master weights (+ fused biases), rebuilt only when a master or the wanted type changed."""
 
     def __init__(self):
         self.key = None
         self.val = None
 
-    def get(self, params: Iterable[Tensor], build):
-        key = tuple((p.data_ptr(), p._version, p.device) for p in params)
+    def get(self, params: Iterable[Tensor], build, dtype: torch.dtype = torch.bfloat16):
+        key = (dtype,) + tuple((p.data_ptr(), p._version, p.device) for p in params)
         if key != self.key:
             with torch.no_grad():
                 self.val = build()
@@ -301,7 +339,7 @@ class LayerNorm(nn.LayerNorm):
 
     def forward(self, x: Tensor) -> Tensor:
         shp = x.shape
-        y = K.layernorm_fwd(_as_bf16_2d(x), _f32(self.weight), _f32(self.bias), self.eps, want_stats=False)
+        y = K.layernorm_fwd(_as16_2d(x, compute_dtype()), _f32(self.weight), _f32(self.bias), self.eps, want_stats=False)
         return y.view(shp)
 
 
@@ -313,18 +351,24 @@ class Linear(nn.Linear):
         nn.init.kaiming_normal_(self.weight, mode="fan_in", nonlinearity="relu")
         self._shadow = _ShadowCache()
 
-    _slab_view: Optional[Tensor] = None   # set by OLMoASRBase.use_slabs(): a view into the bf16 shadow slab
+    _slab_view: Optional[Tensor] = None   # set by OLMoASRBase.use_slabs(): a view into the shadow slab
 
     def weight_bf16(self) -> Tensor:
+        return self.weight16(torch.bfloat16)
+
+    def weight16(self, dtype: torch.dtype) -> Tensor:
         if self._slab_view is not None:
-            return self._slab_view
-        if self.weight.dtype == torch.bfloat16:      # FSDP bf16 param_dtype: the unsharded view IS the operand (never cached)
+            return _slab16(self._slab_view, dtype)
+        if self.weight.dtype == dtype:      # FSDP param_dtype: the unsharded view IS the operand (never cached)
             return self.weight.detach()
-        return self._shadow.get((self.weight,), lambda: K.cast_bf16(self.weight.detach().contiguous()))
+        if not _is_master(self.weight):
+            return K.convert(self.weight.detach().contiguous(), dtype=dtype)
+        return self._shadow.get((self.weight,), lambda: _cast16(self.weight.detach().contiguous(), dtype), dtype)
 
     def forward(self, x: Tensor) -> Tensor:  # inference / hook path (no autograd through the kernels)
         shp = x.shape
-        y = linear_fwd(_as_bf16_2d(x), self.weight_bf16(), None if self.bias is None else _f32(self.bias))
+        dt = compute_dtype()
+        y = linear_fwd(_as16_2d(x, dt), self.weight16(dt), None if self.bias is None else _f32(self.bias))
         return y.view(*shp[:-1], self.out_features)
 
 
@@ -338,10 +382,14 @@ class Conv1d(nn.Conv1d):
         nn.init.kaiming_normal_(self.weight, mode="fan_in", nonlinearity="relu")
         self._shadow = _ShadowCache()
 
-    def weight_bf16(self) -> Tensor:  # (C_out, 3*C_in) with column = k*C_in + c
+    def weight_bf16(self) -> Tensor:
+        return self.weight16(torch.bfloat16)
+
+    def weight16(self, dtype: torch.dtype) -> Tensor:  # (C_out, 3*C_in) with column = k*C_in + c
         if not _is_master(self.weight):
-            return K.cast_conv_weight(_f32(self.weight).contiguous())
-        return self._shadow.get((self.weight,), lambda: K.cast_conv_weight(self.weight.detach().contiguous()))
+            return K.cast_conv_weight(_f32(self.weight).contiguous(), **_f16_kw(dtype))
+        return self._shadow.get((self.weight,), lambda: K.cast_conv_weight(self.weight.detach().contiguous(), **_f16_kw(dtype)),
+                                dtype)
 
 
 def sinusoids(length, channels, max_timescale=10000):
@@ -353,10 +401,20 @@ def sinusoids(length, channels, max_timescale=10000):
     return torch.cat([torch.sin(scaled_time), torch.cos(scaled_time)], dim=1)
 
 
-def _as_bf16_2d(x: Tensor) -> Tensor:
-    if x.dtype != torch.bfloat16:
-        x = x.to(torch.bfloat16)
+def _as16_2d(x: Tensor, dtype: torch.dtype) -> Tensor:
+    if x.dtype != dtype:
+        x = x.to(dtype)
     return x.reshape(-1, x.shape[-1]).contiguous()
+
+
+def _as_bf16_2d(x: Tensor) -> Tensor:
+    return _as16_2d(x, torch.bfloat16)
+
+
+def _slab16(view: Tensor, dtype: torch.dtype) -> Tensor:
+    """A view of the shadow slab S as `dtype`: S holds the type the model last computed in (ParamSlabs.ensure_synced),
+    and bf16 and fp16 have the same size, so either is a reinterpretation of the same bytes."""
+    return view if view.dtype == dtype else view.view(dtype)
 
 
 def _f32(p: Tensor) -> Tensor:
@@ -400,24 +458,27 @@ class MultiHeadAttention(nn.Module):
             nn.init.kaiming_normal_(self.out.weight, mode="fan_in", nonlinearity="relu")
         self._fused = _ShadowCache()
 
-    # ---- fused bf16 shadows -------------------------------------------------------------------------
+    # ---- fused 16-bit shadows -----------------------------------------------------------------------
     _slab_fused = None   # set by OLMoASRBase.use_slabs(): ([Wq;Wk;Wv] view of the shadow slab, [bq;0;bv] view of the masters)
 
-    def fused_qkv(self):
-        """([Wq;Wk;Wv] (3d, d) bf16, [bq;0;bv] (3d,) f32) -- key has no bias (model.py:259)."""
+    def fused_qkv(self, dtype: torch.dtype = torch.bfloat16):
+        """([Wq;Wk;Wv] (3d, d) in `dtype`, [bq;0;bv] (3d,) f32) -- key has no bias (model.py:259)."""
         if self._slab_fused is not None:
-            return self._slab_fused
+            w, b = self._slab_fused
+            return _slab16(w, dtype), b
         ps = (self.query.weight, self.key.weight, self.value.weight, self.query.bias, self.value.bias)
 
         def build():
             d = self.query.weight.shape[0]
-            w = torch.empty((3 * d, d), device=ps[0].device, dtype=torch.bfloat16)
+            w = torch.empty((3 * d, d), device=ps[0].device, dtype=dtype)
             b = torch.zeros(3 * d, device=ps[0].device, dtype=torch.float32)
             for i, p in enumerate(ps[:3]):
                 if _is_master(p):
-                    K.cast_bf16(p.detach().contiguous(), w[i * d:(i + 1) * d])
-                else:
+                    _cast16(p.detach().contiguous(), dtype, w[i * d:(i + 1) * d])
+                elif p.dtype == dtype:
                     w[i * d:(i + 1) * d].copy_(p.detach())     # bf16 unsharded FSDP view: a device-to-device copy
+                else:
+                    K.convert(p.detach().contiguous(), w[i * d:(i + 1) * d])
             for p, sl in ((ps[3], slice(0, d)), (ps[4], slice(2 * d, 3 * d))):
                 if _is_master(p):
                     b[sl].copy_(p.detach())
@@ -428,10 +489,10 @@ class MultiHeadAttention(nn.Module):
         if not _is_master(ps[0]):
             with torch.no_grad():
                 return build()                                  # transient FSDP views: nothing to key a cache on
-        return self._fused.get(ps, build)
+        return self._fused.get(ps, build, dtype)
 
-    def fused_kv(self):
-        w, b = self.fused_qkv()
+    def fused_kv(self, dtype: torch.dtype = torch.bfloat16):
+        w, b = self.fused_qkv(dtype)
         d = self.query.weight.shape[0]
         return w[d:], b[d:]
 
@@ -460,7 +521,8 @@ class MultiHeadAttention(nn.Module):
 # fused training blocks
 # =====================================================================================================
 class _BlockFn(torch.autograd.Function):
-    """ResidualAttentionBlock.forward (model.py:485-528) for a (B*T, d) bf16 residual stream.
+    """ResidualAttentionBlock.forward (model.py:485-528) for a (B*T, d) bf16 or fp16 residual stream (x's type is the
+    block's compute type).
 
     inputs: x, xa (or None), kv_len (or None), then the block's parameters in `ResidualAttentionBlock._param_list`
     order.  Saves every GEMM input it needs for wgrad; recomputes nothing."""
@@ -470,11 +532,11 @@ class _BlockFn(torch.autograd.Function):
         ctx.xa_state = xa_state
         H = blk.attn.n_head
         d = x.shape[1]
-        sh = blk._shadows()
+        sh = blk._shadows(x.dtype)
         side = _Side(x.device)
         kvc = None
         if xa is not None:   # the cross-attention K/V projection only needs the encoder output: side stream, joined below
-            kvc = torch.empty((xa.shape[0], 2 * d), device=x.device, dtype=torch.bfloat16)
+            kvc = torch.empty((xa.shape[0], 2 * d), device=x.device, dtype=x.dtype)
             side.run(lambda: linear_fwd(xa, sh["wckv"], sh["bckv"], out=kvc))
         ln1, mean1, rstd1 = K.layernorm_fwd(x, sh["ln1w"], sh["ln1b"])
         qkv = linear_fwd(ln1, sh["wqkv"], sh["bqkv"])
@@ -503,10 +565,10 @@ class _BlockFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dx3):
         blk, sh = ctx.blk, ctx.sh
-        if not _is_master(blk.attn.query.weight):
-            sh = blk._shadows()      # FSDP frees and re-gathers the unsharded parameters between forward and backward
-        B, T, Ta, H, d, causal, cross, has_len = ctx.dims
         sv = list(ctx.saved_tensors)
+        if not _is_master(blk.attn.query.weight):
+            sh = blk._shadows(sv[0].dtype)   # FSDP frees and re-gathers the unsharded parameters between forward and backward
+        B, T, Ta, H, d, causal, cross, has_len = ctx.dims
         kv_len = sv.pop() if has_len else None
         x, mean1, rstd1, ln1, qkv, ao, lse, x1 = sv[:8]
         if cross:
@@ -592,34 +654,39 @@ class ResidualAttentionBlock(nn.Module):
         # slab mode (OLMoASRBase.use_slabs): precomputed operand views, gradient-slab targets, completion callback
         self._slabs = None
         self._slab_sh: Optional[Dict[str, Tensor]] = None
+        self._slab_sh16: Optional[Dict[str, Tensor]] = None
         self._direct: Optional[Dict[str, Tensor]] = None
         self._bwd_done_cb = None
 
-    def _build_shadows(self) -> Dict[str, Tensor]:
-        """Every operand the fused block kernels read that derives from a parameter: bf16 weights (fused where the GEMMs are
-        fused) and fp32 vectors (biases, LayerNorm affine)."""
+    def _build_shadows(self, dtype: torch.dtype = torch.bfloat16) -> Dict[str, Tensor]:
+        """Every operand the fused block kernels read that derives from a parameter: 16-bit weights of type `dtype` (fused
+        where the GEMMs are fused) and fp32 vectors (biases, LayerNorm affine)."""
         a, c = self.attn, self.cross_attn
         sh: Dict[str, Tensor] = {}
-        sh["wqkv"], sh["bqkv"] = a.fused_qkv()
-        sh["wo"], sh["bo"] = a.out.weight_bf16(), _f32(a.out.bias)
+        sh["wqkv"], sh["bqkv"] = a.fused_qkv(dtype)
+        sh["wo"], sh["bo"] = a.out.weight16(dtype), _f32(a.out.bias)
         sh["ln1w"], sh["ln1b"] = _f32(self.attn_ln.weight), _f32(self.attn_ln.bias)
         if c is not None:
-            sh["wcq"], sh["bcq"] = c.query.weight_bf16(), _f32(c.query.bias)
-            sh["wckv"], sh["bckv"] = c.fused_kv()
-            sh["wco"], sh["bco"] = c.out.weight_bf16(), _f32(c.out.bias)
+            sh["wcq"], sh["bcq"] = c.query.weight16(dtype), _f32(c.query.bias)
+            sh["wckv"], sh["bckv"] = c.fused_kv(dtype)
+            sh["wco"], sh["bco"] = c.out.weight16(dtype), _f32(c.out.bias)
             sh["lncw"], sh["lncb"] = _f32(self.cross_attn_ln.weight), _f32(self.cross_attn_ln.bias)
-        sh["w1"], sh["b1"] = self.mlp[0].weight_bf16(), _f32(self.mlp[0].bias)
-        sh["w2"], sh["b2"] = self.mlp[2].weight_bf16(), _f32(self.mlp[2].bias)
+        sh["w1"], sh["b1"] = self.mlp[0].weight16(dtype), _f32(self.mlp[0].bias)
+        sh["w2"], sh["b2"] = self.mlp[2].weight16(dtype), _f32(self.mlp[2].bias)
         sh["ln2w"], sh["ln2b"] = _f32(self.mlp_ln.weight), _f32(self.mlp_ln.bias)
         return sh
 
-    def _shadows(self) -> Dict[str, Tensor]:
+    def _shadows(self, dtype: torch.dtype = torch.bfloat16) -> Dict[str, Tensor]:
         if self._slab_sh is not None:
-            return self._slab_sh
+            if dtype == torch.bfloat16:
+                return self._slab_sh
+            if self._slab_sh16 is None:     # the same slab bytes, read as fp16 (see _slab16)
+                self._slab_sh16 = {k: _slab16(v, torch.float16) if v.dtype == torch.bfloat16 else v for k, v in self._slab_sh.items()}
+            return self._slab_sh16
         if not _is_master(self.attn.query.weight):
             with torch.no_grad():
-                return self._build_shadows()        # FSDP mixed precision: parameters are transient views, never cached
-        return self._shadow.get([p for _, p in self.named_parameters()], self._build_shadows)
+                return self._build_shadows(dtype)   # FSDP mixed precision: parameters are transient views, never cached
+        return self._shadow.get([p for _, p in self.named_parameters()], lambda: self._build_shadows(dtype), dtype)
 
     def forward(self, x: Tensor, xa: Optional[Tensor] = None, mask: Optional[Tensor] = None,
                 kv_cache: Optional[dict] = None, verbose: bool = False, _xa_state: Optional[dict] = None):
@@ -632,20 +699,22 @@ class ResidualAttentionBlock(nn.Module):
             if mask.dim() == 3:
                 kv_len = kv_len_from_padding_mask(mask)
         Ta = xa.shape[1] if xa is not None else 0
-        xa2 = _as_bf16_2d(xa) if xa is not None else None
+        dt = x.dtype if x.dtype in K.ACT16 else torch.bfloat16
+        xa2 = _as16_2d(xa, dt) if xa is not None else None
         # attribute walk, not get_parameter(): under FSDP the attributes are plain tensor views of the flat parameter
         params = [_attr_by_path(self, n) for n in self._param_names]
-        y = _BlockFn.apply(self, B, T, Ta, causal, kv_len, _xa_state, _as_bf16_2d(x), xa2, *params)
+        y = _BlockFn.apply(self, B, T, Ta, causal, kv_len, _xa_state, _as16_2d(x, dt), xa2, *params)
         return y.view(B, T, d)
 
     def _forward_cached(self, x, xa, mask, kv_cache):
         """Decode path: unfused modules so that the forward hooks on key / value fire (model.py:925-964)."""
         B, T, d = x.shape
+        dt = compute_dtype()     # the type the Linear / LayerNorm modules below compute in
         x = x + self.attn(self.attn_ln(x), mask=mask, kv_cache=kv_cache)[0]
         if self.cross_attn is not None:
             x = x + self.cross_attn(self.cross_attn_ln(x), xa, kv_cache=kv_cache)[0]
-        h, g = linear_fwd(_as_bf16_2d(self.mlp_ln(x)), self.mlp[0].weight_bf16(), _f32(self.mlp[0].bias), epi=K.EPI_BF16_GELU)
-        y = linear_fwd(g, self.mlp[2].weight_bf16(), _f32(self.mlp[2].bias), epi=K.EPI_BF16_RESIDUAL, aux=_as_bf16_2d(x))
+        h, g = linear_fwd(_as16_2d(self.mlp_ln(x), dt), self.mlp[0].weight16(dt), _f32(self.mlp[0].bias), epi=K.EPI_BF16_GELU)
+        y = linear_fwd(g, self.mlp[2].weight16(dt), _f32(self.mlp[2].bias), epi=K.EPI_BF16_RESIDUAL, aux=_as16_2d(x, dt))
         return y.view(B, T, d)
 
 
@@ -657,17 +726,17 @@ class _StemFn(torch.autograd.Function):
     im2col + wgmma GEMM with fused bias/GELU epilogues, time-major throughout."""
 
     @staticmethod
-    def forward(ctx, enc, mel, w1, b1, w2, b2):
+    def forward(ctx, enc, mel, w1, b1, w2, b2, dtype=torch.bfloat16):
         B, C, T = mel.shape
         d = w1.shape[0]
         T2 = (T + 2 - 3) // 2 + 1
         mel = mel.contiguous()
         if mel.dtype != torch.float32:        # FSDP MixedPrecision hands the root module a bf16 mel, as it does to the reference
             mel = K.convert(mel, dtype=torch.float32)
-        A1 = K.im2col_conv1(mel, 3 * C)
-        pre1, h1 = linear_fwd(A1, enc.conv1.weight_bf16(), _f32(b1), epi=K.EPI_BF16_GELU)
+        A1 = K.im2col_conv1(mel, 3 * C, **_f16_kw(dtype))
+        pre1, h1 = linear_fwd(A1, enc.conv1.weight16(dtype), _f32(b1), epi=K.EPI_BF16_GELU)
         A2 = K.im2col_conv2(h1, B, T, d)
-        pre2, h2 = linear_fwd(A2, enc.conv2.weight_bf16(), _f32(b2), epi=K.EPI_BF16_GELU)
+        pre2, h2 = linear_fwd(A2, enc.conv2.weight16(dtype), _f32(b2), epi=K.EPI_BF16_GELU)
         x0 = K.add_pos(h2, _f32(enc.positional_embedding), T2)
         ctx.save_for_backward(A1, pre1, A2, pre2)
         ctx.enc, ctx.dims = enc, (B, C, T, T2, d)
@@ -682,12 +751,12 @@ class _StemFn(torch.autograd.Function):
         dpre2 = K.gelu_bwd(dx0.contiguous(), pre2)
         grads.keep("conv2.weight", K.unpermute_conv_wgrad(linear_wgrad(dpre2, A2), d, d, out=grads.out("conv2.weight")))
         grads.bias("conv2.bias", dpre2)
-        dA2 = linear_dgrad(dpre2, enc.conv2.weight_bf16())
+        dA2 = linear_dgrad(dpre2, enc.conv2.weight16(pre2.dtype))
         dpre1 = K.col2im_conv2_gelu_bwd(dA2, pre1, B, T, T2, d)
         grads.keep("conv1.weight", K.unpermute_conv_wgrad(linear_wgrad(dpre1, A1), d, C, out=grads.out("conv1.weight")))
         grads.bias("conv1.bias", dpre1)
         grads.done()     # last gradients of the whole backward pass
-        return (None, None, *grads.grads_for(("conv1.weight", "conv1.bias", "conv2.weight", "conv2.bias")))
+        return (None, None, *grads.grads_for(("conv1.weight", "conv1.bias", "conv2.weight", "conv2.bias")), None)
 
 
 class AudioEncoder(nn.Module):
@@ -706,13 +775,14 @@ class AudioEncoder(nn.Module):
         self._bwd_done_cb = None
 
     def forward(self, x: Tensor, verbose: bool = False):
+        dt = compute_dtype()
         if self._slabs is not None:
-            self._slabs.ensure_synced()
+            self._slabs.ensure_synced(dt)
         B = x.shape[0]
         n_ctx, d = self.positional_embedding.shape
         assert x.dim() == 3 and (x.shape[2] + 2 - 3) // 2 + 1 == n_ctx and x.shape[1] == self.conv1.in_channels, \
             "incorrect audio shape"
-        x0 = _StemFn.apply(self, x, self.conv1.weight, self.conv1.bias, self.conv2.weight, self.conv2.bias)
+        x0 = _StemFn.apply(self, x, self.conv1.weight, self.conv1.bias, self.conv2.weight, self.conv2.bias, dt)
         h = x0.view(B, n_ctx, d)
         for block in self.blocks:
             h = block(h)
@@ -744,11 +814,11 @@ class _LayerNormFn(torch.autograd.Function):
 # decoder
 # =====================================================================================================
 class _EmbedFn(torch.autograd.Function):
-    """(token_embedding(ids) + positional_embedding[offset:offset+S]).to(bf16)  (model.py:728-732)."""
+    """(token_embedding(ids) + positional_embedding[offset:offset+S]).to(dtype)  (model.py:728-732)."""
 
     @staticmethod
-    def forward(ctx, ids, emb, pos, offset, padding_idx, dec=None):
-        out = K.embed_fwd(ids.contiguous(), _f32(emb), _f32(pos), offset)
+    def forward(ctx, ids, emb, pos, offset, padding_idx, dec=None, dtype=torch.bfloat16):
+        out = K.embed_fwd(ids.contiguous(), _f32(emb), _f32(pos), offset, **_f16_kw(dtype))
         ctx.save_for_backward(ids)
         ctx.meta = (emb.shape, pos.shape, offset, padding_idx)
         ctx.dec = dec
@@ -764,7 +834,7 @@ class _EmbedFn(torch.autograd.Function):
         demb, dpos = grads.vec(names[0], eshape), grads.vec(names[1], pshape)
         K.embed_bwd(ids.contiguous(), dx.contiguous(), demb, dpos[offset:], pad)
         grads.done()     # decoder gradients (incl. the tied embedding) are final
-        return (None, *grads.grads_for(names), None, None, None)
+        return (None, *grads.grads_for(names), None, None, None, None)
 
 
 def _logits_ld(V: int) -> int:
@@ -778,7 +848,7 @@ class _LogitsFn(torch.autograd.Function):
     def forward(ctx, x, emb, emb_bf16, dec=None):
         M, d = x.shape
         V = emb.shape[0]
-        buf = torch.empty((M, _logits_ld(V)), device=x.device, dtype=torch.bfloat16)
+        buf = torch.empty((M, _logits_ld(V)), device=x.device, dtype=x.dtype)
         K.gemm(x, emb_bf16, M, V, d, out=buf, block_n=256)
         ctx.save_for_backward(x, emb_bf16)
         ctx.dec = dec
@@ -789,8 +859,8 @@ class _LogitsFn(torch.autograd.Function):
         x, emb_bf16 = ctx.saved_tensors
         M, d = x.shape
         V = emb_bf16.shape[0]
-        buf = torch.empty((M, _logits_ld(V)), device=x.device, dtype=torch.bfloat16)
-        buf[:, :V].copy_(dlogits)  # `.float()` backward: the gradient enters the matmul as bf16
+        buf = torch.empty((M, _logits_ld(V)), device=x.device, dtype=x.dtype)
+        buf[:, :V].copy_(dlogits)  # `.float()` backward: the gradient enters the matmul in the logits' 16-bit type
         dx = K.gemm(buf[:, :V], emb_bf16, M, d, V, b_mn=True, block_n=_pick_block_n(M, d))
         grads = _GradDest(ctx.dec)
         grads.weight("token_embedding.weight", buf, x, n_valid=V)
@@ -798,7 +868,7 @@ class _LogitsFn(torch.autograd.Function):
 
 
 class _LossHeadFn(torch.autograd.Function):
-    """Fused tail of the training step: tied logits GEMM (bf16, never widened to fp32) + token cross-entropy
+    """Fused tail of the training step: tied logits GEMM (16-bit, never widened to fp32) + token cross-entropy
     (model.py:768-770 followed by train_timestamps.py:1444-1448).  The backward turns the logits buffer into
     d(logits) in place and feeds it to the dgrad / wgrad GEMMs."""
 
@@ -807,7 +877,7 @@ class _LossHeadFn(torch.autograd.Function):
         ctx.dec = dec
         M, d = x.shape
         V = emb.shape[0]
-        buf = torch.empty((M, _logits_ld(V)), device=x.device, dtype=torch.bfloat16)
+        buf = torch.empty((M, _logits_ld(V)), device=x.device, dtype=x.dtype)
         K.gemm(x, emb_bf16, M, V, d, out=buf, block_n=256)
         t = targets.reshape(-1).contiguous()
         lse, lsc = K.ce_fwd(buf, t, V, ignore_index)
@@ -858,22 +928,29 @@ class TextDecoder(nn.Module):
         self._emb_slab_view: Optional[Tensor] = None
 
     def embedding_bf16(self) -> Tensor:
-        if self._emb_slab_view is not None:
-            return self._emb_slab_view
-        w = self.token_embedding.weight
-        if w.dtype == torch.bfloat16:
-            return w.detach()
-        return self._emb_shadow.get((w,), lambda: K.cast_bf16(w.detach().contiguous()))
+        return self.embedding16(torch.bfloat16)
 
-    def hidden(self, x: Tensor, xa: Tensor, kv_cache: Optional[dict] = None, padding_mask: Optional[Tensor] = None) -> Tensor:
-        """Everything up to and including the final LayerNorm: (B, S) ids -> (B*S, d) bf16."""
+    def embedding16(self, dtype: torch.dtype) -> Tensor:
+        if self._emb_slab_view is not None:
+            return _slab16(self._emb_slab_view, dtype)
+        w = self.token_embedding.weight
+        if w.dtype == dtype:
+            return w.detach()
+        if not _is_master(w):
+            return K.convert(w.detach().contiguous(), dtype=dtype)
+        return self._emb_shadow.get((w,), lambda: _cast16(w.detach().contiguous(), dtype), dtype)
+
+    def hidden(self, x: Tensor, xa: Tensor, kv_cache: Optional[dict] = None, padding_mask: Optional[Tensor] = None,
+               dtype: Optional[torch.dtype] = None) -> Tensor:
+        """Everything up to and including the final LayerNorm: (B, S) ids -> (B*S, d) in `dtype` (default: compute_dtype())."""
+        dt = compute_dtype() if dtype is None else dtype
         if self._slabs is not None:
-            self._slabs.ensure_synced()
+            self._slabs.ensure_synced(dt)
         offset = next(iter(kv_cache.values())).shape[1] if kv_cache else 0
         B, S = x.shape
         d = self.positional_embedding.shape[1]
         h = _EmbedFn.apply(x, self.token_embedding.weight, self.positional_embedding, offset,
-                           self.token_embedding.padding_idx, self).view(B, S, d)
+                           self.token_embedding.padding_idx, self, dt).view(B, S, d)
         mask = padding_mask if padding_mask is not None else self.mask[:S, :S]
         # shared accumulator of the layers' gradients w.r.t. the encoder output (see _BlockFn.backward); one per forward pass
         xa_state = {"buf": None, "left": len(self.blocks)} if (kv_cache is None and torch.is_grad_enabled() and xa.requires_grad) else None
@@ -885,13 +962,15 @@ class TextDecoder(nn.Module):
     def forward(self, x: Tensor, xa: Tensor, kv_cache: Optional[dict] = None, padding_mask: Optional[Tensor] = None,
                 verbose: bool = False):
         B, S = x.shape
-        h = self.hidden(x, xa, kv_cache, padding_mask)
-        logits = _LogitsFn.apply(h, self.token_embedding.weight, self.embedding_bf16(), self)
+        dt = compute_dtype()
+        h = self.hidden(x, xa, kv_cache, padding_mask, dt)
+        logits = _LogitsFn.apply(h, self.token_embedding.weight, self.embedding16(dt), self)
         return logits.view(B, S, -1)
 
     def loss(self, x: Tensor, xa: Tensor, targets: Tensor, padding_mask: Optional[Tensor] = None, ignore_index: int = PAD_ID_EN):
-        h = self.hidden(x, xa, None, padding_mask)
-        return _LossHeadFn.apply(h, self.token_embedding.weight, self.embedding_bf16(), targets, ignore_index, self)
+        dt = compute_dtype()
+        h = self.hidden(x, xa, None, padding_mask, dt)
+        return _LossHeadFn.apply(h, self.token_embedding.weight, self.embedding16(dt), targets, ignore_index, self)
 
 
 # =====================================================================================================
@@ -973,8 +1052,8 @@ class OLMoASRBase(nn.Module):
                 if members[0] + ".weight" in direct:
                     w = _attr_by_path(b, members[0]).weight
                     direct[name + ".weight"] = sl.span("G", w, len(members) * w.numel()).view(len(members) * w.shape[0], -1)
-            sh = b._build_shadows()      # slab views throughout: bf16 weights from S, fp32 vectors from P
-            b._slabs, b._slab_sh, b._direct = sl, sh, direct
+            sh = b._build_shadows()      # slab views throughout: 16-bit weights from S, fp32 vectors from P
+            b._slabs, b._slab_sh, b._slab_sh16, b._direct = sl, sh, None, direct
         enc._slabs, dec._slabs = sl, sl
         enc._direct, dec._direct = grad_views(enc), grad_views(dec)
         dec._emb_slab_view = sl.shadow(dec.token_embedding.weight)

@@ -131,6 +131,31 @@ _SIGNATURES = {
     "oasr_convert": [c_void_p, c_int, c_void_p, c_int, c_i64, c_void_p],
     "oasr_gemm_bf16": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_void_p, c_i64, c_void_p, c_void_p,
                        c_void_p, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_void_p],
+    # 16-bit activation dtype (OASR_DTYPE_BF16 / OASR_DTYPE_F16) before the stream
+    "oasr_gemm16": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_void_p, c_i64, c_void_p, c_void_p,
+                    c_void_p, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_int, c_void_p],
+    "oasr_layernorm_fwd16": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_float, c_int, c_void_p],
+    "oasr_layernorm_bwd16": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                             c_i64, c_i64, c_int, c_void_p],
+    "oasr_attention_fwd16": [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p,
+                             c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_void_p, c_float, c_int, c_void_p],
+    "oasr_attention_bwd16": [c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64,
+                             c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64,
+                             c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_void_p, c_float, c_int, c_void_p],
+    "oasr_ce_fwd16": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_i64, c_int, c_void_p],
+    "oasr_ce_bwd16": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_i64, c_int, c_void_p],
+    "oasr_logits_to_f32_16": [c_void_p, c_void_p, c_i64, c_i64, c_i64, c_int, c_void_p],
+    "oasr_embed_fwd16": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_void_p],
+    "oasr_embed_bwd16": [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_void_p],
+    "oasr_cast_conv_weight16": [c_void_p, c_void_p, c_i64, c_i64, c_int, c_void_p],
+    "oasr_im2col_conv1_16": [c_void_p, c_void_p, c_i64, c_i64, c_i64, c_i64, c_int, c_void_p],
+    "oasr_col2im_conv2_gelu_bwd16": [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_i64, c_int, c_void_p],
+    "oasr_add_pos16": [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_int, c_void_p],
+    "oasr_gelu_bwd16": [c_void_p, c_void_p, c_void_p, c_i64, c_int, c_void_p],
+    "oasr_colsum16": [c_void_p, c_void_p, c_i64, c_i64, c_i64, c_int, c_void_p],
+    "oasr_adamw_flat16": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_void_p, c_float, c_float, c_float,
+                          c_float, c_float, c_int, c_void_p],
+    "oasr_optim_prepare_amp": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_void_p],
 }
 _RESTYPES = {"oasr_last_error": ctypes.c_char_p}
 
@@ -193,7 +218,8 @@ def stream():
 _LAUNCHES_PER_CALL = {"oasr_logmel": 3, "oasr_attention_bwd": 3, "oasr_dec_attention": 2, "oasr_dec_sample": 2,
                       "oasr_dec_sample_rules": 2, "oasr_dec_attention_grouped": 2, "oasr_dec_beam_select": 2,
                       "oasr_ce_fwd": 2, "oasr_colsum_bf16": 2, "oasr_layernorm_bwd": 3, "oasr_grad_sqnorm": 2,
-                      "oasr_grad_sqnorm_flat": 2}
+                      "oasr_grad_sqnorm_flat": 2, "oasr_attention_bwd16": 3, "oasr_ce_fwd16": 2, "oasr_colsum16": 2,
+                      "oasr_layernorm_bwd16": 3}
 LAUNCH_COUNT = 0
 
 

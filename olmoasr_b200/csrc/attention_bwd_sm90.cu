@@ -35,9 +35,9 @@ constexpr int BWD_THREADS = 256;
 struct BwdParams {
   const float* lse;   // (B,H,Tq) log2 domain
   const float* delta; // (B,H,Tq) rowsum(dO o O)
-  bf16* dq;
-  bf16* dk;
-  bf16* dv;
+  void* dq;
+  void* dk;
+  void* dv;
   int64_t lddq, lddk, lddv;
   const int32_t* kv_len;
   int B, H, Tq, Tkv;
@@ -45,6 +45,7 @@ struct BwdParams {
   float scale, scale_log2;
 };
 
+template <typename T>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdParams p) {
@@ -128,15 +129,15 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       const uint64_t q_desc = ptx::desc_sw128(sQ, 16, 1024), do_desc = ptx::desc_sw128(sdO, 16, 1024);
       ptx::wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n64k16_ss<0, 0>(s, ptx::desc_add(k_desc, 32 * k), ptx::desc_add(q_desc, 32 * k), k > 0);
+      for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n64k16_ss<0, 0, T>(s, ptx::desc_add(k_desc, 32 * k), ptx::desc_add(q_desc, 32 * k), k > 0);
 #pragma unroll
-      for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n64k16_ss<0, 0>(dp, ptx::desc_add(v_desc, 32 * k), ptx::desc_add(do_desc, 32 * k), k > 0);
+      for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n64k16_ss<0, 0, T>(dp, ptx::desc_add(v_desc, 32 * k), ptx::desc_add(do_desc, 32 * k), k > 0);
       ptx::wgmma_commit();
       ptx::wgmma_wait<0>();
       ptx::fence_regs(s);
       ptx::fence_regs(dp);
 
-      // P^T, dS^T; packed to bf16 in the A-fragment order (k = queries)
+      // P^T, dS^T; packed to T in the A-fragment order (k = queries)
       uint32_t pa[4][4], da[4][4];
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -152,8 +153,8 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
             pe[e] = vis ? fast_exp2(fmaf(s[x], c, -lse_c[2 * i + e])) : 0.f;
             ds[e] = pe[e] * (dp[x] - dlt_c[2 * i + e]);
           }
-          pa[i >> 1][(i & 1) * 2 + hh] = pack_bf16x2(pe[0], pe[1]);
-          da[i >> 1][(i & 1) * 2 + hh] = pack_bf16x2(ds[0], ds[1]);
+          pa[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(pe[0], pe[1]);
+          da[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(ds[0], ds[1]);
         }
       }
 
@@ -161,8 +162,8 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       ptx::wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < BQ / 16; ++kk) {
-        ptx::wgmma_m64n64k16_rs<1>(dv, pa[kk], ptx::desc_add(doB_desc, 2048 * kk), 1u);
-        ptx::wgmma_m64n64k16_rs<1>(dk, da[kk], ptx::desc_add(qB_desc, 2048 * kk), 1u);
+        ptx::wgmma_m64n64k16_rs<1, T>(dv, pa[kk], ptx::desc_add(doB_desc, 2048 * kk), 1u);
+        ptx::wgmma_m64n64k16_rs<1, T>(dk, da[kk], ptx::desc_add(qB_desc, 2048 * kk), 1u);
       }
       ptx::wgmma_commit();
       ptx::wgmma_wait<0>();
@@ -177,12 +178,12 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   for (int hh = 0; hh < 2; ++hh) {
     const int key = kv0 + key_loc + 8 * hh;
     if (key < p.Tkv) {
-      bf16* dvp = p.dv + (static_cast<int64_t>(b) * p.Tkv + key) * p.lddv + h * HD + qc;
-      bf16* dkp = p.dk + (static_cast<int64_t>(b) * p.Tkv + key) * p.lddk + h * HD + qc;
+      T* dvp = static_cast<T*>(p.dv) + (static_cast<int64_t>(b) * p.Tkv + key) * p.lddv + h * HD + qc;
+      T* dkp = static_cast<T*>(p.dk) + (static_cast<int64_t>(b) * p.Tkv + key) * p.lddk + h * HD + qc;
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        *reinterpret_cast<uint32_t*>(dvp + 8 * i) = pack_bf16x2(dv[4 * i + 2 * hh], dv[4 * i + 2 * hh + 1]);
-        *reinterpret_cast<uint32_t*>(dkp + 8 * i) = pack_bf16x2(dk[4 * i + 2 * hh] * p.scale, dk[4 * i + 2 * hh + 1] * p.scale);
+        *reinterpret_cast<uint32_t*>(dvp + 8 * i) = Act16<T>::pack2(dv[4 * i + 2 * hh], dv[4 * i + 2 * hh + 1]);
+        *reinterpret_cast<uint32_t*>(dkp + 8 * i) = Act16<T>::pack2(dk[4 * i + 2 * hh] * p.scale, dk[4 * i + 2 * hh + 1] * p.scale);
       }
     }
   }
@@ -195,6 +196,7 @@ constexpr int DQ_TILE = 128 * HD * 2;                            // 16 KB
 constexpr int DQ_TILES = 2 * DQ_TILE /*Q, dO*/ + 2 * 2 * DQ_TILE /*K, V x 2 stages*/;   // 96 KB
 constexpr int DQ_SMEM = DQ_TILES + 1024 /*barriers*/ + 1024 /*alignment slack*/;
 
+template <typename T>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                         const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const BwdParams p) {
@@ -268,15 +270,15 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
     const uint64_t k_desc = ptx::desc_sw128(sK, 16, 1024), v_desc = ptx::desc_sw128(sV, 16, 1024);
     ptx::wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n128k16_ss<0, 0>(s, ptx::desc_add(q_desc, 32 * k), ptx::desc_add(k_desc, 32 * k), k > 0);
+    for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n128k16_ss<0, 0, T>(s, ptx::desc_add(q_desc, 32 * k), ptx::desc_add(k_desc, 32 * k), k > 0);
 #pragma unroll
-    for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n128k16_ss<0, 0>(dp, ptx::desc_add(do_desc, 32 * k), ptx::desc_add(v_desc, 32 * k), k > 0);
+    for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n128k16_ss<0, 0, T>(dp, ptx::desc_add(do_desc, 32 * k), ptx::desc_add(v_desc, 32 * k), k > 0);
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
     ptx::fence_regs(s);
     ptx::fence_regs(dp);
 
-    // dS = P o (dP - D), P = 2^(S c - LSE) on the visible keys [0, limit); packed to bf16 in the A-fragment order (k = keys)
+    // dS = P o (dP - D), P = 2^(S c - LSE) on the visible keys [0, limit); packed to T in the A-fragment order (k = keys)
     const int k0 = j * DQ_BKV;
     uint32_t da[8][4];
 #pragma unroll
@@ -294,13 +296,13 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
           const float pe = (8 * i + kc + e < limit) ? fast_exp2(fmaf(s[x], c, -lse_r[hh])) : 0.f;
           ds[e] = pe * (dp[x] - dlt_r[hh]);
         }
-        da[i >> 1][(i & 1) * 2 + hh] = pack_bf16x2(ds[0], ds[1]);
+        da[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(ds[0], ds[1]);
       }
     }
     const uint64_t kB_desc = ptx::desc_sw128(sK, DQ_BKV * 128, 1024);   // K as the MN-major B operand (keys are k)
     ptx::wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < DQ_BKV / 16; ++kk) ptx::wgmma_m64n64k16_rs<1>(dq, da[kk], ptx::desc_add(kB_desc, 2048 * kk), 1u);
+    for (int kk = 0; kk < DQ_BKV / 16; ++kk) ptx::wgmma_m64n64k16_rs<1, T>(dq, da[kk], ptx::desc_add(kB_desc, 2048 * kk), 1u);
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
     ptx::fence_regs(dq);
@@ -310,15 +312,16 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     if (!q_ok[hh]) continue;
-    bf16* dst = p.dq + (static_cast<int64_t>(b) * p.Tq + q_base + r_loc + 8 * hh) * p.lddq + h * HD + kc;
+    T* dst = static_cast<T*>(p.dq) + (static_cast<int64_t>(b) * p.Tq + q_base + r_loc + 8 * hh) * p.lddq + h * HD + kc;
 #pragma unroll
     for (int i = 0; i < 8; ++i)
-      *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16x2(dq[4 * i + 2 * hh] * p.scale, dq[4 * i + 2 * hh + 1] * p.scale);
+      *reinterpret_cast<uint32_t*>(dst + 8 * i) = Act16<T>::pack2(dq[4 * i + 2 * hh] * p.scale, dq[4 * i + 2 * hh + 1] * p.scale);
   }
 }
 
 // delta[b,h,q] = sum_d dO[b,q,h,d] * O[b,q,h,d]   (8 lanes per (row, head), 16-byte loads, 3 shuffle steps)
-__global__ void attention_delta_kernel(const bf16* __restrict__ o, const bf16* __restrict__ dout, float* __restrict__ delta,
+template <typename T>
+__global__ void attention_delta_kernel(const T* __restrict__ o, const T* __restrict__ dout, float* __restrict__ delta,
                                        int64_t ldo, int64_t lddo, int B, int H, int Tq) {
   const int64_t item = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 3;  // (row, head) pair
   const int sub = threadIdx.x & 7;
@@ -334,7 +337,7 @@ __global__ void attention_delta_kernel(const bf16* __restrict__ o, const bf16* _
     const uint32_t av[4] = {a.x, a.y, a.z, a.w}, gv[4] = {g.x, g.y, g.z, g.w};
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const float2 p = unpack_bf16x2(av[j]), q = unpack_bf16x2(gv[j]);
+      const float2 p = Act16<T>::unpack2(av[j]), q = Act16<T>::unpack2(gv[j]);
       s += p.x * q.x + p.y * q.y;
     }
   }
@@ -347,16 +350,11 @@ __global__ void attention_delta_kernel(const bf16* __restrict__ o, const bf16* _
   }
 }
 
-}  // namespace
-}  // namespace oasr
-
-using namespace oasr;
-
-extern "C" int oasr_attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
-                                  const void* o, int64_t ldo, const void* dout, int64_t lddo, const float* lse,
-                                  float* delta, void* dq, int64_t lddq, void* dk, int64_t lddk,
-                                  void* dv, int64_t lddv, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
-                                  int64_t head_dim, int causal, const int32_t* kv_len, float scale, void* stream) {
+template <typename T>
+int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* o,
+                  int64_t ldo, const void* dout, int64_t lddo, const float* lse, float* delta, void* dq, int64_t lddq,
+                  void* dk, int64_t lddk, void* dv, int64_t lddv, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
+                  int64_t head_dim, int causal, const int32_t* kv_len, float scale, void* stream) {
   OASR_REQUIRE(head_dim == HD, "attention_bwd: head_dim %ld unsupported", (long)head_dim);
   OASR_REQUIRE(B > 0 && H > 0 && Tq > 0 && Tkv > 0, "attention_bwd: empty problem");
   OASR_REQUIRE(((ldq | ldk | ldv | ldo | lddo | lddq | lddk | lddv) & 7) == 0, "attention_bwd: strides must be multiples of 8");
@@ -367,36 +365,60 @@ extern "C" int oasr_attention_bwd(const void* q, int64_t ldq, const void* k, int
   OASR_REQUIRE(B <= 65535 && H <= 65535, "attention_bwd: B and H must fit the grid");
   cudaStream_t st = (cudaStream_t)stream;
   CUtensorMap tmQ, tmK, tmV, tmdO, tmQ128, tmdO128;
+  constexpr bool f16 = Act16<T>::is_fp16;
   int rc;
-  if ((rc = make_tmap_2d(&tmQ, q, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)ldq * 2, HD, BQ, true))) return rc;
-  if ((rc = make_tmap_2d(&tmK, k, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldk * 2, HD, BKV, true))) return rc;
-  if ((rc = make_tmap_2d(&tmV, v, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldv * 2, HD, BKV, true))) return rc;
-  if ((rc = make_tmap_2d(&tmdO, dout, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)lddo * 2, HD, BQ, true))) return rc;
-  if ((rc = make_tmap_2d(&tmQ128, q, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)ldq * 2, HD, DQ_BQ, true))) return rc;
-  if ((rc = make_tmap_2d(&tmdO128, dout, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)lddo * 2, HD, DQ_BQ, true))) return rc;
+  if ((rc = make_tmap_2d(&tmQ, q, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)ldq * 2, HD, BQ, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmK, k, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldk * 2, HD, BKV, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmV, v, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldv * 2, HD, BKV, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmdO, dout, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)lddo * 2, HD, BQ, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmQ128, q, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)ldq * 2, HD, DQ_BQ, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmdO128, dout, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)lddo * 2, HD, DQ_BQ, true, f16))) return rc;
 
   const int64_t n_rows = B * Tq * H;
-  attention_delta_kernel<<<(unsigned)ceil_div(n_rows * 8, 256), 256, 0, st>>>((const bf16*)o, (const bf16*)dout, delta, ldo, lddo,
+  attention_delta_kernel<T><<<(unsigned)ceil_div(n_rows * 8, 256), 256, 0, st>>>((const T*)o, (const T*)dout, delta, ldo, lddo,
                                                                               (int)B, (int)H, (int)Tq);
   OASR_LAUNCH_CHECK();
 
   BwdParams p;
   p.lse = lse; p.delta = delta; p.kv_len = kv_len;
-  p.dq = static_cast<bf16*>(dq); p.dk = static_cast<bf16*>(dk); p.dv = static_cast<bf16*>(dv);
+  p.dq = dq; p.dk = dk; p.dv = dv;
   p.lddq = lddq; p.lddk = lddk; p.lddv = lddv;
   p.B = (int)B; p.H = (int)H; p.Tq = (int)Tq; p.Tkv = (int)Tkv; p.causal = causal;
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
   static bool attr_set = false;
   if (!attr_set) {
-    OASR_CUDA_OK(cudaFuncSetAttribute(attention_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
-    OASR_CUDA_OK(cudaFuncSetAttribute(attention_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DQ_SMEM));
+    OASR_CUDA_OK(cudaFuncSetAttribute(attention_bwd_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM));
+    OASR_CUDA_OK(cudaFuncSetAttribute(attention_bwd_dq_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, DQ_SMEM));
     attr_set = true;
   }
   const dim3 grid((unsigned)ceil_div(Tkv, BKV), (unsigned)H, (unsigned)B);
-  attention_bwd_kernel<<<grid, BWD_THREADS, BWD_SMEM, st>>>(tmQ, tmK, tmV, tmdO, p);
+  attention_bwd_kernel<T><<<grid, BWD_THREADS, BWD_SMEM, st>>>(tmQ, tmK, tmV, tmdO, p);
   OASR_LAUNCH_CHECK();
   const dim3 grid_dq((unsigned)ceil_div(Tq, DQ_BQ), (unsigned)H, (unsigned)B);
-  attention_bwd_dq_kernel<<<grid_dq, BWD_THREADS, DQ_SMEM, st>>>(tmQ128, tmK, tmV, tmdO128, p);
+  attention_bwd_dq_kernel<T><<<grid_dq, BWD_THREADS, DQ_SMEM, st>>>(tmQ128, tmK, tmV, tmdO128, p);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
+}
+
+}  // namespace
+}  // namespace oasr
+
+using namespace oasr;
+
+extern "C" int oasr_attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                  const void* o, int64_t ldo, const void* dout, int64_t lddo, const float* lse,
+                                  float* delta, void* dq, int64_t lddq, void* dk, int64_t lddk,
+                                  void* dv, int64_t lddv, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
+                                  int64_t head_dim, int causal, const int32_t* kv_len, float scale, void* stream) {
+  return attention_bwd<bf16>(q, ldq, k, ldk, v, ldv, o, ldo, dout, lddo, lse, delta, dq, lddq, dk, lddk, dv, lddv, B, H, Tq,
+                             Tkv, head_dim, causal, kv_len, scale, stream);
+}
+
+extern "C" int oasr_attention_bwd16(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                    const void* o, int64_t ldo, const void* dout, int64_t lddo, const float* lse,
+                                    float* delta, void* dq, int64_t lddq, void* dk, int64_t lddk,
+                                    void* dv, int64_t lddv, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
+                                    int64_t head_dim, int causal, const int32_t* kv_len, float scale, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, attention_bwd, q, ldq, k, ldk, v, ldv, o, ldo, dout, lddo, lse, delta, dq, lddq, dk, lddk, dv,
+                         lddv, B, H, Tq, Tkv, head_dim, causal, kv_len, scale, stream);
 }

@@ -1,6 +1,6 @@
 // Flash-style attention forward for head_dim 64 on wgmma (sm_90a).
 //
-//   O = softmax(Q K^T * scale + mask) V        per (batch, head); bf16 in/out, fp32 softmax
+//   O = softmax(Q K^T * scale + mask) V        per (batch, head); bf16 or fp16 in/out, fp32 softmax
 //
 // Replaces F.scaled_dot_product_attention in MultiHeadAttention.forward (olmoasr/model.py:331-340):
 //   encoder self-attention (no mask), decoder self-attention (causal + per-sample key length, derived
@@ -31,7 +31,7 @@ constexpr int ATT_SMEM = ATT_TILES + 1024 /*barriers*/ + 1024 /*alignment slack*
 constexpr int THREADS = 256;
 
 struct AttnParams {
-  bf16* o;
+  void* o;
   int64_t ldo;
   float* lse;        // (B, H, Tq) log2-domain log-sum-exp, nullable
   const int32_t* kv_len;  // (B,) valid keys per sample, nullable
@@ -49,6 +49,7 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
+template <typename T>
 __global__ void __launch_bounds__(THREADS, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
@@ -110,7 +111,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     const uint64_t k_desc = ptx::desc_sw128(sK, 16, 1024);
     ptx::wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n128k16_ss<0, 0>(s, ptx::desc_add(q_desc, 32 * k), ptx::desc_add(k_desc, 32 * k), k > 0);
+    for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n128k16_ss<0, 0, T>(s, ptx::desc_add(q_desc, 32 * k), ptx::desc_add(k_desc, 32 * k), k > 0);
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
     ptx::fence_regs(s);
@@ -144,7 +145,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       m[hh] = m_new;
       l[hh] *= alpha[hh];
     }
-    // p = 2^(s c - m c); P packed to bf16 in the A-fragment order of the P V MMA
+    // p = 2^(s c - m c); P packed to T in the A-fragment order of the P V MMA
     uint32_t pa[8][4];
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
@@ -153,7 +154,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         const float p0 = fast_exp2(fmaf(s[4 * i + 2 * hh], c, neg[hh]));
         const float p1 = fast_exp2(fmaf(s[4 * i + 2 * hh + 1], c, neg[hh]));
         l[hh] += p0 + p1;
-        pa[i >> 1][(i & 1) * 2 + hh] = pack_bf16x2(p0, p1);
+        pa[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(p0, p1);
       }
     }
 #pragma unroll
@@ -164,27 +165,59 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     const uint64_t v_desc = ptx::desc_sw128(sV, BKV * 128, 1024);
     ptx::wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < BKV / 16; ++kk) ptx::wgmma_m64n64k16_rs<1>(o, pa[kk], ptx::desc_add(v_desc, 2048 * kk), 1u);
+    for (int kk = 0; kk < BKV / 16; ++kk) ptx::wgmma_m64n64k16_rs<1, T>(o, pa[kk], ptx::desc_add(v_desc, 2048 * kk), 1u);
     ptx::wgmma_commit();
     ptx::wgmma_wait<0>();
     ptx::fence_regs(o);
     __syncthreads();   // both warpgroups are done with this stage: it may be refilled
   }
 
-  // ---- output: O / l -> bf16, rows past Tq are not written; lse in the log2 domain
+  // ---- output: O / l -> T, rows past Tq are not written; lse in the log2 domain
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const float lsum = quad_sum(l[hh]);
     const float inv = 1.f / lsum;
     const int qi = q_base + r_loc + 8 * hh;
     if (qi < p.Tq) {
-      bf16* dst = p.o + (static_cast<int64_t>(b) * p.Tq + qi) * p.ldo + h * HD + 2 * (lane & 3);
+      T* dst = static_cast<T*>(p.o) + (static_cast<int64_t>(b) * p.Tq + qi) * p.ldo + h * HD + 2 * (lane & 3);
 #pragma unroll
       for (int i = 0; i < 8; ++i)
-        *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_bf16x2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
+        *reinterpret_cast<uint32_t*>(dst + 8 * i) = Act16<T>::pack2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
       if (p.lse && (lane & 3) == 0) p.lse[(static_cast<int64_t>(b) * p.H + h) * p.Tq + qi] = m[hh] * c + log2f(lsum);
     }
   }
+}
+
+template <typename T>
+int attention_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o, int64_t ldo,
+                  float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tkv, int64_t head_dim, int causal,
+                  const int32_t* kv_len, float scale, void* stream) {
+  OASR_REQUIRE(head_dim == HD, "attention: head_dim %ld unsupported (every OLMoASR variant uses 64)", (long)head_dim);
+  OASR_REQUIRE(B > 0 && H > 0 && Tq > 0 && Tkv > 0, "attention: empty problem");
+  OASR_REQUIRE((ldq & 7) == 0 && (ldk & 7) == 0 && (ldv & 7) == 0 && (ldo & 7) == 0, "attention: strides must be multiples of 8");
+  OASR_REQUIRE((reinterpret_cast<uintptr_t>(o) & 3) == 0, "attention: output must be 4-byte aligned");
+  OASR_REQUIRE(!causal || Tq == Tkv, "attention: causal needs Tq == Tkv");
+  OASR_REQUIRE(B <= 65535 && H <= 65535, "attention: B and H must fit the grid");
+  CUtensorMap tmQ, tmK, tmV;
+  constexpr bool f16 = Act16<T>::is_fp16;
+  int rc;
+  if ((rc = make_tmap_2d(&tmQ, q, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)ldq * 2, HD, BQ, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmK, k, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldk * 2, HD, BKV, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmV, v, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldv * 2, HD, BKV, true, f16))) return rc;
+  AttnParams p;
+  p.o = o; p.ldo = ldo;
+  p.lse = lse; p.kv_len = kv_len;
+  p.B = (int)B; p.H = (int)H; p.Tq = (int)Tq; p.Tkv = (int)Tkv; p.causal = causal;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  static bool attr_set = false;
+  if (!attr_set) {
+    OASR_CUDA_OK(cudaFuncSetAttribute(attention_fwd_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+    attr_set = true;
+  }
+  const dim3 grid((unsigned)ceil_div(Tq, BQ), (unsigned)H, (unsigned)B);
+  attention_fwd_kernel<T><<<grid, THREADS, ATT_SMEM, (cudaStream_t)stream>>>(tmQ, tmK, tmV, p);
+  OASR_LAUNCH_CHECK();
+  return OASR_OK;
 }
 
 }  // namespace
@@ -195,29 +228,12 @@ using namespace oasr;
 extern "C" int oasr_attention_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
                                   void* o, int64_t ldo, float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
                                   int64_t head_dim, int causal, const int32_t* kv_len, float scale, void* stream) {
-  OASR_REQUIRE(head_dim == HD, "attention: head_dim %ld unsupported (every OLMoASR variant uses 64)", (long)head_dim);
-  OASR_REQUIRE(B > 0 && H > 0 && Tq > 0 && Tkv > 0, "attention: empty problem");
-  OASR_REQUIRE((ldq & 7) == 0 && (ldk & 7) == 0 && (ldv & 7) == 0 && (ldo & 7) == 0, "attention: strides must be multiples of 8");
-  OASR_REQUIRE((reinterpret_cast<uintptr_t>(o) & 3) == 0, "attention: output must be 4-byte aligned");
-  OASR_REQUIRE(!causal || Tq == Tkv, "attention: causal needs Tq == Tkv");
-  OASR_REQUIRE(B <= 65535 && H <= 65535, "attention: B and H must fit the grid");
-  CUtensorMap tmQ, tmK, tmV;
-  int rc;
-  if ((rc = make_tmap_2d(&tmQ, q, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)ldq * 2, HD, BQ, true))) return rc;
-  if ((rc = make_tmap_2d(&tmK, k, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldk * 2, HD, BKV, true))) return rc;
-  if ((rc = make_tmap_2d(&tmV, v, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldv * 2, HD, BKV, true))) return rc;
-  AttnParams p;
-  p.o = static_cast<bf16*>(o); p.ldo = ldo;
-  p.lse = lse; p.kv_len = kv_len;
-  p.B = (int)B; p.H = (int)H; p.Tq = (int)Tq; p.Tkv = (int)Tkv; p.causal = causal;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  static bool attr_set = false;
-  if (!attr_set) {
-    OASR_CUDA_OK(cudaFuncSetAttribute(attention_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-    attr_set = true;
-  }
-  const dim3 grid((unsigned)ceil_div(Tq, BQ), (unsigned)H, (unsigned)B);
-  attention_fwd_kernel<<<grid, THREADS, ATT_SMEM, (cudaStream_t)stream>>>(tmQ, tmK, tmV, p);
-  OASR_LAUNCH_CHECK();
-  return OASR_OK;
+  return attention_fwd<bf16>(q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Tq, Tkv, head_dim, causal, kv_len, scale, stream);
+}
+
+extern "C" int oasr_attention_fwd16(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                    void* o, int64_t ldo, float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
+                                    int64_t head_dim, int causal, const int32_t* kv_len, float scale, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, attention_fwd, q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Tq, Tkv, head_dim, causal, kv_len,
+                         scale, stream);
 }

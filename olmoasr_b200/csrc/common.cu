@@ -50,8 +50,9 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-static CUtensorMapDataType dtype_of(int elt_bytes) {
-  return elt_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+static CUtensorMapDataType dtype_of(int elt_bytes, bool fp16) {
+  if (elt_bytes == 2) return fp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  return CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
 }
 
 // Host-side cache of encoded tensor maps.  A training step encodes ~3000 of them (3-7 per GEMM / attention launch) and the
@@ -63,10 +64,10 @@ struct TmapKey {
   uintptr_t base;
   uint64_t d0, d1, d2, s1, s2;
   uint32_t b0, b1, b2;
-  int32_t elt, swz, rank;
+  int32_t dtype, swz, rank;   // dtype: the CUtensorMapDataType
   bool operator==(const TmapKey& o) const {
     return base == o.base && d0 == o.d0 && d1 == o.d1 && d2 == o.d2 && s1 == o.s1 && s2 == o.s2 && b0 == o.b0 && b1 == o.b1 &&
-           b2 == o.b2 && elt == o.elt && swz == o.swz && rank == o.rank;
+           b2 == o.b2 && dtype == o.dtype && swz == o.swz && rank == o.rank;
   }
 };
 struct TmapKeyHash {
@@ -74,7 +75,7 @@ struct TmapKeyHash {
     uint64_t h = 0x9E3779B97F4A7C15ull;
     auto mix = [&h](uint64_t v) { h ^= v + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2); };
     mix(k.base); mix(k.d0); mix(k.d1); mix(k.d2); mix(k.s1); mix(k.s2);
-    mix((uint64_t(k.b0) << 32) | k.b1); mix((uint64_t(k.b2) << 32) | uint32_t(k.elt));
+    mix((uint64_t(k.b0) << 32) | k.b1); mix((uint64_t(k.b2) << 32) | uint32_t(k.dtype));
     mix((uint64_t(uint32_t(k.swz)) << 32) | uint32_t(k.rank));
     return static_cast<size_t>(h);
   }
@@ -104,25 +105,25 @@ void tmap_store(const TmapKey& k, const CUtensorMap& m) {
 }  // namespace
 
 int make_tmap_2d(CUtensorMap* out, const void* base, int elt_bytes, uint64_t inner, uint64_t outer,
-                 uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle128) {
-  return make_tmap_2d_sw(out, base, elt_bytes, inner, outer, row_stride_bytes, box_inner, box_outer, swizzle128 ? 128 : 0);
+                 uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle128, bool fp16) {
+  return make_tmap_2d_sw(out, base, elt_bytes, inner, outer, row_stride_bytes, box_inner, box_outer, swizzle128 ? 128 : 0, fp16);
 }
 
 int make_tmap_2d_sw(CUtensorMap* out, const void* base, int elt_bytes, uint64_t inner, uint64_t outer,
-                    uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, int swizzle_bytes) {
+                    uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, int swizzle_bytes, bool fp16) {
   EncodeTiledFn enc = get_encode();
   OASR_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
   OASR_REQUIRE((row_stride_bytes & 15) == 0, "tensor map: row stride %llu B not a multiple of 16",
                (unsigned long long)row_stride_bytes);
   OASR_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "tensor map: base not 16-byte aligned");
-  const TmapKey key{reinterpret_cast<uintptr_t>(base), inner, outer, 0, row_stride_bytes, 0, box_inner, box_outer, 0, elt_bytes,
-                    swizzle_bytes, 2};
+  const TmapKey key{reinterpret_cast<uintptr_t>(base), inner, outer, 0, row_stride_bytes, 0, box_inner, box_outer, 0,
+                    (int32_t)dtype_of(elt_bytes, fp16), swizzle_bytes, 2};
   if (tmap_lookup(key, out)) return OASR_OK;
   cuuint64_t dims[2] = {inner, outer};
   cuuint64_t strides[1] = {row_stride_bytes};
   cuuint32_t box[2] = {box_inner, box_outer};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(out, dtype_of(elt_bytes), 2, const_cast<void*>(base), dims, strides, box, estr,
+  CUresult r = enc(out, dtype_of(elt_bytes, fp16), 2, const_cast<void*>(base), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE,
                    swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
                                         : (swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE),
@@ -140,14 +141,14 @@ int make_tmap_3d(CUtensorMap* out, const void* base, int elt_bytes, uint64_t d0,
   EncodeTiledFn enc = get_encode();
   OASR_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
   OASR_REQUIRE((stride1_bytes & 15) == 0 && (stride2_bytes & 15) == 0, "tensor map: strides must be multiples of 16 B");
-  const TmapKey key{reinterpret_cast<uintptr_t>(base), d0, d1, d2, stride1_bytes, stride2_bytes, b0, b1, b2, elt_bytes,
+  const TmapKey key{reinterpret_cast<uintptr_t>(base), d0, d1, d2, stride1_bytes, stride2_bytes, b0, b1, b2, (int32_t)dtype_of(elt_bytes, false),
                     swizzle128 ? 128 : 0, 3};
   if (tmap_lookup(key, out)) return OASR_OK;
   cuuint64_t dims[3] = {d0, d1, d2};
   cuuint64_t strides[2] = {stride1_bytes, stride2_bytes};
   cuuint32_t box[3] = {b0, b1, b2};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(out, dtype_of(elt_bytes), 3, const_cast<void*>(base), dims, strides, box, estr,
+  CUresult r = enc(out, dtype_of(elt_bytes, false), 3, const_cast<void*>(base), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE,
                    swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

@@ -3,6 +3,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -11,6 +12,7 @@
 namespace oasr {
 
 typedef __nv_bfloat16 bf16;
+typedef __half f16;
 
 #define OASR_CUDA_OK(expr)                                                                   \
   do {                                                                                       \
@@ -38,11 +40,12 @@ int num_sms();
 // `row_stride_bytes` between rows, box = box_inner x box_outer, 128-byte swizzle when
 // swizzle128 (box_inner * elt must then be 128 bytes).
 int gemm_sm_budget();   // SMs the persistent GEMM may occupy (oasr_gemm_set_sm_budget)
+// elt_bytes is 2 or 4 (f32); 2-byte maps are bf16, or IEEE fp16 when fp16.
 int make_tmap_2d(CUtensorMap* out, const void* base, int elt_bytes, uint64_t inner, uint64_t outer,
-                 uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle128);
+                 uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle128, bool fp16 = false);
 // swizzle_bytes: 0 (none), 64 or 128
 int make_tmap_2d_sw(CUtensorMap* out, const void* base, int elt_bytes, uint64_t inner, uint64_t outer,
-                    uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, int swizzle_bytes);
+                    uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer, int swizzle_bytes, bool fp16 = false);
 int make_tmap_3d(CUtensorMap* out, const void* base, int elt_bytes, uint64_t d0, uint64_t d1,
                  uint64_t d2, uint64_t stride1_bytes, uint64_t stride2_bytes, uint32_t b0,
                  uint32_t b1, uint32_t b2, bool swizzle128);
@@ -149,6 +152,43 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
 __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {   // one shift + one mask (the intrinsic costs 4-5 PRMT / IMAD)
   return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u));
 }
+
+// The two 16-bit activation types: bf16 (the default, and bf16 autocast) and fp16 (torch.autocast(float16)).  Kernels
+// that read or write activations take one of them as a template parameter; the arithmetic is fp32 in both and only
+// these conversions differ.  fp16 conversions round to nearest and give +-inf outside +-65504, as torch's casts do.
+template <typename T>
+struct Act16;
+template <>
+struct Act16<bf16> {
+  static constexpr bool is_fp16 = false;   // tensor maps of this type: bf16
+  static __device__ __forceinline__ uint32_t pack2(float lo, float hi) { return pack_bf16x2(lo, hi); }
+  static __device__ __forceinline__ float2 unpack2(uint32_t u) { return unpack_bf16x2(u); }
+  static __device__ __forceinline__ float to_f(bf16 x) { return __bfloat162float(x); }
+  static __device__ __forceinline__ bf16 from_f(float x) { return __float2bfloat16_rn(x); }
+  static __device__ __forceinline__ float round(float x) { return bf16_round(x); }
+};
+template <>
+struct Act16<f16> {
+  static constexpr bool is_fp16 = true;    // tensor maps of this type: FLOAT16
+  static __device__ __forceinline__ uint32_t pack2(float lo, float hi) {   // cvt.rn.f16x2.f32
+    __half2 v = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<uint32_t*>(&v);
+  }
+  static __device__ __forceinline__ float2 unpack2(uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); }
+  static __device__ __forceinline__ float to_f(f16 x) { return __half2float(x); }
+  static __device__ __forceinline__ f16 from_f(float x) { return __float2half_rn(x); }
+  static __device__ __forceinline__ float round(float x) { return __half2float(__float2half_rn(x)); }
+};
+
+// Calls fn<bf16>(args...) or fn<f16>(args...) for an OASR_DTYPE_BF16 / OASR_DTYPE_F16 code.
+inline int bad_dtype16(int dtype) {
+  set_last_error("16-bit activation dtype must be OASR_DTYPE_BF16 or OASR_DTYPE_F16, got %d", dtype);
+  return OASR_ERR_INVALID;
+}
+#define OASR_BY_DTYPE16(dtype, fn, ...)                                   \
+  ((dtype) == OASR_DTYPE_BF16  ? fn<oasr::bf16>(__VA_ARGS__)              \
+   : (dtype) == OASR_DTYPE_F16 ? fn<oasr::f16>(__VA_ARGS__)               \
+                               : oasr::bad_dtype16(dtype))
 
 template <typename T>
 __device__ __forceinline__ T warp_sum(T v) {

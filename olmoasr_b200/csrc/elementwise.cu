@@ -22,15 +22,16 @@ __global__ void cast_f32_bf16_kernel(const float* __restrict__ src, bf16* __rest
   }
 }
 
-// Conv1d weight (C_out, C_in, 3) f32 -> (C_out, 3, C_in) bf16 so that im2col rows are plain slabs.
-__global__ void cast_conv_weight_kernel(const float* __restrict__ src, bf16* __restrict__ dst, int c_out, int c_in) {
+// Conv1d weight (C_out, C_in, 3) f32 -> (C_out, 3, C_in) T so that im2col rows are plain slabs.
+template <typename T>
+__global__ void cast_conv_weight_kernel(const float* __restrict__ src, T* __restrict__ dst, int c_out, int c_in) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;  // index into dst
   const int64_t n = static_cast<int64_t>(c_out) * 3 * c_in;
   if (i >= n) return;
   const int c = i % c_in;
   const int k = (i / c_in) % 3;
   const int64_t o = i / (3 * c_in);
-  dst[i] = __float2bfloat16_rn(src[(o * c_in + c) * 3 + k]);
+  dst[i] = Act16<T>::from_f(src[(o * c_in + c) * 3 + k]);
 }
 // and its inverse for the weight gradient: (C_out, 3, C_in) f32 -> (C_out, C_in, 3) f32
 __global__ void unpermute_conv_wgrad_kernel(const float* __restrict__ src, float* __restrict__ dst, int c_out, int c_in,
@@ -93,9 +94,10 @@ mask_to_kvlen_kernel(const float* __restrict__ mask, int32_t* __restrict__ kv_le
 }
 
 // ------------------------------------------------------------------ embedding
-// x = (token_embedding(ids) + positional_embedding[offset : offset+S]).to(bf16)   (model.py:728-732)
+// x = (token_embedding(ids) + positional_embedding[offset : offset+S]).to(T)   (model.py:728-732)
+template <typename T>
 __global__ void embed_fwd_kernel(const int64_t* __restrict__ ids, const float* __restrict__ emb,
-                                 const float* __restrict__ pos, bf16* __restrict__ out, int64_t rows, int S,
+                                 const float* __restrict__ pos, T* __restrict__ out, int64_t rows, int S,
                                  int d, int pos_offset, int64_t n_rows_emb) {
   const int64_t row = blockIdx.x;
   if (row >= rows) return;
@@ -108,8 +110,8 @@ __global__ void embed_fwd_kernel(const int64_t* __restrict__ ids, const float* _
   for (int v = threadIdx.x; v < (d >> 2); v += blockDim.x) {
     const float4 a = __ldg(e + v), b = __ldg(p + v);
     uint2 u;
-    u.x = pack_bf16x2(a.x + b.x, a.y + b.y);
-    u.y = pack_bf16x2(a.z + b.z, a.w + b.w);
+    u.x = Act16<T>::pack2(a.x + b.x, a.y + b.y);
+    u.y = Act16<T>::pack2(a.z + b.z, a.w + b.w);
     o[v] = u;
   }
 }
@@ -118,8 +120,9 @@ __global__ void embed_fwd_kernel(const int64_t* __restrict__ ids, const float* _
 // with b == 0 writes dP[s] (sum over the batch), the block of the FIRST row carrying an id writes dE[id] (sum over
 // every row with that id, gathered 128 rows at a time).
 constexpr int EMB_COLS = 10;   // columns per thread: 128 threads cover d <= 1280 (every OLMoASR width)
+template <typename T>
 __global__ void __launch_bounds__(128)
-embed_bwd_kernel(const int64_t* __restrict__ ids, const bf16* __restrict__ dx,
+embed_bwd_kernel(const int64_t* __restrict__ ids, const T* __restrict__ dx,
                  float* __restrict__ demb, float* __restrict__ dpos, int64_t rows, int S, int d,
                  int64_t padding_idx, int64_t n_rows_emb) {
   __shared__ int64_t s_rows[128];
@@ -131,7 +134,7 @@ embed_bwd_kernel(const int64_t* __restrict__ ids, const bf16* __restrict__ dx,
     const int64_t batch = rows / S;
     for (int c = t; c < d; c += blockDim.x) {
       float v = 0.f;
-      for (int64_t b = 0; b < batch; ++b) v += __bfloat162float(dx[(b * S + row) * d + c]);
+      for (int64_t b = 0; b < batch; ++b) v += Act16<T>::to_f(dx[(b * S + row) * d + c]);
       dpos[row * d + c] += v;
     }
   }
@@ -152,10 +155,10 @@ embed_bwd_kernel(const int64_t* __restrict__ ids, const bf16* __restrict__ dx,
     if (hit) s_rows[before + __popc(bal & ((1u << lane) - 1u))] = base + t;
     __syncthreads();
     for (int k = 0; k < total; ++k) {   // matches in row order
-      const bf16* g = dx + s_rows[k] * d;
+      const T* g = dx + s_rows[k] * d;
 #pragma unroll
       for (int j = 0; j < EMB_COLS; ++j)
-        if (t + j * 128 < d) acc[j] += __bfloat162float(g[t + j * 128]);
+        if (t + j * 128 < d) acc[j] += Act16<T>::to_f(g[t + j * 128]);
     }
     __syncthreads();
   }
@@ -165,9 +168,10 @@ embed_bwd_kernel(const int64_t* __restrict__ ids, const bf16* __restrict__ dx,
 }
 
 // ------------------------------------------------------------------ conv stem data movement
-// conv1 im2col: mel (B, C, T) f32 -> A (B*T, Kpad) bf16 with A[b,t][k*C + c] = mel[b][c][t+k-1]  (k3, p1)
+// conv1 im2col: mel (B, C, T) f32 -> A (B*T, Kpad) E (bf16 / fp16) with A[b,t][k*C + c] = mel[b][c][t+k-1]  (k3, p1)
 // Columns >= 3*C (Kpad padding for TMA row-stride alignment) are zero.
-__global__ void im2col_conv1_kernel(const float* __restrict__ mel, bf16* __restrict__ A, int C, int T, int kpad) {
+template <typename E>
+__global__ void im2col_conv1_kernel(const float* __restrict__ mel, E* __restrict__ A, int C, int T, int kpad) {
   extern __shared__ float tile[];  // [C][34]
   const int b = blockIdx.y;
   const int t0 = blockIdx.x * 32;
@@ -185,11 +189,11 @@ __global__ void im2col_conv1_kernel(const float* __restrict__ mel, bf16* __restr
       const int k = col / C, c = col % C;
       v = tile[c * 34 + tt + k];
     }
-    A[(static_cast<int64_t>(b) * T + t0 + tt) * kpad + col] = __float2bfloat16_rn(v);
+    A[(static_cast<int64_t>(b) * T + t0 + tt) * kpad + col] = Act16<E>::from_f(v);
   }
 }
 // conv2 im2col (k3, s2, p1) on time-major activations: A[b,t] = [h[b,2t-1], h[b,2t], h[b,2t+1]]  (each d wide)
-__global__ void im2col_conv2_kernel(const bf16* __restrict__ h, bf16* __restrict__ A, int T_in, int T_out, int d) {
+__global__ void im2col_conv2_kernel(const uint16_t* __restrict__ h, uint16_t* __restrict__ A, int T_in, int T_out, int d) {
   const int64_t row = blockIdx.x;  // b * T_out + t
   const int b = row / T_out, t = row % T_out;
   const int nvec = d >> 3;
@@ -202,29 +206,31 @@ __global__ void im2col_conv2_kernel(const bf16* __restrict__ h, bf16* __restrict
   }
 }
 // col2im of the conv2 input gradient fused with the GELU backward of conv1:
-//   dpre1[b,r] = bf16( bf16(sum_{(t,k): 2t+k-1=r} dA[b,t][k]) * gelu'(pre1[b,r]) )
-__global__ void col2im_conv2_gelu_bwd_kernel(const bf16* __restrict__ dA, const bf16* __restrict__ pre1,
-                                             bf16* __restrict__ dpre1, int T_in, int T_out, int d) {
+//   dpre1[b,r] = T( T(sum_{(t,k): 2t+k-1=r} dA[b,t][k]) * gelu'(pre1[b,r]) )
+template <typename T>
+__global__ void col2im_conv2_gelu_bwd_kernel(const T* __restrict__ dA, const T* __restrict__ pre1,
+                                             T* __restrict__ dpre1, int T_in, int T_out, int d) {
   const int64_t row = blockIdx.x;  // b * T_in + r
   const int b = row / T_in, r = row % T_in;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
     float g = 0.f;
     if ((r & 1) == 0) {
       const int t = r >> 1;  // k = 1
-      if (t < T_out) g = __bfloat162float(dA[((static_cast<int64_t>(b) * T_out + t) * 3 + 1) * d + c]);
+      if (t < T_out) g = Act16<T>::to_f(dA[((static_cast<int64_t>(b) * T_out + t) * 3 + 1) * d + c]);
     } else {
       const int ta = (r + 1) >> 1;  // k = 0
       const int tb = (r - 1) >> 1;  // k = 2
-      if (ta < T_out) g += __bfloat162float(dA[((static_cast<int64_t>(b) * T_out + ta) * 3 + 0) * d + c]);
-      if (tb >= 0 && tb < T_out) g += __bfloat162float(dA[((static_cast<int64_t>(b) * T_out + tb) * 3 + 2) * d + c]);
+      if (ta < T_out) g += Act16<T>::to_f(dA[((static_cast<int64_t>(b) * T_out + ta) * 3 + 0) * d + c]);
+      if (tb >= 0 && tb < T_out) g += Act16<T>::to_f(dA[((static_cast<int64_t>(b) * T_out + tb) * 3 + 2) * d + c]);
     }
-    const float p = __bfloat162float(pre1[row * d + c]);
-    dpre1[row * d + c] = __float2bfloat16_rn(bf16_round(g) * gelu_erf_grad(p));
+    const float p = Act16<T>::to_f(pre1[row * d + c]);
+    dpre1[row * d + c] = Act16<T>::from_f(Act16<T>::round(g) * gelu_erf_grad(p));
   }
 }
 
-// x = (x + positional_embedding).to(bf16), positional rows repeat every T rows  (model.py:602)
-__global__ void add_pos_kernel(const bf16* __restrict__ x, const float* __restrict__ pos, bf16* __restrict__ out,
+// x = (x + positional_embedding).to(E), positional rows repeat every T rows  (model.py:602)
+template <typename E>
+__global__ void add_pos_kernel(const E* __restrict__ x, const float* __restrict__ pos, E* __restrict__ out,
                                int64_t rows, int T, int d) {
   const int64_t nvec = rows * (d >> 3);
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec;
@@ -234,16 +240,18 @@ __global__ void add_pos_kernel(const bf16* __restrict__ x, const float* __restri
     const uint4 u = reinterpret_cast<const uint4*>(x)[i];
     const float4* p = reinterpret_cast<const float4*>(pos + (row % T) * d) + 2 * v;
     const float4 p0 = __ldg(p), p1 = __ldg(p + 1);
-    float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), e = unpack_bf16x2(u.w);
+    using A = Act16<E>;
+    float2 a = A::unpack2(u.x), b = A::unpack2(u.y), c = A::unpack2(u.z), e = A::unpack2(u.w);
     uint4 o;
-    o.x = pack_bf16x2(a.x + p0.x, a.y + p0.y); o.y = pack_bf16x2(b.x + p0.z, b.y + p0.w);
-    o.z = pack_bf16x2(c.x + p1.x, c.y + p1.y); o.w = pack_bf16x2(e.x + p1.z, e.y + p1.w);
+    o.x = A::pack2(a.x + p0.x, a.y + p0.y); o.y = A::pack2(b.x + p0.z, b.y + p0.w);
+    o.z = A::pack2(c.x + p1.x, c.y + p1.y); o.w = A::pack2(e.x + p1.z, e.y + p1.w);
     reinterpret_cast<uint4*>(out)[i] = o;
   }
 }
 
 // dy * gelu'(pre) elementwise (conv2 backward, where the upstream gradient is not a GEMM output)
-__global__ void gelu_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ pre, bf16* __restrict__ out, int64_t n) {
+template <typename T>
+__global__ void gelu_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ pre, T* __restrict__ out, int64_t n) {
   for (int64_t i = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) * 8; i < n;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x * 8) {
     const uint4 a = *reinterpret_cast<const uint4*>(dy + i), b = *reinterpret_cast<const uint4*>(pre + i);
@@ -251,8 +259,8 @@ __global__ void gelu_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restr
     uint32_t ov[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const float2 g = unpack_bf16x2(av[j]), p = unpack_bf16x2(bv[j]);
-      ov[j] = pack_bf16x2(g.x * gelu_erf_grad(p.x), g.y * gelu_erf_grad(p.y));
+      const float2 g = Act16<T>::unpack2(av[j]), p = Act16<T>::unpack2(bv[j]);
+      ov[j] = Act16<T>::pack2(g.x * gelu_erf_grad(p.x), g.y * gelu_erf_grad(p.y));
     }
     *reinterpret_cast<uint4*>(out + i) = make_uint4(ov[0], ov[1], ov[2], ov[3]);
   }
@@ -261,8 +269,9 @@ __global__ void gelu_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restr
 // ------------------------------------------------------------------ bias gradient: db[n] += sum_m dy[m,n]
 // Block = 32 x 8 threads; tile = 256 columns (8 per thread, one 16-byte load) x a slab of rows.  Each slab of rows
 // writes its column sums to part[slab][n]; add_partials adds the slabs in order.
+template <typename T>
 __global__ void __launch_bounds__(256)
-colsum_kernel(const bf16* __restrict__ dy, float* __restrict__ part, int64_t M, int N, int64_t ld, int rows_per_block) {
+colsum_kernel(const T* __restrict__ dy, float* __restrict__ part, int64_t M, int N, int64_t ld, int rows_per_block) {
   __shared__ float red[8][256 + 8];
   const int col = blockIdx.x * 256 + threadIdx.x * 8;
   const int64_t r0 = static_cast<int64_t>(blockIdx.y) * rows_per_block;
@@ -278,7 +287,7 @@ colsum_kernel(const bf16* __restrict__ dy, float* __restrict__ part, int64_t M, 
       const uint32_t av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const float2 p = unpack_bf16x2(av[j]), q = unpack_bf16x2(bv[j]);
+        const float2 p = Act16<T>::unpack2(av[j]), q = Act16<T>::unpack2(bv[j]);
         s[2 * j] += p.x + q.x; s[2 * j + 1] += p.y + q.y;
       }
     }
@@ -286,13 +295,13 @@ colsum_kernel(const bf16* __restrict__ dy, float* __restrict__ part, int64_t M, 
       const uint4 a = *reinterpret_cast<const uint4*>(dy + r * ld + col);
       const uint32_t av[4] = {a.x, a.y, a.z, a.w};
 #pragma unroll
-      for (int j = 0; j < 4; ++j) { const float2 p = unpack_bf16x2(av[j]); s[2 * j] += p.x; s[2 * j + 1] += p.y; }
+      for (int j = 0; j < 4; ++j) { const float2 p = Act16<T>::unpack2(av[j]); s[2 * j] += p.x; s[2 * j + 1] += p.y; }
     }
   } else {
     for (int64_t r = r0 + threadIdx.y; r < r1; r += 8)
 #pragma unroll
       for (int j = 0; j < 8; ++j)
-        if (col + j < N) s[j] += __bfloat162float(dy[r * ld + col + j]);
+        if (col + j < N) s[j] += Act16<T>::to_f(dy[r * ld + col + j]);
   }
 #pragma unroll
   for (int j = 0; j < 8; ++j) red[threadIdx.y][threadIdx.x * 8 + j] = s[j];
@@ -324,9 +333,10 @@ extern "C" int oasr_cast_f32_to_bf16(const float* src, void* dst, int64_t n, voi
   return OASR_OK;
 }
 
-extern "C" int oasr_cast_conv_weight(const float* src, void* dst, int64_t c_out, int64_t c_in, void* stream) {
+template <typename T>
+static int cast_conv_weight(const float* src, void* dst, int64_t c_out, int64_t c_in, void* stream) {
   const int64_t n = c_out * 3 * c_in;
-  cast_conv_weight_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(src, (bf16*)dst, (int)c_out, (int)c_in);
+  cast_conv_weight_kernel<T><<<(unsigned)ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(src, (T*)dst, (int)c_out, (int)c_in);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
@@ -345,62 +355,69 @@ extern "C" int oasr_mask_to_kvlen(const float* mask, int32_t* kv_len, int32_t* e
   return OASR_OK;
 }
 
-extern "C" int oasr_embed_fwd(const int64_t* ids, const float* emb, const float* pos, void* out, int64_t batch,
-                              int64_t S, int64_t d, int64_t pos_offset, int64_t n_rows_emb, void* stream) {
+template <typename T>
+static int embed_fwd(const int64_t* ids, const float* emb, const float* pos, void* out, int64_t batch, int64_t S, int64_t d,
+              int64_t pos_offset, int64_t n_rows_emb, void* stream) {
   OASR_REQUIRE(batch > 0 && S > 0 && (d & 3) == 0, "embed_fwd: bad shape");
-  embed_fwd_kernel<<<(unsigned)(batch * S), 128, 0, (cudaStream_t)stream>>>(ids, emb, pos, (bf16*)out, batch * S, (int)S, (int)d,
+  embed_fwd_kernel<T><<<(unsigned)(batch * S), 128, 0, (cudaStream_t)stream>>>(ids, emb, pos, (T*)out, batch * S, (int)S, (int)d,
                                                                            (int)pos_offset, n_rows_emb);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
 
-extern "C" int oasr_embed_bwd(const int64_t* ids, const void* dx, float* demb, float* dpos, int64_t batch, int64_t S,
-                              int64_t d, int64_t padding_idx, int64_t n_rows_emb, void* stream) {
+template <typename T>
+static int embed_bwd(const int64_t* ids, const void* dx, float* demb, float* dpos, int64_t batch, int64_t S, int64_t d,
+              int64_t padding_idx, int64_t n_rows_emb, void* stream) {
   OASR_REQUIRE(batch > 0 && S > 0 && d <= 128 * EMB_COLS, "embed_bwd: bad shape");
-  embed_bwd_kernel<<<(unsigned)(batch * S), 128, 0, (cudaStream_t)stream>>>(ids, (const bf16*)dx, demb, dpos, batch * S, (int)S, (int)d,
+  embed_bwd_kernel<T><<<(unsigned)(batch * S), 128, 0, (cudaStream_t)stream>>>(ids, (const T*)dx, demb, dpos, batch * S, (int)S, (int)d,
                                                                            padding_idx, n_rows_emb);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
 
-extern "C" int oasr_im2col_conv1(const float* mel, void* A, int64_t batch, int64_t C, int64_t T, int64_t kpad, void* stream) {
+template <typename E>
+static int im2col_conv1(const float* mel, void* A, int64_t batch, int64_t C, int64_t T, int64_t kpad, void* stream) {
   OASR_REQUIRE(kpad >= 3 * C && (kpad & 7) == 0, "im2col_conv1: kpad must be >= 3C and a multiple of 8");
   dim3 grid((unsigned)ceil_div(T, 32), (unsigned)batch);
-  im2col_conv1_kernel<<<grid, 256, C * 34 * sizeof(float), (cudaStream_t)stream>>>(mel, (bf16*)A, (int)C, (int)T, (int)kpad);
+  im2col_conv1_kernel<E><<<grid, 256, C * 34 * sizeof(float), (cudaStream_t)stream>>>(mel, (E*)A, (int)C, (int)T, (int)kpad);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
 
 extern "C" int oasr_im2col_conv2(const void* h, void* A, int64_t batch, int64_t T_in, int64_t T_out, int64_t d, void* stream) {
   OASR_REQUIRE((d & 7) == 0, "im2col_conv2: d must be a multiple of 8");
-  im2col_conv2_kernel<<<(unsigned)(batch * T_out), 128, 0, (cudaStream_t)stream>>>((const bf16*)h, (bf16*)A, (int)T_in, (int)T_out, (int)d);
+  im2col_conv2_kernel<<<(unsigned)(batch * T_out), 128, 0, (cudaStream_t)stream>>>((const uint16_t*)h, (uint16_t*)A, (int)T_in, (int)T_out, (int)d);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
 
-extern "C" int oasr_col2im_conv2_gelu_bwd(const void* dA, const void* pre1, void* dpre1, int64_t batch, int64_t T_in,
-                                          int64_t T_out, int64_t d, void* stream) {
-  col2im_conv2_gelu_bwd_kernel<<<(unsigned)(batch * T_in), 128, 0, (cudaStream_t)stream>>>((const bf16*)dA, (const bf16*)pre1,
-                                                                                          (bf16*)dpre1, (int)T_in, (int)T_out, (int)d);
+template <typename T>
+static int col2im_conv2_gelu_bwd(const void* dA, const void* pre1, void* dpre1, int64_t batch, int64_t T_in, int64_t T_out, int64_t d,
+                          void* stream) {
+  col2im_conv2_gelu_bwd_kernel<T><<<(unsigned)(batch * T_in), 128, 0, (cudaStream_t)stream>>>((const T*)dA, (const T*)pre1,
+                                                                                             (T*)dpre1, (int)T_in, (int)T_out, (int)d);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
 
-extern "C" int oasr_add_pos(const void* x, const float* pos, void* out, int64_t rows, int64_t T, int64_t d, void* stream) {
+template <typename E>
+static int add_pos(const void* x, const float* pos, void* out, int64_t rows, int64_t T, int64_t d, void* stream) {
   OASR_REQUIRE((d & 7) == 0, "add_pos: d must be a multiple of 8");
-  add_pos_kernel<<<grid_1d(rows * (d >> 3), 256), 256, 0, (cudaStream_t)stream>>>((const bf16*)x, pos, (bf16*)out, rows, (int)T, (int)d);
+  add_pos_kernel<E><<<grid_1d(rows * (d >> 3), 256), 256, 0, (cudaStream_t)stream>>>((const E*)x, pos, (E*)out, rows, (int)T, (int)d);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
 
-extern "C" int oasr_gelu_bwd(const void* dy, const void* pre, void* out, int64_t n, void* stream) {
+template <typename T>
+static int gelu_bwd(const void* dy, const void* pre, void* out, int64_t n, void* stream) {
   OASR_REQUIRE((n & 7) == 0, "gelu_bwd: n must be a multiple of 8");
-  gelu_bwd_kernel<<<grid_1d(n >> 3, 256), 256, 0, (cudaStream_t)stream>>>((const bf16*)dy, (const bf16*)pre, (bf16*)out, n);
+  gelu_bwd_kernel<T><<<grid_1d(n >> 3, 256), 256, 0, (cudaStream_t)stream>>>((const T*)dy, (const T*)pre, (T*)out, n);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
 
-extern "C" int oasr_colsum_bf16(const void* dy, float* db, int64_t M, int64_t N, int64_t ld, void* stream) {
+template <typename T>
+static int colsum(const void* dy, float* db, int64_t M, int64_t N, int64_t ld, void* stream) {
   OASR_REQUIRE(M > 0 && N > 0 && (ld & 1) == 0, "colsum: bad shape");
   const int col_tiles = (int)ceil_div(N, 256);
   int row_blocks = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(M, 64), (num_sms() * 6) / col_tiles + 1));
@@ -409,9 +426,67 @@ extern "C" int oasr_colsum_bf16(const void* dy, float* db, int64_t M, int64_t N,
   cudaStream_t st = (cudaStream_t)stream;
   float* part = static_cast<float*>(scratch_alloc(sizeof(float) * row_blocks * N, st));
   if (!part) return OASR_ERR_CUDA;
-  colsum_kernel<<<dim3(col_tiles, row_blocks), dim3(32, 8), 0, st>>>((const bf16*)dy, part, M, (int)N, ld, rows_per_block);
+  colsum_kernel<T><<<dim3(col_tiles, row_blocks), dim3(32, 8), 0, st>>>((const T*)dy, part, M, (int)N, ld, rows_per_block);
   OASR_LAUNCH_CHECK();
   const int rc = add_partials(part, row_blocks, N, db, st);
   scratch_free(part, st);
   return rc;
+}
+
+extern "C" int oasr_cast_conv_weight(const float* src, void* dst, int64_t c_out, int64_t c_in, void* stream) {
+  return cast_conv_weight<bf16>(src, dst, c_out, c_in, stream);
+}
+extern "C" int oasr_embed_fwd(const int64_t* ids, const float* emb, const float* pos, void* out, int64_t batch,
+                              int64_t S, int64_t d, int64_t pos_offset, int64_t n_rows_emb, void* stream) {
+  return embed_fwd<bf16>(ids, emb, pos, out, batch, S, d, pos_offset, n_rows_emb, stream);
+}
+extern "C" int oasr_embed_bwd(const int64_t* ids, const void* dx, float* demb, float* dpos, int64_t batch, int64_t S,
+                              int64_t d, int64_t padding_idx, int64_t n_rows_emb, void* stream) {
+  return embed_bwd<bf16>(ids, dx, demb, dpos, batch, S, d, padding_idx, n_rows_emb, stream);
+}
+extern "C" int oasr_im2col_conv1(const float* mel, void* A, int64_t batch, int64_t C, int64_t T, int64_t kpad, void* stream) {
+  return im2col_conv1<bf16>(mel, A, batch, C, T, kpad, stream);
+}
+extern "C" int oasr_col2im_conv2_gelu_bwd(const void* dA, const void* pre1, void* dpre1, int64_t batch, int64_t T_in,
+                                          int64_t T_out, int64_t d, void* stream) {
+  return col2im_conv2_gelu_bwd<bf16>(dA, pre1, dpre1, batch, T_in, T_out, d, stream);
+}
+extern "C" int oasr_add_pos(const void* x, const float* pos, void* out, int64_t rows, int64_t T, int64_t d, void* stream) {
+  return add_pos<bf16>(x, pos, out, rows, T, d, stream);
+}
+extern "C" int oasr_gelu_bwd(const void* dy, const void* pre, void* out, int64_t n, void* stream) {
+  return gelu_bwd<bf16>(dy, pre, out, n, stream);
+}
+extern "C" int oasr_colsum_bf16(const void* dy, float* db, int64_t M, int64_t N, int64_t ld, void* stream) {
+  return colsum<bf16>(dy, db, M, N, ld, stream);
+}
+
+extern "C" int oasr_cast_conv_weight16(const float* src, void* dst, int64_t c_out, int64_t c_in, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, cast_conv_weight, src, dst, c_out, c_in, stream);
+}
+extern "C" int oasr_embed_fwd16(const int64_t* ids, const float* emb, const float* pos, void* out, int64_t batch,
+                                int64_t S, int64_t d, int64_t pos_offset, int64_t n_rows_emb, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, embed_fwd, ids, emb, pos, out, batch, S, d, pos_offset, n_rows_emb, stream);
+}
+extern "C" int oasr_embed_bwd16(const int64_t* ids, const void* dx, float* demb, float* dpos, int64_t batch, int64_t S,
+                                int64_t d, int64_t padding_idx, int64_t n_rows_emb, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, embed_bwd, ids, dx, demb, dpos, batch, S, d, padding_idx, n_rows_emb, stream);
+}
+extern "C" int oasr_im2col_conv1_16(const float* mel, void* A, int64_t batch, int64_t C, int64_t T, int64_t kpad, int dtype,
+                                    void* stream) {
+  return OASR_BY_DTYPE16(dtype, im2col_conv1, mel, A, batch, C, T, kpad, stream);
+}
+extern "C" int oasr_col2im_conv2_gelu_bwd16(const void* dA, const void* pre1, void* dpre1, int64_t batch, int64_t T_in,
+                                            int64_t T_out, int64_t d, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, col2im_conv2_gelu_bwd, dA, pre1, dpre1, batch, T_in, T_out, d, stream);
+}
+extern "C" int oasr_add_pos16(const void* x, const float* pos, void* out, int64_t rows, int64_t T, int64_t d, int dtype,
+                              void* stream) {
+  return OASR_BY_DTYPE16(dtype, add_pos, x, pos, out, rows, T, d, stream);
+}
+extern "C" int oasr_gelu_bwd16(const void* dy, const void* pre, void* out, int64_t n, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, gelu_bwd, dy, pre, out, n, stream);
+}
+extern "C" int oasr_colsum16(const void* dy, float* db, int64_t M, int64_t N, int64_t ld, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, colsum, dy, db, M, N, ld, stream);
 }

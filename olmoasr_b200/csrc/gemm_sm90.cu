@@ -86,14 +86,15 @@ __device__ __forceinline__ void quad_transpose(const uint32_t (&w)[4], uint32_t 
   }
 }
 
-// bf16 epilogues: 8 consecutive columns col .. col+7 of one row, v[k] = bf16(acc + bias) of columns col+2k, col+2k+1
-template <int EPI>
-__device__ __forceinline__ void store_bf16x8(const GemmParams& p, int row, int col, const uint32_t (&v)[4], bool vec_c,
+// 16-bit epilogues: 8 consecutive columns col .. col+7 of one row, v[k] = T(acc + bias) of columns col+2k, col+2k+1
+template <typename T, int EPI>
+__device__ __forceinline__ void store_16x8(const GemmParams& p, int row, int col, const uint32_t (&v)[4], bool vec_c,
                                              bool vec_aux) {
   const bool full = col + 8 <= p.N;
   uint32_t a[4];
   if constexpr (reads_aux(EPI)) {   // plain loads: aux may be the output itself (in-place residual)
-    const bf16* ap = reinterpret_cast<const bf16*>(p.aux) + static_cast<int64_t>(row) * p.ldaux + col;
+    using A = Act16<T>;
+    const T* ap = reinterpret_cast<const T*>(p.aux) + static_cast<int64_t>(row) * p.ldaux + col;
     if (full && vec_aux) {
       const uint4 t = *reinterpret_cast<const uint4*>(ap);
       a[0] = t.x; a[1] = t.y; a[2] = t.z; a[3] = t.w;
@@ -107,26 +108,27 @@ __device__ __forceinline__ void store_bf16x8(const GemmParams& p, int row, int c
       }
     }
   }
+  using A = Act16<T>;
   uint32_t o[4], g[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     o[k] = v[k];
     if constexpr (EPI == OASR_EPI_BF16_GELU) {   // h = bf16(acc + b), g = bf16(gelu(h))
-      const float2 x = gelu_erf2(unpack_bf16x2(v[k]));
-      g[k] = pack_bf16x2(x.x, x.y);
+      const float2 x = gelu_erf2(A::unpack2(v[k]));
+      g[k] = A::pack2(x.x, x.y);
     } else if constexpr (EPI == OASR_EPI_BF16_RESIDUAL) {   // C = bf16(aux + bf16(acc + b))
-      const float2 x = fadd2(unpack_bf16x2(a[k]), unpack_bf16x2(v[k]));
-      o[k] = pack_bf16x2(x.x, x.y);
+      const float2 x = fadd2(A::unpack2(a[k]), A::unpack2(v[k]));
+      o[k] = A::pack2(x.x, x.y);
     } else if constexpr (EPI == OASR_EPI_BF16_GELU_BWD) {   // C = bf16(bf16(acc) * gelu'(aux))
-      const float2 x = fmul2(unpack_bf16x2(v[k]), gelu_erf_grad2(unpack_bf16x2(a[k])));
-      o[k] = pack_bf16x2(x.x, x.y);
+      const float2 x = fmul2(A::unpack2(v[k]), gelu_erf_grad2(A::unpack2(a[k])));
+      o[k] = A::pack2(x.x, x.y);
     }
   }
   const int64_t off = static_cast<int64_t>(row) * p.ldc + col;
 #pragma unroll
   for (int out = 0; out < (EPI == OASR_EPI_BF16_GELU ? 2 : 1); ++out) {
     const uint32_t* src = out ? g : o;
-    bf16* dst = reinterpret_cast<bf16*>(out ? p.C2 : p.C) + off;
+    T* dst = reinterpret_cast<T*>(out ? p.C2 : p.C) + off;
     if (full && vec_c) {
       *reinterpret_cast<uint4*>(dst) = make_uint4(src[0], src[1], src[2], src[3]);
     } else {
@@ -140,7 +142,7 @@ __device__ __forceinline__ void store_bf16x8(const GemmParams& p, int row, int c
   }
 }
 
-template <int BN, int A_MN, int B_MN, int EPI>
+template <typename T, int BN, int A_MN, int B_MN, int EPI>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   using C = Cfg<BN>;
@@ -238,9 +240,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       for (int k = 0; k < BK / 16; ++k) {
         const uint32_t accumulate = (kb > kb0 || k > 0) ? 1u : 0u;
         const uint64_t da = ptx::desc_add(ad, k * a_kstep), db = ptx::desc_add(bd, k * b_kstep);
-        if constexpr (BN == 256) ptx::wgmma_m64n256k16_ss<A_MN, B_MN>(acc, da, db, accumulate);
-        else if constexpr (BN == 128) ptx::wgmma_m64n128k16_ss<A_MN, B_MN>(acc, da, db, accumulate);
-        else ptx::wgmma_m64n64k16_ss<A_MN, B_MN>(acc, da, db, accumulate);
+        if constexpr (BN == 256) ptx::wgmma_m64n256k16_ss<A_MN, B_MN, T>(acc, da, db, accumulate);
+        else if constexpr (BN == 128) ptx::wgmma_m64n128k16_ss<A_MN, B_MN, T>(acc, da, db, accumulate);
+        else ptx::wgmma_m64n64k16_ss<A_MN, B_MN, T>(acc, da, db, accumulate);
       }
       ptx::wgmma_commit();
       ptx::wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot may be refilled
@@ -285,7 +287,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     } else {
-      // bf16(acc + bf16(bias)) per column pair, then a quad transpose so that each lane stores 8 consecutive columns
+      // T(acc + T(bias)) per column pair, then a quad transpose so that each lane stores 8 consecutive columns
 #pragma unroll
       for (int j = 0; j < BN / 32; ++j) {
         if (ncol0 + 32 * j >= p.N) break;   // warp-uniform: the quad shuffles below need every lane
@@ -295,20 +297,20 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const int i = 4 * j + k;
           const int col = ncol0 + 8 * i + 2 * (lane & 3);
           float b0 = 0.f, b1 = 0.f;
-          if (p.bias != nullptr) {   // rounded to bf16 like bias.to(x.dtype)
-            if (col < p.N) b0 = bf16_round(__ldg(p.bias + col));
-            if (col + 1 < p.N) b1 = bf16_round(__ldg(p.bias + col + 1));
+          if (p.bias != nullptr) {   // rounded to T like bias.to(x.dtype)
+            if (col < p.N) b0 = Act16<T>::round(__ldg(p.bias + col));
+            if (col + 1 < p.N) b1 = Act16<T>::round(__ldg(p.bias + col + 1));
           }
 #pragma unroll
           for (int h = 0; h < 2; ++h)
-            w[h][k] = pack_bf16x2(__fadd_rn(acc[4 * i + 2 * h], b0), __fadd_rn(acc[4 * i + 2 * h + 1], b1));
+            w[h][k] = Act16<T>::pack2(__fadd_rn(acc[4 * i + 2 * h], b0), __fadd_rn(acc[4 * i + 2 * h + 1], b1));
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           uint32_t v[4];
           quad_transpose(w[h], v, lane);
           const int row = row0 + 8 * h;
-          if (row < p.M) store_bf16x8<EPI>(p, row, ncol0 + 32 * j + 8 * (lane & 3), v, vec_c, vec_aux);
+          if (row < p.M) store_16x8<T, EPI>(p, row, ncol0 + 32 * j + 8 * (lane & 3), v, vec_c, vec_aux);
         }
       }
     }
@@ -325,10 +327,10 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, int splits, i
   }
 }
 
-template <int BN, int A_MN, int B_MN, int EPI>
+template <typename T, int BN, int A_MN, int B_MN, int EPI>
 int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
   using C = Cfg<BN>;
-  auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, EPI>;
+  auto kern = gemm_wgmma_kernel<T, BN, A_MN, B_MN, EPI>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     OASR_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
@@ -346,42 +348,37 @@ int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, 
 //   A K-major,  B MN-major (dgrad, logits dx):                     BF16, BF16_RESIDUAL, BF16_GELU_BWD, F32
 //   A MN-major, B MN-major (wgrad):                                F32, F32_ATOMIC_ADD
 // (split-K launches store fp32 partials: they run the F32 kernel).  Any other pair is rejected.
-template <int BN>
+template <typename T, int BN>
 int dispatch(int a_mn, int b_mn, int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
   if (!a_mn && !b_mn) {
     switch (epi) {
-      case OASR_EPI_BF16: return launch<BN, 0, 0, OASR_EPI_BF16>(tmA, tmB, p, st);
-      case OASR_EPI_BF16_GELU: return launch<BN, 0, 0, OASR_EPI_BF16_GELU>(tmA, tmB, p, st);
-      case OASR_EPI_BF16_RESIDUAL: return launch<BN, 0, 0, OASR_EPI_BF16_RESIDUAL>(tmA, tmB, p, st);
-      case OASR_EPI_BF16_GELU_BWD: return launch<BN, 0, 0, OASR_EPI_BF16_GELU_BWD>(tmA, tmB, p, st);
-      case OASR_EPI_F32: return launch<BN, 0, 0, OASR_EPI_F32>(tmA, tmB, p, st);
+      case OASR_EPI_BF16: return launch<T, BN, 0, 0, OASR_EPI_BF16>(tmA, tmB, p, st);
+      case OASR_EPI_BF16_GELU: return launch<T, BN, 0, 0, OASR_EPI_BF16_GELU>(tmA, tmB, p, st);
+      case OASR_EPI_BF16_RESIDUAL: return launch<T, BN, 0, 0, OASR_EPI_BF16_RESIDUAL>(tmA, tmB, p, st);
+      case OASR_EPI_BF16_GELU_BWD: return launch<T, BN, 0, 0, OASR_EPI_BF16_GELU_BWD>(tmA, tmB, p, st);
+      case OASR_EPI_F32: return launch<T, BN, 0, 0, OASR_EPI_F32>(tmA, tmB, p, st);
     }
   } else if (!a_mn && b_mn) {
     switch (epi) {
-      case OASR_EPI_BF16: return launch<BN, 0, 1, OASR_EPI_BF16>(tmA, tmB, p, st);
-      case OASR_EPI_BF16_RESIDUAL: return launch<BN, 0, 1, OASR_EPI_BF16_RESIDUAL>(tmA, tmB, p, st);
-      case OASR_EPI_BF16_GELU_BWD: return launch<BN, 0, 1, OASR_EPI_BF16_GELU_BWD>(tmA, tmB, p, st);
-      case OASR_EPI_F32: return launch<BN, 0, 1, OASR_EPI_F32>(tmA, tmB, p, st);
+      case OASR_EPI_BF16: return launch<T, BN, 0, 1, OASR_EPI_BF16>(tmA, tmB, p, st);
+      case OASR_EPI_BF16_RESIDUAL: return launch<T, BN, 0, 1, OASR_EPI_BF16_RESIDUAL>(tmA, tmB, p, st);
+      case OASR_EPI_BF16_GELU_BWD: return launch<T, BN, 0, 1, OASR_EPI_BF16_GELU_BWD>(tmA, tmB, p, st);
+      case OASR_EPI_F32: return launch<T, BN, 0, 1, OASR_EPI_F32>(tmA, tmB, p, st);
     }
   } else if (a_mn && b_mn) {
     switch (epi) {
-      case OASR_EPI_F32: return launch<BN, 1, 1, OASR_EPI_F32>(tmA, tmB, p, st);
-      case OASR_EPI_F32_ATOMIC_ADD: return launch<BN, 1, 1, OASR_EPI_F32_ATOMIC_ADD>(tmA, tmB, p, st);
+      case OASR_EPI_F32: return launch<T, BN, 1, 1, OASR_EPI_F32>(tmA, tmB, p, st);
+      case OASR_EPI_F32_ATOMIC_ADD: return launch<T, BN, 1, 1, OASR_EPI_F32_ATOMIC_ADD>(tmA, tmB, p, st);
     }
   }
   set_last_error("gemm: no kernel for a_layout=%d b_layout=%d epilogue=%d", a_mn, b_mn, epi);
   return OASR_ERR_UNSUPPORTED;
 }
 
-}  // namespace
-}  // namespace oasr
-
-using namespace oasr;
-
-extern "C" int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb,
-                              int b_layout, void* Cout, int64_t ldc, void* C2, const float* bias,
-                              const void* aux, int64_t ldaux, int64_t M, int64_t N, int64_t K,
-                              int epilogue, int split_k, int block_n, void* stream) {
+template <typename T>
+int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, int b_layout, void* Cout, int64_t ldc,
+         void* C2, const float* bias, const void* aux, int64_t ldaux, int64_t M, int64_t N, int64_t K, int epilogue,
+         int split_k, int block_n, void* stream) {
   OASR_REQUIRE(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%ld N=%ld K=%ld", (long)M, (long)N, (long)K);
   OASR_REQUIRE(A && B && Cout, "gemm: null operand");
   OASR_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0,
@@ -411,16 +408,17 @@ extern "C" int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const vo
   p.split_stride = 0;
 
   CUtensorMap tmA, tmB;
+  constexpr bool f16 = Act16<T>::is_fp16;
   int rc;
   if (a_layout == OASR_K_MAJOR)
-    rc = make_tmap_2d(&tmA, A, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BK, BM, true);
+    rc = make_tmap_2d(&tmA, A, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BK, BM, true, f16);
   else
-    rc = make_tmap_2d(&tmA, A, 2, (uint64_t)M, (uint64_t)K, (uint64_t)lda * 2, 64, BK, true);
+    rc = make_tmap_2d(&tmA, A, 2, (uint64_t)M, (uint64_t)K, (uint64_t)lda * 2, 64, BK, true, f16);
   if (rc) return rc;
   if (b_layout == OASR_K_MAJOR)
-    rc = make_tmap_2d(&tmB, B, 2, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, BK, block_n, true);
+    rc = make_tmap_2d(&tmB, B, 2, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, BK, block_n, true, f16);
   else
-    rc = make_tmap_2d(&tmB, B, 2, (uint64_t)N, (uint64_t)K, (uint64_t)ldb * 2, 64, BK, true);
+    rc = make_tmap_2d(&tmB, B, 2, (uint64_t)N, (uint64_t)K, (uint64_t)ldb * 2, 64, BK, true, f16);
   if (rc) return rc;
 
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -430,9 +428,9 @@ extern "C" int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const vo
     if (!ws) return OASR_ERR_CUDA;
     p.C = ws; p.ldc = N; epilogue = OASR_EPI_F32; p.split_stride = M * N;
   }
-  rc = block_n == 256 ? dispatch<256>(a_layout, b_layout, epilogue, tmA, tmB, p, st)
-     : block_n == 128 ? dispatch<128>(a_layout, b_layout, epilogue, tmA, tmB, p, st)
-                      : dispatch<64>(a_layout, b_layout, epilogue, tmA, tmB, p, st);
+  rc = block_n == 256 ? dispatch<T, 256>(a_layout, b_layout, epilogue, tmA, tmB, p, st)
+     : block_n == 128 ? dispatch<T, 128>(a_layout, b_layout, epilogue, tmA, tmB, p, st)
+                      : dispatch<T, 64>(a_layout, b_layout, epilogue, tmA, tmB, p, st);
   if (ws) {
     if (rc == OASR_OK) {
       int64_t blocks = ceil_div(M * N, 256);
@@ -444,4 +442,24 @@ extern "C" int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const vo
     scratch_free(ws, st);
   }
   return rc;
+}
+
+}  // namespace
+}  // namespace oasr
+
+using namespace oasr;
+
+extern "C" int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb,
+                              int b_layout, void* Cout, int64_t ldc, void* C2, const float* bias,
+                              const void* aux, int64_t ldaux, int64_t M, int64_t N, int64_t K,
+                              int epilogue, int split_k, int block_n, void* stream) {
+  return gemm<bf16>(A, lda, a_layout, B, ldb, b_layout, Cout, ldc, C2, bias, aux, ldaux, M, N, K, epilogue, split_k, block_n,
+                    stream);
+}
+
+extern "C" int oasr_gemm16(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, int b_layout, void* Cout,
+                           int64_t ldc, void* C2, const float* bias, const void* aux, int64_t ldaux, int64_t M, int64_t N,
+                           int64_t K, int epilogue, int split_k, int block_n, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, gemm, A, lda, a_layout, B, ldb, b_layout, Cout, ldc, C2, bias, aux, ldaux, M, N, K, epilogue,
+                         split_k, block_n, stream);
 }

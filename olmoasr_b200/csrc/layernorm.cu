@@ -1,4 +1,4 @@
-// LayerNorm forward / backward, bf16 in/out with fp32 statistics (one warp per row, 16-byte loads,
+// LayerNorm forward / backward, bf16 or fp16 in/out with fp32 statistics (one warp per row, 16-byte loads,
 // shuffle reductions).  HBM-bound: 4 B/element forward, 6-8 B/element backward.
 //
 // Reference: LayerNorm.forward = F.layer_norm(x.float(), eps=1e-5).type(x.dtype)  (olmoasr/model.py:25-39);
@@ -11,10 +11,10 @@ namespace {
 
 constexpr int LN_MAX_VEC = 5;  // d <= 5 * 32 * 8 = 1280; kernels are instantiated per ceil(d / 256) to bound registers
 
-template <bool kWriteStats, int NV>
+template <typename T, bool kWriteStats, int NV>
 __global__ void __launch_bounds__(256)
-layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
-                     bf16* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out,
+layernorm_fwd_kernel(const T* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
+                     T* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out,
                      int64_t rows, int d, float eps) {
   const int warps_per_block = blockDim.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -29,7 +29,7 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ w, co
       const int vi = lane + 32 * i;
       if (vi < nvec) {
         const uint4 u = xr[vi];
-        float2 p0 = unpack_bf16x2(u.x), p1 = unpack_bf16x2(u.y), p2 = unpack_bf16x2(u.z), p3 = unpack_bf16x2(u.w);
+        float2 p0 = Act16<T>::unpack2(u.x), p1 = Act16<T>::unpack2(u.y), p2 = Act16<T>::unpack2(u.z), p3 = Act16<T>::unpack2(u.w);
         v[i][0] = p0.x; v[i][1] = p0.y; v[i][2] = p1.x; v[i][3] = p1.y;
         v[i][4] = p2.x; v[i][5] = p2.y; v[i][6] = p3.x; v[i][7] = p3.y;
 #pragma unroll
@@ -59,8 +59,8 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ w, co
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] = (v[i][j] - mean) * rstd * ww[j] + bb[j];
         uint4 u;
-        u.x = pack_bf16x2(o[0], o[1]); u.y = pack_bf16x2(o[2], o[3]);
-        u.z = pack_bf16x2(o[4], o[5]); u.w = pack_bf16x2(o[6], o[7]);
+        u.x = Act16<T>::pack2(o[0], o[1]); u.y = Act16<T>::pack2(o[2], o[3]);
+        u.z = Act16<T>::pack2(o[4], o[5]); u.w = Act16<T>::pack2(o[6], o[7]);
         yr[vi] = u;
       }
     }
@@ -74,11 +74,11 @@ layernorm_fwd_kernel(const bf16* __restrict__ x, const float* __restrict__ w, co
 // pass and the dx pass and are unpacked twice -- 32 registers instead of 64.  (History: all-fp32-in-registers needed
 // 214 registers -> 23 % of the HBM roofline; staging every row through shared memory with two __syncthreads per 8
 // rows -> 37 %.)
-template <int NV>
+template <typename T, int NV>
 __global__ void __launch_bounds__(256, 2)
-layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, const float* __restrict__ w,
+layernorm_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ x, const float* __restrict__ w,
                      const float* __restrict__ mean, const float* __restrict__ rstd,
-                     const bf16* __restrict__ dres, bf16* __restrict__ dx, float* __restrict__ part,
+                     const T* __restrict__ dres, T* __restrict__ dx, float* __restrict__ part,
                      int64_t rows, int d) {
   extern __shared__ __align__(16) float fold[];  // [8][d], used once at the end
   const int warp = threadIdx.x >> 5;
@@ -131,8 +131,8 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
         const uint32_t gw[4] = {ug[i].x, ug[i].y, ug[i].z, ug[i].w};
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          const float2 xh = fmul2(fadd2(unpack_bf16x2(xw[j]), make_float2(-mu, -mu)), rs2);
-          const float2 g = unpack_bf16x2(gw[j]);
+          const float2 xh = fmul2(fadd2(Act16<T>::unpack2(xw[j]), make_float2(-mu, -mu)), rs2);
+          const float2 g = Act16<T>::unpack2(gw[j]);
           const float2 gwj = fmul2(g, ww[j]);
           s1 = fadd2(s1, gwj);
           s2 = ffma2(gwj, xh, s2);
@@ -159,16 +159,16 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
         uint32_t ow[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          const float2 xh = fmul2(fadd2(unpack_bf16x2(xw[j]), make_float2(-mu, -mu)), rs2);
-          const float2 gwj = fmul2(unpack_bf16x2(gw[j]), ww[j]);
+          const float2 xh = fmul2(fadd2(Act16<T>::unpack2(xw[j]), make_float2(-mu, -mu)), rs2);
+          const float2 gwj = fmul2(Act16<T>::unpack2(gw[j]), ww[j]);
           // rs * (g*w - mean(g*w) - xhat * mean(g*w*xhat))
           float2 o = ffma2(xh, make_float2(-m2, -m2), fadd2(gwj, make_float2(-m1, -m1)));
           o = fmul2(o, rs2);
           if (rr) {
-            const float2 ob = unpack_bf16x2(pack_bf16x2(o.x, o.y));   // bf16(dx_ln) first, like autograd's accumulation
-            o = fadd2(unpack_bf16x2(rw[j]), ob);
+            const float2 ob = Act16<T>::unpack2(Act16<T>::pack2(o.x, o.y));   // T(dx_ln) first, like autograd's accumulation
+            o = fadd2(Act16<T>::unpack2(rw[j]), ob);
           }
-          ow[j] = pack_bf16x2(o.x, o.y);
+          ow[j] = Act16<T>::pack2(o.x, o.y);
         }
         dxr[vi] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
       }
@@ -200,13 +200,9 @@ layernorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x, co
   }
 }
 
-}  // namespace
-}  // namespace oasr
-
-using namespace oasr;
-
-extern "C" int oasr_layernorm_fwd(const void* x, const float* weight, const float* bias, void* y, float* mean,
-                                  float* rstd, int64_t rows, int64_t d, float eps, void* stream) {
+template <typename T>
+int layernorm_fwd(const void* x, const float* weight, const float* bias, void* y, float* mean, float* rstd, int64_t rows,
+                  int64_t d, float eps, void* stream) {
   OASR_REQUIRE(rows > 0 && d > 0, "layernorm: empty input");
   OASR_REQUIRE((d & 7) == 0 && d <= LN_MAX_VEC * 256, "layernorm: d=%ld must be a multiple of 8 and <= %d", (long)d, LN_MAX_VEC * 256);
   OASR_REQUIRE((mean == nullptr) == (rstd == nullptr), "layernorm: mean and rstd go together");
@@ -218,9 +214,9 @@ extern "C" int oasr_layernorm_fwd(const void* x, const float* weight, const floa
 #define OASR_LN_FWD(NVv)                                                                                          \
   do {                                                                                                           \
     if (mean)                                                                                                    \
-      layernorm_fwd_kernel<true, NVv><<<(int)blocks, wpb * 32, 0, st>>>((const bf16*)x, weight, bias, (bf16*)y, mean, rstd, rows, (int)d, eps); \
+      layernorm_fwd_kernel<T, true, NVv><<<(int)blocks, wpb * 32, 0, st>>>((const T*)x, weight, bias, (T*)y, mean, rstd, rows, (int)d, eps); \
     else                                                                                                         \
-      layernorm_fwd_kernel<false, NVv><<<(int)blocks, wpb * 32, 0, st>>>((const bf16*)x, weight, bias, (bf16*)y, nullptr, nullptr, rows, (int)d, eps); \
+      layernorm_fwd_kernel<T, false, NVv><<<(int)blocks, wpb * 32, 0, st>>>((const T*)x, weight, bias, (T*)y, nullptr, nullptr, rows, (int)d, eps); \
   } while (0)
   switch ((int)ceil_div(d, 256)) {
     case 1: case 2: OASR_LN_FWD(2); break;
@@ -233,9 +229,9 @@ extern "C" int oasr_layernorm_fwd(const void* x, const float* weight, const floa
   return OASR_OK;
 }
 
-extern "C" int oasr_layernorm_bwd(const void* dy, const void* x, const float* weight, const float* mean,
-                                  const float* rstd, const void* dresidual, void* dx, float* dweight,
-                                  float* dbias, int64_t rows, int64_t d, void* stream) {
+template <typename T>
+int layernorm_bwd(const void* dy, const void* x, const float* weight, const float* mean, const float* rstd,
+                  const void* dresidual, void* dx, float* dweight, float* dbias, int64_t rows, int64_t d, void* stream) {
   OASR_REQUIRE(rows > 0 && d > 0, "layernorm_bwd: empty input");
   OASR_REQUIRE((d & 7) == 0 && d <= LN_MAX_VEC * 256, "layernorm_bwd: unsupported d=%ld", (long)d);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -250,11 +246,11 @@ extern "C" int oasr_layernorm_bwd(const void* dy, const void* x, const float* we
   do {                                                                                                                 \
     static bool attr_set = false;                                                                                      \
     if (!attr_set) {                                                                                                   \
-      OASR_CUDA_OK(cudaFuncSetAttribute(layernorm_bwd_kernel<NVv>, cudaFuncAttributeMaxDynamicSharedMemorySize, NVv * 256 * 32)); \
+      OASR_CUDA_OK(cudaFuncSetAttribute(layernorm_bwd_kernel<T, NVv>, cudaFuncAttributeMaxDynamicSharedMemorySize, NVv * 256 * 32)); \
       attr_set = true;                                                                                                 \
     }                                                                                                                  \
-    layernorm_bwd_kernel<NVv><<<(int)blocks, wpb * 32, smem, st>>>(                                                    \
-        (const bf16*)dy, (const bf16*)x, weight, mean, rstd, (const bf16*)dresidual, (bf16*)dx, part, rows, (int)d); \
+    layernorm_bwd_kernel<T, NVv><<<(int)blocks, wpb * 32, smem, st>>>(                                                 \
+        (const T*)dy, (const T*)x, weight, mean, rstd, (const T*)dresidual, (T*)dx, part, rows, (int)d);             \
   } while (0)
   switch ((int)ceil_div(d, 256)) {
     case 1: case 2: OASR_LN_BWD(2); break;
@@ -268,4 +264,31 @@ extern "C" int oasr_layernorm_bwd(const void* dy, const void* x, const float* we
   if (rc == OASR_OK) rc = add_partials(part + blocks * d, (int)blocks, d, dbias, st);
   scratch_free(part, st);
   return rc;
+}
+
+}  // namespace
+}  // namespace oasr
+
+using namespace oasr;
+
+extern "C" int oasr_layernorm_fwd(const void* x, const float* weight, const float* bias, void* y, float* mean,
+                                  float* rstd, int64_t rows, int64_t d, float eps, void* stream) {
+  return layernorm_fwd<bf16>(x, weight, bias, y, mean, rstd, rows, d, eps, stream);
+}
+
+extern "C" int oasr_layernorm_bwd(const void* dy, const void* x, const float* weight, const float* mean,
+                                  const float* rstd, const void* dresidual, void* dx, float* dweight,
+                                  float* dbias, int64_t rows, int64_t d, void* stream) {
+  return layernorm_bwd<bf16>(dy, x, weight, mean, rstd, dresidual, dx, dweight, dbias, rows, d, stream);
+}
+
+extern "C" int oasr_layernorm_fwd16(const void* x, const float* weight, const float* bias, void* y, float* mean,
+                                    float* rstd, int64_t rows, int64_t d, float eps, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, layernorm_fwd, x, weight, bias, y, mean, rstd, rows, d, eps, stream);
+}
+
+extern "C" int oasr_layernorm_bwd16(const void* dy, const void* x, const float* weight, const float* mean,
+                                    const float* rstd, const void* dresidual, void* dx, float* dweight,
+                                    float* dbias, int64_t rows, int64_t d, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, layernorm_bwd, dy, x, weight, mean, rstd, dresidual, dx, dweight, dbias, rows, d, stream);
 }

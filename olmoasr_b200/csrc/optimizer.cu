@@ -16,7 +16,7 @@ struct TensorRec {  // one row of the device-side table (6 x int64)
   float* m;
   float* v;
   int64_t numel;
-  bf16* shadow;  // optional bf16 copy of p, refreshed by the update itself (nullptr: none)
+  bf16* shadow;  // optional bf16 (or, in the fp16 kernels, fp16) copy of p, refreshed by the update itself (nullptr: none)
 };
 
 // sum over the block into this block's partial (added up in block order afterwards: add_partials).  Callers square
@@ -77,10 +77,9 @@ sqnorm_flat_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ p
 // One thread: turns the squared norm into the step's scalars.  The step counter lives on the device and advances only
 // when the update is applied (GradScaler + AdamW do not count skipped steps), so no host read is needed per step.
 //   st[0] step  st[1] coef (unscale x clip)  st[2] 1 - beta1^t  st[3] sqrt(1 - beta2^t)  st[4] skip  st[5] grad norm
-__global__ void optim_prepare_kernel(const float* __restrict__ norm_sq, float* __restrict__ found_inf, float* __restrict__ st,
-                                     float inv_scale, float max_norm, float beta1, float beta2) {
-  const float nsq = *norm_sq;          // of the UNSCALED gradients (inv_scale is applied before squaring)
-  if (!isfinite(nsq)) {
+__device__ __forceinline__ void prepare_step(float nsq, bool skip, float* __restrict__ found_inf, float* __restrict__ st,
+                                             float inv_scale, float max_norm, float beta1, float beta2) {
+  if (skip || !isfinite(nsq)) {
     *found_inf = 1.f;
     st[4] = 1.f;
     st[5] = nsq;
@@ -97,12 +96,34 @@ __global__ void optim_prepare_kernel(const float* __restrict__ norm_sq, float* _
   st[4] = 0.f;
   st[5] = total_norm;
 }
+__global__ void optim_prepare_kernel(const float* __restrict__ norm_sq, float* __restrict__ found_inf, float* __restrict__ st,
+                                     float inv_scale, float max_norm, float beta1, float beta2) {
+  // of the UNSCALED gradients (inv_scale is applied before squaring)
+  prepare_step(*norm_sq, false, found_inf, st, inv_scale, max_norm, beta1, beta2);
+}
+// GradScaler form: the loss scale S and GradScaler's found_inf flag are read on the device, so the host never waits for
+// them.  norm_sq was taken over g * inv_scale, still multiplied by S: the norm of the unscaled gradients is
+// sqrt(norm_sq) / S, and every gradient is multiplied by inv_scale / S.  A set flag skips the step like a non-finite norm.
+__global__ void optim_prepare_amp_kernel(const float* __restrict__ norm_sq, float* __restrict__ found_inf,
+                                         float* __restrict__ st, const float* __restrict__ loss_scale,
+                                         const float* __restrict__ ext_found_inf, float inv_scale, float max_norm,
+                                         float beta1, float beta2) {
+  float nsq = *norm_sq;
+  if (loss_scale != nullptr) {
+    const float r = 1.f / *loss_scale;
+    nsq = nsq * r * r;
+    inv_scale *= r;
+  }
+  const bool skip = ext_found_inf != nullptr && *ext_found_inf != 0.f;
+  prepare_step(nsq, skip, found_inf, st, inv_scale, max_norm, beta1, beta2);
+}
 
 // One CHUNK of the update.  `st` is written by optim_prepare_kernel; when it flags a non-finite norm the whole update is
-// skipped (GradScaler semantics).  When `sh` is given the bf16 shadow the GEMMs read is refreshed from the value still
-// in registers -- the reference instead re-casts every fp32 master on every forward (olmoasr/model.py:97-101).
+// skipped (GradScaler semantics).  When `sh` is given the T (bf16 / fp16) shadow the GEMMs read is refreshed from the value
+// still in registers -- the reference instead re-casts every fp32 master on every forward (olmoasr/model.py:97-101).
+template <typename T>
 __device__ __forceinline__ void adamw_chunk(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                                            float* __restrict__ v, bf16* __restrict__ sh, int n, const float* __restrict__ st,
+                                            float* __restrict__ v, T* __restrict__ sh, int n, const float* __restrict__ st,
                                             float lr, float beta1, float beta2, float eps, float weight_decay) {
   if (st[4] != 0.f) return;
   const float coef = st[1], bc1 = st[2], bc2_sqrt = st[3];
@@ -128,7 +149,7 @@ __device__ __forceinline__ void adamw_chunk(float* __restrict__ p, const float* 
       *reinterpret_cast<float4*>(p + i) = pv;
       *reinterpret_cast<float4*>(m + i) = mv;
       *reinterpret_cast<float4*>(v + i) = vv;
-      if (sh != nullptr) *reinterpret_cast<uint2*>(sh + i) = make_uint2(pack_bf16x2(pv.x, pv.y), pack_bf16x2(pv.z, pv.w));
+      if (sh != nullptr) *reinterpret_cast<uint2*>(sh + i) = make_uint2(Act16<T>::pack2(pv.x, pv.y), Act16<T>::pack2(pv.z, pv.w));
     }
     i0 = n4;
   }
@@ -141,10 +162,11 @@ __device__ __forceinline__ void adamw_chunk(float* __restrict__ p, const float* 
     p[i] = pi;
     m[i] = mi;
     v[i] = vi;
-    if (sh != nullptr) sh[i] = __float2bfloat16_rn(pi);
+    if (sh != nullptr) sh[i] = Act16<T>::from_f(pi);
   }
 }
 
+template <typename T>
 __global__ void __launch_bounds__(256)
 adamw_kernel(const TensorRec* __restrict__ recs, const int2* __restrict__ chunks, const float* __restrict__ st, float lr,
              float beta1, float beta2, float eps, float weight_decay) {
@@ -152,13 +174,14 @@ adamw_kernel(const TensorRec* __restrict__ recs, const int2* __restrict__ chunks
   const TensorRec r = recs[ch.x];
   const int64_t start = static_cast<int64_t>(ch.y) * CHUNK;
   const int n = static_cast<int>(min(r.numel, start + CHUNK) - start);
-  adamw_chunk(r.p + start, r.g + start, r.m + start, r.v + start, r.shadow ? r.shadow + start : nullptr, n, st, lr, beta1,
+  adamw_chunk(r.p + start, r.g + start, r.m + start, r.v + start, r.shadow ? reinterpret_cast<T*>(r.shadow) + start : nullptr, n, st, lr, beta1,
               beta2, eps, weight_decay);
 }
 
+template <typename T>
 __global__ void __launch_bounds__(256)
 adamw_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                  bf16* __restrict__ sh, int64_t numel, const float* __restrict__ st, float lr, float beta1, float beta2,
+                  T* __restrict__ sh, int64_t numel, const float* __restrict__ st, float lr, float beta1, float beta2,
                   float eps, float weight_decay) {
   const int64_t start = static_cast<int64_t>(blockIdx.x) * CHUNK;
   const int n = static_cast<int>(min(numel, start + CHUNK) - start);
@@ -207,22 +230,48 @@ extern "C" int oasr_optim_prepare(const float* norm_sq, float* found_inf, float*
   return OASR_OK;
 }
 
-extern "C" int oasr_adamw_step(const void* recs, const void* chunks, int64_t n_chunks, const float* state, float lr, float beta1,
-                               float beta2, float eps, float weight_decay, void* stream) {
+static int adamw_step(const void* recs, const void* chunks, int64_t n_chunks, const float* state, float lr, float beta1,
+                      float beta2, float eps, float weight_decay, void* stream) {
   OASR_REQUIRE(n_chunks > 0 && state, "adamw: bad arguments");
-  adamw_kernel<<<(unsigned)n_chunks, 256, 0, (cudaStream_t)stream>>>((const TensorRec*)recs, (const int2*)chunks, state, lr, beta1,
+  adamw_kernel<bf16><<<(unsigned)n_chunks, 256, 0, (cudaStream_t)stream>>>((const TensorRec*)recs, (const int2*)chunks, state, lr, beta1,
                                                                     beta2, eps, weight_decay);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
 
-extern "C" int oasr_adamw_flat(float* p, const float* g, float* m, float* v, void* shadow_bf16, int64_t numel, const float* state,
-                               float lr, float beta1, float beta2, float eps, float weight_decay, void* stream) {
+template <typename T>
+static int adamw_flat(float* p, const float* g, float* m, float* v, void* shadow_bf16, int64_t numel, const float* state,
+                      float lr, float beta1, float beta2, float eps, float weight_decay, void* stream) {
   OASR_REQUIRE(numel > 0 && state, "adamw_flat: bad arguments");
   OASR_REQUIRE((((uintptr_t)p | (uintptr_t)g | (uintptr_t)m | (uintptr_t)v) & 15) == 0 && ((uintptr_t)shadow_bf16 & 7) == 0,
                "adamw_flat: slabs must be 16-byte aligned");
-  adamw_flat_kernel<<<(unsigned)ceil_div(numel, CHUNK), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, (bf16*)shadow_bf16, numel, state, lr,
+  adamw_flat_kernel<T><<<(unsigned)ceil_div(numel, CHUNK), 256, 0, (cudaStream_t)stream>>>(p, g, m, v, (T*)shadow_bf16, numel, state, lr,
                                                                                       beta1, beta2, eps, weight_decay);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
+}
+
+extern "C" int oasr_optim_prepare_amp(const float* norm_sq, float* found_inf, float* state, const float* loss_scale,
+                                      const float* ext_found_inf, float inv_scale, float max_norm, float beta1, float beta2,
+                                      void* stream) {
+  OASR_REQUIRE(norm_sq && found_inf && state, "optim_prepare_amp: null pointer");
+  optim_prepare_amp_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(norm_sq, found_inf, state, loss_scale, ext_found_inf, inv_scale,
+                                                              max_norm, beta1, beta2);
+  OASR_LAUNCH_CHECK();
+  return OASR_OK;
+}
+
+extern "C" int oasr_adamw_step(const void* recs, const void* chunks, int64_t n_chunks, const float* state, float lr, float beta1,
+                               float beta2, float eps, float weight_decay, void* stream) {
+  return adamw_step(recs, chunks, n_chunks, state, lr, beta1, beta2, eps, weight_decay, stream);
+}
+
+extern "C" int oasr_adamw_flat(float* p, const float* g, float* m, float* v, void* shadow_bf16, int64_t numel, const float* state,
+                               float lr, float beta1, float beta2, float eps, float weight_decay, void* stream) {
+  return adamw_flat<bf16>(p, g, m, v, shadow_bf16, numel, state, lr, beta1, beta2, eps, weight_decay, stream);
+}
+
+extern "C" int oasr_adamw_flat16(float* p, const float* g, float* m, float* v, void* shadow, int64_t numel, const float* state,
+                                 float lr, float beta1, float beta2, float eps, float weight_decay, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, adamw_flat, p, g, m, v, shadow, numel, state, lr, beta1, beta2, eps, weight_decay, stream);
 }

@@ -300,6 +300,8 @@ class DecodeEngine:
         from ._core import _as_bf16_2d, linear_fwd
 
         self.refresh_weights()
+        if getattr(self.model, "_slabs", None) is not None:
+            self.model._slabs.ensure_synced()    # the shadow slab in bf16 again after an fp16 training step
         n = audio_features.shape[0]
         if n > self.max_batch:
             raise ValueError(f"DecodeEngine: {n} sequences > max_batch {self.max_batch}")

@@ -199,6 +199,12 @@ class DecodingTask:
 
     @torch.no_grad()
     def run(self, mel: Tensor, tokenizer=None) -> List[DecodingResult]:
+        from ._core import bf16_compute
+
+        with bf16_compute():     # decoding computes in bf16 / its engine's type, also inside an fp16 autocast region
+            return self._run(mel, tokenizer)
+
+    def _run(self, mel: Tensor, tokenizer=None) -> List[DecodingResult]:
         model, opt = self.model, self.options
         if mel.shape[-2:] == (model.dims.n_audio_ctx, model.dims.n_audio_state):
             audio_features = mel  # encoded features were passed in (DecodingTask._get_audio_features)

@@ -2,6 +2,10 @@
 
 Shapes / dtypes are validated here so that a bad call fails with a Python exception before any
 kernel is launched; the kernels themselves never allocate.
+
+Activations are bf16 or fp16 (the model under torch.autocast(dtype=torch.float16)); each wrapper takes the type from
+its 16-bit tensor arguments, or from `dtype` where every input is fp32.  bf16 calls go to the bf16 entry points, fp16
+calls to their `16` twins (include/oasr_b200.h).
 """
 from __future__ import annotations
 
@@ -30,11 +34,25 @@ def _req(cond, msg):
         raise ValueError(msg)
 
 
+ACT16 = (torch.bfloat16, torch.float16)
+_TWIN16 = {"oasr_gemm_bf16": "oasr_gemm16", "oasr_colsum_bf16": "oasr_colsum16", "oasr_logits_to_f32": "oasr_logits_to_f32_16",
+           "oasr_im2col_conv1": "oasr_im2col_conv1_16"}
+
+
+def _call16(name, dtype, *args):
+    """Entry point `name` for bf16; for fp16 its twin, which takes the dtype code before the stream."""
+    if dtype == torch.bfloat16:
+        return call(name, *args)
+    _req(dtype == torch.float16, f"{name}: 16-bit activations must be bf16 or fp16, got {dtype}")
+    call(_TWIN16.get(name, name + "16"), *args[:-1], _lib.DTYPE_F16, args[-1])
+
+
 def gemm(a, b, M, N, K, *, a_mn=False, b_mn=False, out=None, out2=None, bias=None, aux=None,
          epi=EPI_BF16, split_k=1, block_n=0):
     """D[M,N] = epi(sum_k A[m,k] B[n,k]) on wgmma.  `a` is (M,K) (or (K,M) when a_mn), `b` is (N,K)
-    (or (K,N) when b_mn); both bf16 with unit inner stride.  See include/oasr_b200.h."""
-    _req(a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16, "gemm: operands must be bf16")
+    (or (K,N) when b_mn); both bf16 or both fp16, with unit inner stride.  See include/oasr_b200.h."""
+    dt = a.dtype
+    _req(dt in ACT16 and b.dtype == dt, "gemm: operands must be both bf16 or both fp16")
     _req(a.is_cuda and b.is_cuda, "gemm: operands must be CUDA tensors")
     _req(a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1, "gemm: 2-D, unit inner stride")
     _req(tuple(a.shape) == ((K, M) if a_mn else (M, K)), f"gemm: A shape {tuple(a.shape)} vs M={M} K={K} a_mn={a_mn}")
@@ -42,13 +60,13 @@ def gemm(a, b, M, N, K, *, a_mn=False, b_mn=False, out=None, out2=None, bias=Non
     f32_out = epi in (EPI_F32, EPI_F32_ATOMIC_ADD)
     if out is None:
         _req(epi != EPI_F32_ATOMIC_ADD, "gemm: atomic-add epilogue needs a pre-initialised `out`")
-        out = torch.empty((M, N), device=a.device, dtype=torch.float32 if f32_out else torch.bfloat16)
-    _req(out.dtype == (torch.float32 if f32_out else torch.bfloat16), "gemm: out dtype")
+        out = torch.empty((M, N), device=a.device, dtype=torch.float32 if f32_out else dt)
+    _req(out.dtype == (torch.float32 if f32_out else dt), "gemm: out dtype")
     _req(out.dim() == 2 and out.shape[0] == M and out.shape[1] >= N and out.stride(1) == 1, "gemm: out shape")
     if epi == EPI_BF16_GELU and out2 is None:
         out2 = torch.empty_like(out)
     if aux is not None:
-        _req(aux.dtype == torch.bfloat16 and aux.stride(1) == 1 and aux.shape[0] == M, "gemm: aux")
+        _req(aux.dtype == dt and aux.stride(1) == 1 and aux.shape[0] == M, "gemm: aux")
     if bias is not None:
         _req(bias.dtype == torch.float32 and bias.numel() >= N and bias.is_contiguous(), "gemm: bias must be f32")
     prof = GEMM_PROFILE
@@ -56,7 +74,7 @@ def gemm(a, b, M, N, K, *, a_mn=False, b_mn=False, out=None, out2=None, bias=Non
         e0 = torch.cuda.Event(enable_timing=True)
         e1 = torch.cuda.Event(enable_timing=True)
         e0.record()
-    call("oasr_gemm_bf16", ptr(a), a.stride(0), int(a_mn), ptr(b), b.stride(0), int(b_mn),
+    _call16("oasr_gemm_bf16", dt, ptr(a), a.stride(0), int(a_mn), ptr(b), b.stride(0), int(b_mn),
          ptr(out), out.stride(0), ptr(out2), ptr(bias), ptr(aux), aux.stride(0) if aux is not None else 0,
          M, N, K, epi, split_k, block_n, stream())
     if prof is not None:
@@ -68,13 +86,15 @@ def gemm(a, b, M, N, K, *, a_mn=False, b_mn=False, out=None, out2=None, bias=Non
 
 
 # ----------------------------------------------------------------------------------------------------
-def _bf16_2d(t, name):
-    _req(t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(1) == 1, f"{name}: 2-D bf16 CUDA tensor, unit inner stride")
+def _bf16_2d(t, name, dtype=torch.bfloat16):
+    _req(t.is_cuda and t.dtype == dtype and t.dim() == 2 and t.stride(1) == 1,
+         f"{name}: 2-D {str(dtype).removeprefix('torch.')} CUDA tensor, unit inner stride")
 
 
 def layernorm_fwd(x, weight, bias, eps=1e-5, want_stats=True):
-    """x (rows, d) bf16 contiguous -> y bf16 [, mean, rstd f32].  model.py:25-39."""
-    _bf16_2d(x, "layernorm x")
+    """x (rows, d) bf16 / fp16 contiguous -> y of x's type [, mean, rstd f32].  model.py:25-39."""
+    _req(x.dtype in ACT16, "layernorm: x must be bf16 or fp16")
+    _bf16_2d(x, "layernorm x", x.dtype)
     _req(x.is_contiguous() and weight.dtype == torch.float32 and bias.dtype == torch.float32, "layernorm: contiguous x, f32 params")
     rows, d = x.shape
     y = torch.empty_like(x)
@@ -82,67 +102,72 @@ def layernorm_fwd(x, weight, bias, eps=1e-5, want_stats=True):
     if want_stats:
         mean = torch.empty(rows, device=x.device, dtype=torch.float32)
         rstd = torch.empty(rows, device=x.device, dtype=torch.float32)
-    call("oasr_layernorm_fwd", ptr(x), ptr(weight), ptr(bias), ptr(y), ptr(mean), ptr(rstd), rows, d, eps, stream())
+    _call16("oasr_layernorm_fwd", x.dtype, ptr(x), ptr(weight), ptr(bias), ptr(y), ptr(mean), ptr(rstd), rows, d, eps, stream())
     return (y, mean, rstd) if want_stats else y
 
 
 def layernorm_bwd(dy, x, weight, mean, rstd, dweight, dbias, dresidual=None):
-    """Returns dx = bf16(dresidual + bf16(dx_ln)); accumulates into dweight / dbias (f32)."""
-    _bf16_2d(dy, "layernorm dy"); _bf16_2d(x, "layernorm x")
+    """Returns dx = T(dresidual + T(dx_ln)) (T = x's 16-bit type); accumulates into dweight / dbias (f32)."""
+    _req(x.dtype in ACT16, "layernorm_bwd: x must be bf16 or fp16")
+    _bf16_2d(dy, "layernorm dy", x.dtype); _bf16_2d(x, "layernorm x", x.dtype)
     _req(dy.is_contiguous() and x.is_contiguous() and (dresidual is None or dresidual.is_contiguous()), "layernorm_bwd: contiguous")
     rows, d = x.shape
     dx = torch.empty_like(x)
-    call("oasr_layernorm_bwd", ptr(dy), ptr(x), ptr(weight), ptr(mean), ptr(rstd), ptr(dresidual), ptr(dx), ptr(dweight),
+    _call16("oasr_layernorm_bwd", x.dtype, ptr(dy), ptr(x), ptr(weight), ptr(mean), ptr(rstd), ptr(dresidual), ptr(dx), ptr(dweight),
          ptr(dbias), rows, d, stream())
     return dx
 
 
 def attention_fwd(q, k, v, B, H, Tq, Tkv, causal=False, kv_len=None, scale=None, want_lse=True, out=None):
-    """q (B*Tq, >=H*64) bf16 view, k/v (B*Tkv, ...) views (column slices of fused projections are fine)."""
+    """q (B*Tq, >=H*64) bf16 / fp16 view, k/v (B*Tkv, ...) views (column slices of fused projections are fine)."""
+    _req(q.dtype in ACT16, "attention: q must be bf16 or fp16")
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
-        _bf16_2d(t, n)
+        _bf16_2d(t, n, q.dtype)
     _req(q.shape[0] == B * Tq and k.shape[0] == B * Tkv and v.shape[0] == B * Tkv, "attention: row counts")
     _req(q.shape[1] == H * 64 and k.shape[1] == H * 64 and v.shape[1] == H * 64, "attention: width must be H*64")
     if scale is None:
         scale = 64 ** -0.5
     if out is None:
-        out = torch.empty((B * Tq, H * 64), device=q.device, dtype=torch.bfloat16)
+        out = torch.empty((B * Tq, H * 64), device=q.device, dtype=q.dtype)
     lse = torch.empty((B, H, Tq), device=q.device, dtype=torch.float32) if want_lse else None
     if kv_len is not None:
         _req(kv_len.dtype == torch.int32 and kv_len.numel() == B, "attention: kv_len must be int32 (B,)")
-    call("oasr_attention_fwd", ptr(q), q.stride(0), ptr(k), k.stride(0), ptr(v), v.stride(0), ptr(out), out.stride(0),
+    _call16("oasr_attention_fwd", q.dtype, ptr(q), q.stride(0), ptr(k), k.stride(0), ptr(v), v.stride(0), ptr(out), out.stride(0),
          ptr(lse), B, H, Tq, Tkv, 64, int(causal), ptr(kv_len), float(scale), stream())
     return out, lse
 
 
 def attention_bwd(q, k, v, o, dout, lse, B, H, Tq, Tkv, causal=False, kv_len=None, scale=None, dq=None, dk=None, dv=None):
+    dt = q.dtype
+    _req(dt in ACT16, "attention_bwd: q must be bf16 or fp16")
     for t, n in ((q, "q"), (k, "k"), (v, "v"), (o, "o"), (dout, "dout")):
-        _bf16_2d(t, n)
+        _bf16_2d(t, n, dt)
     if scale is None:
         scale = 64 ** -0.5
     dev = q.device
     if dq is None:
-        dq = torch.empty((B * Tq, H * 64), device=dev, dtype=torch.bfloat16)
+        dq = torch.empty((B * Tq, H * 64), device=dev, dtype=dt)
     if dk is None:
-        dk = torch.empty((B * Tkv, H * 64), device=dev, dtype=torch.bfloat16)
+        dk = torch.empty((B * Tkv, H * 64), device=dev, dtype=dt)
     if dv is None:
-        dv = torch.empty((B * Tkv, H * 64), device=dev, dtype=torch.bfloat16)
+        dv = torch.empty((B * Tkv, H * 64), device=dev, dtype=dt)
     delta = torch.empty((B, H, Tq), device=dev, dtype=torch.float32)
-    call("oasr_attention_bwd", ptr(q), q.stride(0), ptr(k), k.stride(0), ptr(v), v.stride(0), ptr(o), o.stride(0),
+    _call16("oasr_attention_bwd", dt, ptr(q), q.stride(0), ptr(k), k.stride(0), ptr(v), v.stride(0), ptr(o), o.stride(0),
          ptr(dout), dout.stride(0), ptr(lse), ptr(delta), ptr(dq), dq.stride(0), ptr(dk), dk.stride(0),
          ptr(dv), dv.stride(0), B, H, Tq, Tkv, 64, int(causal), ptr(kv_len), float(scale), stream())
     return dq, dk, dv
 
 
 def ce_fwd(logits, targets, V, ignore_index):
-    """logits (rows, ld) bf16; returns (lse (rows,), lsc (4,)): lsc = [loss sum, target count, bad-target count, -];
+    """logits (rows, ld) bf16 / fp16; returns (lse (rows,), lsc (4,)): lsc = [loss sum, target count, bad-target count, -];
     `ce_finalize(lsc)` turns it into the mean loss."""
-    _bf16_2d(logits, "ce logits")
+    _req(logits.dtype in ACT16, "ce: logits must be bf16 or fp16")
+    _bf16_2d(logits, "ce logits", logits.dtype)
     rows = logits.shape[0]
     _req(targets.dtype == torch.int64 and targets.numel() == rows and targets.is_contiguous(), "ce: targets int64 (rows,)")
     lse = torch.empty(rows, device=logits.device, dtype=torch.float32)
     lsc = torch.zeros(4, device=logits.device, dtype=torch.float32)
-    call("oasr_ce_fwd", ptr(logits), ptr(targets), ptr(lse), ptr(lsc), rows, V, logits.stride(0), ignore_index, stream())
+    _call16("oasr_ce_fwd", logits.dtype, ptr(logits), ptr(targets), ptr(lse), ptr(lsc), rows, V, logits.stride(0), ignore_index, stream())
     return lse, lsc
 
 
@@ -154,31 +179,31 @@ def ce_finalize(lsc):
 
 
 def ce_bwd_(logits, targets, lse, lsc, grad_out, V, ignore_index):
-    """In place: logits <- d(loss)/d(logits) as bf16."""
+    """In place: logits <- d(loss)/d(logits) in the logits' 16-bit type."""
     _req(grad_out.dtype == torch.float32 and grad_out.numel() == 1, "ce_bwd: grad_out must be one f32")
-    call("oasr_ce_bwd", ptr(logits), ptr(targets), ptr(lse), ptr(lsc), ptr(grad_out), logits.shape[0], V, logits.stride(0),
+    _call16("oasr_ce_bwd", logits.dtype, ptr(logits), ptr(targets), ptr(lse), ptr(lsc), ptr(grad_out), logits.shape[0], V, logits.stride(0),
          ignore_index, stream())
     return logits
 
 
 def logits_to_f32(logits, V):
     out = torch.empty((logits.shape[0], V), device=logits.device, dtype=torch.float32)
-    call("oasr_logits_to_f32", ptr(logits), ptr(out), logits.shape[0], V, logits.stride(0), stream())
+    _call16("oasr_logits_to_f32", logits.dtype, ptr(logits), ptr(out), logits.shape[0], V, logits.stride(0), stream())
     return out
 
 
-def embed_fwd(ids, emb, pos, pos_offset=0):
+def embed_fwd(ids, emb, pos, pos_offset=0, dtype=torch.bfloat16):
     _req(ids.dtype == torch.int64 and ids.dim() == 2 and ids.is_contiguous(), "embed: ids int64 (B,S)")
     B, S = ids.shape
     d = emb.shape[1]
-    out = torch.empty((B * S, d), device=emb.device, dtype=torch.bfloat16)
-    call("oasr_embed_fwd", ptr(ids), ptr(emb), ptr(pos), ptr(out), B, S, d, pos_offset, emb.shape[0], stream())
+    out = torch.empty((B * S, d), device=emb.device, dtype=dtype)
+    _call16("oasr_embed_fwd", dtype, ptr(ids), ptr(emb), ptr(pos), ptr(out), B, S, d, pos_offset, emb.shape[0], stream())
     return out
 
 
 def embed_bwd(ids, dx, demb, dpos, padding_idx):
     B, S = ids.shape
-    call("oasr_embed_bwd", ptr(ids), ptr(dx), ptr(demb), ptr(dpos), B, S, dx.shape[1], padding_idx, demb.shape[0], stream())
+    _call16("oasr_embed_bwd", dx.dtype, ptr(ids), ptr(dx), ptr(demb), ptr(dpos), B, S, dx.shape[1], padding_idx, demb.shape[0], stream())
 
 
 def cast_bf16(src, dst=None):
@@ -189,12 +214,12 @@ def cast_bf16(src, dst=None):
     return dst
 
 
-def cast_conv_weight(w, dst=None):
+def cast_conv_weight(w, dst=None, dtype=torch.bfloat16):
     c_out, c_in, k = w.shape
     _req(k == 3 and w.is_contiguous() and w.dtype == torch.float32, "conv weight (C_out, C_in, 3) f32")
     if dst is None:
-        dst = torch.empty((c_out, 3 * c_in), device=w.device, dtype=torch.bfloat16)
-    call("oasr_cast_conv_weight", ptr(w), ptr(dst), c_out, c_in, stream())
+        dst = torch.empty((c_out, 3 * c_in), device=w.device, dtype=dtype)
+    _call16("oasr_cast_conv_weight", dst.dtype, ptr(w), ptr(dst), c_out, c_in, stream())
     return dst
 
 
@@ -215,44 +240,44 @@ def mask_to_kvlen(mask, err_flag):
     return kv
 
 
-def im2col_conv1(mel, kpad):
+def im2col_conv1(mel, kpad, dtype=torch.bfloat16):
     B, C, T = mel.shape
     _req(mel.dtype == torch.float32 and mel.is_contiguous(), "mel f32 contiguous")
-    A = torch.empty((B * T, kpad), device=mel.device, dtype=torch.bfloat16)
-    call("oasr_im2col_conv1", ptr(mel), ptr(A), B, C, T, kpad, stream())
+    A = torch.empty((B * T, kpad), device=mel.device, dtype=dtype)
+    _call16("oasr_im2col_conv1", dtype, ptr(mel), ptr(A), B, C, T, kpad, stream())
     return A
 
 
 def im2col_conv2(h, B, T_in, d):
     T_out = (T_in + 2 - 3) // 2 + 1
-    A = torch.empty((B * T_out, 3 * d), device=h.device, dtype=torch.bfloat16)
+    A = torch.empty((B * T_out, 3 * d), device=h.device, dtype=h.dtype)   # a copy: one kernel serves both 16-bit types
     call("oasr_im2col_conv2", ptr(h), ptr(A), B, T_in, T_out, d, stream())
     return A
 
 
 def col2im_conv2_gelu_bwd(dA, pre1, B, T_in, T_out, d):
-    out = torch.empty((B * T_in, d), device=dA.device, dtype=torch.bfloat16)
-    call("oasr_col2im_conv2_gelu_bwd", ptr(dA), ptr(pre1), ptr(out), B, T_in, T_out, d, stream())
+    out = torch.empty((B * T_in, d), device=dA.device, dtype=dA.dtype)
+    _call16("oasr_col2im_conv2_gelu_bwd", dA.dtype, ptr(dA), ptr(pre1), ptr(out), B, T_in, T_out, d, stream())
     return out
 
 
 def add_pos(x, pos, T):
     out = torch.empty_like(x)
-    call("oasr_add_pos", ptr(x), ptr(pos), ptr(out), x.shape[0], T, x.shape[1], stream())
+    _call16("oasr_add_pos", x.dtype, ptr(x), ptr(pos), ptr(out), x.shape[0], T, x.shape[1], stream())
     return out
 
 
 def gelu_bwd(dy, pre):
     out = torch.empty_like(dy)
-    call("oasr_gelu_bwd", ptr(dy), ptr(pre), ptr(out), dy.numel(), stream())
+    _call16("oasr_gelu_bwd", dy.dtype, ptr(dy), ptr(pre), ptr(out), dy.numel(), stream())
     return out
 
 
 def colsum_(dy, db, N=None):
-    """db (f32) += column sums of dy (M, N) bf16."""
+    """db (f32) += column sums of dy (M, N) bf16 / fp16."""
     M = dy.shape[0]
     N = dy.shape[1] if N is None else N
-    call("oasr_colsum_bf16", ptr(dy), ptr(db), M, N, dy.stride(0), stream())
+    _call16("oasr_colsum_bf16", dy.dtype, ptr(dy), ptr(db), M, N, dy.stride(0), stream())
     return db
 
 

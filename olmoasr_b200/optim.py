@@ -19,10 +19,21 @@ import math
 import numpy as np
 import torch
 
-from ._lib import call, lib, ptr, stream
+from ._lib import DTYPE_F16 as _DTYPE_F16, call, lib, ptr, stream
+
+
+def _f32_scalar(t):
+    """One fp32 element on the device (GradScaler's scale and found_inf are fp32; None passes through)."""
+    if t is None or t.dtype == torch.float32:
+        return t
+    return t.float()
 
 
 class FusedAdamW(torch.optim.Optimizer):
+    # torch.amp.GradScaler.step hands a scaling-aware optimizer its loss scale and found-inf flag as the device tensors
+    # `grad_scale` / `found_inf` instead of unscaling the gradients and reading the flag on the host
+    _step_supports_amp_scaling = True
+
     def __init__(self, params, lr=1.5e-3, betas=(0.9, 0.98), eps=1e-6, weight_decay=0.1, max_grad_norm=1.0, slabs=None):
         defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
         super().__init__(params, defaults)
@@ -88,7 +99,12 @@ class FusedAdamW(torch.optim.Optimizer):
     @torch.no_grad()
     def step(self, closure=None, inv_scale: float = 1.0):
         """`inv_scale` multiplies every gradient before clipping: 1 / loss_scale (GradScaler.unscale_) and / or
-        1 / world_size when the gradients were summed, not averaged, across ranks (olmoasr_b200.ddp)."""
+        1 / world_size when the gradients were summed, not averaged, across ranks (olmoasr_b200.ddp).
+
+        Under `scaler.step(opt)` GradScaler sets `self.grad_scale` (its scale S, or None when `scaler.unscale_(opt)` already
+        ran) and `self.found_inf` (device tensors): the gradients are then also multiplied by 1 / S and the update is skipped,
+        and not counted, when found_inf is set or the norm is not finite -- decided on the device, so the step never waits
+        for the host."""
         if closure is not None:
             raise ValueError("FusedAdamW does not take a closure")
         if not self._built:
@@ -102,9 +118,19 @@ class FusedAdamW(torch.optim.Optimizer):
         else:
             self._upload_grad_pointers()
             call("oasr_grad_sqnorm", ptr(self._dev_tab), ptr(self._chunks), self._n_chunks, float(inv_scale), ptr(self._norm_sq), s)
-        call("oasr_optim_prepare", ptr(self._norm_sq), ptr(self._found_inf), ptr(self._dev_state), float(inv_scale),
-             float(self.max_grad_norm or 0.0), b1, b2, s)
-        if sl is not None:
+        # instance attributes set by GradScaler.step (found_inf also names a method of this class)
+        grad_scale, found_inf = self.__dict__.get("grad_scale"), self.__dict__.get("found_inf")
+        if grad_scale is None and found_inf is None:
+            call("oasr_optim_prepare", ptr(self._norm_sq), ptr(self._found_inf), ptr(self._dev_state), float(inv_scale),
+                 float(self.max_grad_norm or 0.0), b1, b2, s)
+        else:
+            call("oasr_optim_prepare_amp", ptr(self._norm_sq), ptr(self._found_inf), ptr(self._dev_state),
+                 ptr(_f32_scalar(grad_scale)), ptr(_f32_scalar(found_inf)), float(inv_scale), float(self.max_grad_norm or 0.0),
+                 b1, b2, s)
+        if sl is not None and sl.S_dtype != torch.bfloat16:
+            call("oasr_adamw_flat16", ptr(sl.P), ptr(sl.G), ptr(sl.M), ptr(sl.V), ptr(sl.S), sl.numel, ptr(self._dev_state),
+                 float(group["lr"]), b1, b2, group["eps"], group["weight_decay"], _DTYPE_F16, s)
+        elif sl is not None:
             call("oasr_adamw_flat", ptr(sl.P), ptr(sl.G), ptr(sl.M), ptr(sl.V), ptr(sl.S), sl.numel, ptr(self._dev_state),
                  float(group["lr"]), b1, b2, group["eps"], group["weight_decay"], s)
         else:

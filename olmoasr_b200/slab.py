@@ -8,7 +8,8 @@ layout:
     P  fp32 master weights      (every nn.Parameter is a view into it; state_dict names / shapes are unchanged)
     G  fp32 gradients           (p.grad is a view; wgrad GEMM epilogues accumulate straight into it)
     M, V  fp32 AdamW moments    (optimizer state views, torch.optim.AdamW's names)
-    S  bf16 shadow of P         (what the wgmma GEMMs read; rewritten by the AdamW kernel from registers)
+    S  16-bit shadow of P       (what the wgmma GEMMs read; rewritten by the AdamW kernel from registers).  It holds the
+                                type the model last computed in: bf16, or fp16 under torch.autocast(float16)
 
 so that the optimizer is three launches over flat memory, zero_grad is one memset, the bf16 weights cost no extra
 pass, and a data-parallel gradient sum is a handful of large contiguous NCCL all-reduces (`SlabGradSync` in ddp.py)
@@ -63,6 +64,7 @@ class ParamSlabs:
         self.P = torch.zeros(off, device=dev, dtype=torch.float32)
         self.G = torch.zeros(off, device=dev, dtype=torch.float32)
         self.S = torch.zeros(off, device=dev, dtype=torch.bfloat16) if shadows else None
+        self.S_dtype = torch.bfloat16   # what S holds; S itself stays a bf16 tensor and is read as S_dtype (same size)
         self.M: Optional[Tensor] = None     # allocated by the optimizer (FusedAdamW) on first use
         self.V: Optional[Tensor] = None
         with torch.no_grad():
@@ -112,21 +114,33 @@ class ParamSlabs:
             if g is None or g.data_ptr() != self.G.data_ptr() + 4 * o:
                 p.grad = self.G[o:o + p.numel()].view(p.shape)
 
-    # ---- bf16 shadows ------------------------------------------------------------------------------------
+    # ---- 16-bit shadows ----------------------------------------------------------------------------------
     def _signature(self):
         return tuple(p._version for p in self.params)
 
+    def shadow_slab(self) -> Optional[Tensor]:
+        """S read as the type it holds."""
+        return None if self.S is None else (self.S if self.S_dtype == torch.bfloat16 else self.S.view(self.S_dtype))
+
     def sync_shadows(self):
-        """S <- bf16(P) in one flat cast (+ the model's non-elementwise shadows).  Needed after anything other than the
+        """S <- S_dtype(P) in one flat cast (+ the model's non-elementwise shadows).  Needed after anything other than the
         fused optimizer changed the masters (initialisation, load_state_dict, a foreign optimizer)."""
         if self.S is not None:
             from . import kernels as K
-            K.cast_bf16(self.P, self.S)
+            if self.S_dtype == torch.bfloat16:
+                K.cast_bf16(self.P, self.S)
+            else:
+                K.convert(self.P, self.shadow_slab())
         if self._extra_sync is not None:
             self._extra_sync()
         self._synced_sig = self._signature()
 
-    def ensure_synced(self):
+    def ensure_synced(self, dtype: torch.dtype = torch.bfloat16):
+        """Make S current, in `dtype` (the type of the forward about to run): a change of type re-casts it, e.g. an fp16
+        training step followed by a bf16 evaluation."""
+        if self.S is not None and dtype != self.S_dtype:
+            self.S_dtype = dtype
+            self._synced_sig = None
         if self._synced_sig != self._signature():
             self.sync_shadows()
 

@@ -41,6 +41,15 @@ def main():
         opt.zero_grad()
         loss.backward()
         opt.step()
+    # the same step in fp16 with GradScaler: every fp16 instantiation and the device-side unscale / skip
+    scaler = torch.amp.GradScaler("cuda")
+    for _ in range(2):
+        with torch.autocast("cuda", dtype=torch.float16):
+            loss = m(mel, ti, pmask, targets=ty)
+        opt.zero_grad()
+        scaler.scale(loss).backward()
+        scaler.step(opt)
+        scaler.update()
     # decode engine: direct (3 sequences) and staged (40 sequences) skinny GEMMs, split and fused attention, sampling
     im = InfModel(dims).to(dev)
     with torch.no_grad():
