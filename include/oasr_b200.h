@@ -292,6 +292,32 @@ OASR_API int oasr_dec_beam_reorder(void* k_cache, void* v_cache, int64_t layer_s
                                    const int32_t* src_rows, const int32_t* pos_ptr, int32_t n_clips, int32_t beam, int32_t d,
                                    int32_t n_pos_blocks, int dtype, void* stream);
 
+/* ---- word-level timestamps (whisper/timing.py find_alignment + dtw; the reference's transcribe.py:410-485) --------
+ * oasr_align_cost: the DTW input of one window from the alignment heads' captured 16-bit query rows and cross keys.
+ *   heads: DEVICE table of n_heads entries; q -> element (0, h * 64) of the layer's cross-attention query projection
+ *   (n_tok rows, stride ldq), k -> element (0, h * 64) of that layer's cross key (>= n_frames rows, stride ldk), both of
+ *   type `dtype` (OASR_DTYPE_BF16 / OASR_DTYPE_F16).  Per head, in fp32:
+ *     QK = (q . k) / 8 (= (q hd^-1/4)(k hd^-1/4), qk_scale 1) over frames [0, n_frames);  W = softmax over frames;
+ *     W = (W - mean) / std per frame over all n_tok rows (unbiased=False);  median filter of medfilt_width along frames
+ *     with reflect padding (none when n_frames <= medfilt_width / 2);
+ *   then the mean over heads (added in table order) of rows [1, n_tok - 1) is negated:
+ *     cost (n_tok - 2, n_frames) fp32, row stride ld_cost.
+ *   row_stats: (n_heads, n_tok, 2) fp32 workspace.  head_dim == 64, 3 <= n_tok <= 448, 1 <= n_frames <= 1500,
+ *   medfilt_width odd and <= 7.  Two launches; bit-identical from run to run.
+ * oasr_dtw: dynamic time warping of x (rows, cols) fp32 (row stride ldx), whisper's tie order: with
+ *   c0 = cost[i-1][j-1], c1 = cost[i-1][j], c2 = cost[i][j-1]: t = 0 if c0 < c1 and c0 < c2, else 1 if c1 < c0 and
+ *   c1 < c2, else 2; cost[i][j] = x[i-1][j-1] + c rounded to float32.  trace: (rows + 1) x (cols + 1) byte workspace.
+ *   Writes the path (text_idx, time_idx) (int32, room for rows + cols entries) in path order and its length to
+ *   *path_len.  One CTA; rows <= 17065. */
+typedef struct oasr_align_head {
+  const void* q; const void* k; int64_t ldq; int64_t ldk;
+} oasr_align_head;
+OASR_API int oasr_align_cost(const oasr_align_head* heads, int32_t n_heads, int32_t head_dim, int32_t n_tok,
+                             int32_t n_frames, int32_t medfilt_width, float* row_stats, float* cost, int64_t ld_cost,
+                             int dtype, void* stream);
+OASR_API int oasr_dtw(const float* x, int64_t ldx, int32_t rows, int32_t cols, uint8_t* trace, int32_t* text_idx,
+                      int32_t* time_idx, int32_t* path_len, void* stream);
+
 /* elementwise dtype conversion (weights fp32 -> T once per engine; bf16 encoder output / cross K,V -> fp16) */
 OASR_API int oasr_convert(const void* src, int src_dtype, void* dst, int dst_dtype, int64_t n, void* stream);
 

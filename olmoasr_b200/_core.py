@@ -1105,6 +1105,43 @@ class OLMoASRBase(nn.Module):
     def num_languages(self):
         return self.dims.n_vocab - 51765 - int(self.is_multilingual)
 
+    # ---- word-timestamp alignment heads -------------------------------------------------------------------------
+    # A plain attribute, not a buffer: state_dict(), buffers(), the slab layout and FSDP see exactly the parameters and
+    # buffers of the reference.  Default as upstream Whisper: every head of the upper half of the decoder layers.
+    _alignment_mask: Optional[Tensor] = None
+
+    @property
+    def alignment_heads(self) -> Tensor:
+        """Sparse bool (n_text_layer, n_text_head) tensor of the cross-attention heads word timestamps align with;
+        `.indices()` lists them in ascending (layer, head) order."""
+        if self._alignment_mask is None:
+            mask = torch.zeros(self.dims.n_text_layer, self.dims.n_text_head, dtype=torch.bool)
+            mask[self.dims.n_text_layer // 2:] = True
+            self._alignment_mask = mask
+        return self._alignment_mask.to_sparse()
+
+    def set_alignment_heads(self, dump):
+        """Select the alignment heads: upstream's base85-encoded gzip dump of the bool mask (bytes or str), or a bool
+        array / tensor of shape (n_text_layer, n_text_head)."""
+        shape = (self.dims.n_text_layer, self.dims.n_text_head)
+        if isinstance(dump, (bytes, str)):
+            import base64
+            import gzip
+            array = np.frombuffer(gzip.decompress(base64.b85decode(dump)), dtype=bool).copy()
+            if array.size != shape[0] * shape[1]:
+                raise ValueError(f"alignment-head dump has {array.size} entries, the model has {shape[0]} x {shape[1]} heads")
+            mask = torch.from_numpy(array).reshape(shape)
+        else:
+            mask = torch.as_tensor(dump)
+            if mask.is_sparse:
+                mask = mask.to_dense()
+            if mask.dtype != torch.bool or tuple(mask.shape) != shape:
+                raise ValueError(f"alignment heads must be a bool {shape} mask, got {mask.dtype} {tuple(mask.shape)}")
+            mask = mask.detach().cpu().clone()
+        if not bool(mask.any()):
+            raise ValueError("at least one alignment head is needed")
+        self._alignment_mask = mask
+
     def install_kv_cache_hooks(self, cache: Optional[dict] = None):
         """The reference's kv-cache protocol (model.py:925-964 / inf_model.py:422-453), kept for third-party loops
         (whisper.decoding.PyTorchInference) and for this package's sampling / timestamp-rule paths: forward hooks on every

@@ -292,3 +292,41 @@ def convert(src, dst=None, dtype=None):
     _req(dst.is_contiguous() and dst.numel() == src.numel(), "convert: dst must be contiguous with the same number of elements")
     call("oasr_convert", ptr(src), _DTYPE_CODE[src.dtype], ptr(dst), _DTYPE_CODE[dst.dtype], src.numel(), stream())
     return dst
+
+
+def align_cost(heads, n_frames, medfilt_width=7, out=None):
+    """DTW input of one window (include/oasr_b200.h oasr_align_cost): `heads` lists (q, k) per alignment head in
+    ascending (layer, head) order, q (n_tok, 64) and k (>= n_frames, 64) column slices (unit inner stride) of the
+    cross-attention query rows and cross keys, all bf16 or all fp16.  Returns cost (n_tok - 2, n_frames) fp32."""
+    _req(len(heads) >= 1, "align_cost: need at least one head")
+    q0, k0 = heads[0]
+    dt, dev, n_tok = q0.dtype, q0.device, q0.shape[0]
+    for q, k in heads:
+        _req(q.is_cuda and k.is_cuda and q.dtype == dt and k.dtype == dt and dt in ACT16,
+             "align_cost: q and k must be CUDA tensors of one 16-bit type")
+        _req(q.dim() == 2 and k.dim() == 2 and q.shape == (n_tok, 64) and k.shape[1] == 64 and k.shape[0] >= n_frames,
+             "align_cost: q (n_tok, 64) and k (>= n_frames, 64) per head")
+        _req(q.stride(1) == 1 and k.stride(1) == 1, "align_cost: unit inner stride")
+    table = torch.tensor([[q.data_ptr(), k.data_ptr(), q.stride(0), k.stride(0)] for q, k in heads],
+                         dtype=torch.int64).to(dev, non_blocking=True)
+    stats = torch.empty((len(heads), n_tok, 2), device=dev, dtype=torch.float32)
+    if out is None:
+        out = torch.empty((max(n_tok - 2, 0), n_frames), device=dev, dtype=torch.float32)
+    _req(out.dtype == torch.float32 and out.stride(1) == 1 and out.shape == (n_tok - 2, n_frames),
+         "align_cost: out (n_tok - 2, n_frames) fp32")
+    call("oasr_align_cost", ptr(table), len(heads), 64, n_tok, n_frames, medfilt_width, ptr(stats), ptr(out), out.stride(0),
+         _DTYPE_CODE[dt], stream())
+    return out
+
+
+def dtw(x):
+    """Dynamic time warping of x (rows, cols) fp32 with whisper's tie order (oasr_dtw).  Returns (path, length) on the
+    device: path (2, rows + cols) int32 whose first `length` columns are (text index, time index) in path order."""
+    _req(x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1, "dtw: 2-D fp32 CUDA matrix, unit inner stride")
+    rows, cols = x.shape
+    _req(rows >= 1 and cols >= 1, "dtw: empty matrix")
+    trace = torch.empty((rows + 1) * (cols + 1), device=x.device, dtype=torch.uint8)
+    path = torch.empty((2, rows + cols), device=x.device, dtype=torch.int32)
+    length = torch.empty(1, device=x.device, dtype=torch.int32)
+    call("oasr_dtw", ptr(x), x.stride(0), rows, cols, ptr(trace), ptr(path[0]), ptr(path[1]), ptr(length), stream())
+    return path, length

@@ -6,8 +6,14 @@ Caller of the hot path, kept so that `model.transcribe(...)` stays callable: GPU
 (:348-408).  As in the reference (transcribe.py:199-207), `beam_size` / `patience` apply at temperature 0 (beam search on
 the device decoder) and `best_of` at the fallback temperatures (best-of-n sampling), so the long-form eval options
 `without_timestamps=False, beam_size=5, best_of=5` (scripts/eval/eval.py:2077-2084) work as given.  Like the reference,
-previous-text prompt conditioning is disabled (transcribe.py:297-302).  Not implemented (raises): word_timestamps (needs
-alignment heads OLMoASR never sets, __init__.py:145).
+previous-text prompt conditioning is disabled (transcribe.py:297-302).
+
+`word_timestamps=True` adds upstream's per-word `"words": [{"word", "start", "end", "probability"}]` to every segment
+(transcribe.py:410-485; olmoasr_b200/timing.py): the model's `alignment_heads` (upstream's default, or
+`set_alignment_heads`) are aligned on the device against the window's encoded features, the seek moves to the last
+word's end, `hallucination_silence_threshold` skips silence around anomalous segments, and segments that are
+instantaneous or carry no text are cleared.  It needs `tokenizer=` to split words.  With the default False none of this
+runs and `hallucination_silence_threshold` is ignored, as upstream.
 
 Text needs a tokenizer: pass `tokenizer=` (object with `.decode(list[int]) -> str`); without one, segments carry token
 ids and empty text (the `gpt2.tiktoken` vocabulary cannot be fetched offline).
@@ -22,6 +28,7 @@ import torch
 
 from .audio import HOP_LENGTH, N_FRAMES, N_SAMPLES, SAMPLE_RATE, log_mel_spectrogram, pad_or_trim
 from .decoding import EOT, TIMESTAMP_BEGIN, DecodingOptions, DecodingResult, decode
+from .timing import add_word_timestamps, after_word_timestamps
 
 
 def _compression_ratio(result: DecodingResult) -> float:
@@ -37,8 +44,8 @@ def transcribe(model, audio: Union[str, np.ndarray, torch.Tensor], *, verbose: O
                prepend_punctuations: str = "\"'“¿([{-", append_punctuations: str = "\"'.。,，!！?？:：”)]}、",
                clip_timestamps: Union[str, List[float]] = "0", hallucination_silence_threshold: Optional[float] = None,
                tokenizer=None, **decode_options):
-    if word_timestamps:
-        raise NotImplementedError("word_timestamps needs alignment heads, which OLMoASR checkpoints do not define")
+    if word_timestamps and tokenizer is None:
+        raise ValueError("word_timestamps=True needs tokenizer= to split the text into words")
     decode_options.pop("fp16", None)
     decode_options.setdefault("language", "en")
     mel = log_mel_spectrogram(audio, model.dims.n_mels, padding=N_SAMPLES, device=model.device)
@@ -80,7 +87,9 @@ def transcribe(model, audio: Union[str, np.ndarray, torch.Tensor], *, verbose: O
     all_segments: List[dict] = []
     all_tokens: List[int] = []
     seek = 0
+    last_speech_timestamp = 0.0
     while seek < content_frames:
+        previous_seek = seek
         time_offset = seek * HOP_LENGTH / SAMPLE_RATE
         segment_size = min(N_FRAMES, content_frames - seek)
         segment_duration = segment_size * HOP_LENGTH / SAMPLE_RATE
@@ -117,6 +126,21 @@ def transcribe(model, audio: Union[str, np.ndarray, torch.Tensor], *, verbose: O
                 duration = (ts[-1] - TIMESTAMP_BEGIN) * time_precision
             current.append(new_segment(time_offset, time_offset + duration, tokens, result, seek))
             seek += segment_size
+        if word_timestamps:
+            add_word_timestamps(segments=current, model=model, tokenizer=tokenizer, mel=result.audio_features,
+                                num_frames=segment_size, prepend_punctuations=prepend_punctuations,
+                                append_punctuations=append_punctuations, last_speech_timestamp=last_speech_timestamp)
+            skip, seek, last_speech_timestamp = after_word_timestamps(
+                current, seek=seek, previous_seek=previous_seek, segment_size=segment_size,
+                single_timestamp_ending=single_ending, time_offset=time_offset,
+                window_end_time=(previous_seek + N_FRAMES) * HOP_LENGTH / SAMPLE_RATE, segment_duration=segment_duration,
+                content_frames=content_frames, content_duration=content_frames * HOP_LENGTH / SAMPLE_RATE,
+                last_speech_timestamp=last_speech_timestamp, hallucination_silence_threshold=hallucination_silence_threshold)
+            if skip:
+                continue
+            for seg in current:     # an instantaneous or text-free segment is cleared
+                if seg["start"] == seg["end"] or seg["text"].strip() == "":
+                    seg["text"], seg["tokens"], seg["words"] = "", [], []
         for i, seg in enumerate(current, start=len(all_segments)):
             seg["id"] = i
         all_segments.extend(current)

@@ -10,6 +10,10 @@
   inf_tiny.pt       olmoasr/inf_model.py: full-prefix logits sample and kv-cache step logits.
   ref_tiny_outputs.pt  the reference's train-model forward (tiny, seed 0) in fp32 and under CPU bf16 autocast: dense
                     logits samples and whole-tensor sums, what the oracle is compared with element for element.
+  timing_hf.npz     transformers' _dynamic_time_warping and _median_filter (independent restatements of upstream
+                    whisper/timing.py's dtw and median_filter) on seeded matrices.
+  ref_tiny_cross_qk.pt  the reference's inference model (tiny, seed 0, fp32) with forward hooks on every cross_attn
+                    reading outs[-1], as whisper.timing does: a sample of the raw cross-attention logits.
 """
 import sys
 from pathlib import Path
@@ -197,8 +201,62 @@ def golden_widths(depth=(2, 2)):
         print(f"model_{name}_{depth[0]}x{depth[1]}.pt loss", float(loss), "bf16 logits noise", float((lbf - l32).norm() / l32.norm()))
 
 
+DTW_SHAPES = ((1, 1), (3, 7), (40, 300), (225, 1500))
+MEDFILT_LENGTHS = (2, 3, 4, 750)
+
+
+def timing_inputs():
+    """The seeded DTW and median-filter inputs of timing_hf.npz (tests/test_timing_host.py regenerates them)."""
+    g = np.random.default_rng(11)
+    dtw = {f"dtw_{r}x{c}": g.standard_normal((r, c)).astype(np.float32) for r, c in DTW_SHAPES}
+    planted = g.uniform(0.0, 1.0, (60, 400)).astype(np.float32)
+    cols = np.sort(g.choice(400, 60, replace=False))
+    planted[np.arange(60), cols] = -5.0
+    dtw["dtw_planted"] = planted
+    med = {f"med_{n}": g.standard_normal((3, 5, n)).astype(np.float32) for n in MEDFILT_LENGTHS}
+    return dtw, med
+
+
+def golden_timing_hf():
+    from transformers.models.whisper.generation_whisper import _dynamic_time_warping, _median_filter
+
+    dtw, med = timing_inputs()
+    out = {}
+    for k, x in dtw.items():
+        ti, tj = _dynamic_time_warping(x)
+        out[k + "_text"], out[k + "_time"] = np.asarray(ti, np.int64), np.asarray(tj, np.int64)
+    for k, x in med.items():
+        out[k] = _median_filter(torch.from_numpy(x), 7).numpy()
+    np.savez_compressed(OUT / "timing_hf.npz", **out)
+    print("timing_hf.npz", sorted(out))
+
+
+def golden_cross_qk():
+    ref_model, ref_inf, ref_dims = ref_import.load()
+    dims = ref_dims.VARIANT_TO_DIMS["tiny"]
+    torch.manual_seed(0)
+    im = ref_inf.OLMoASR(dims)
+    sd = im.state_dict()
+    g = torch.Generator().manual_seed(7)
+    sd["decoder.positional_embedding"] = torch.randn(448, dims.n_text_state, generator=g) * 0.01
+    im.load_state_dict(sd)
+    mel = torch.from_numpy(logmel.log_mel_spectrogram(synth.waveforms(1).numpy()))
+    tokens = torch.cat([torch.tensor([50257, 50362]), torch.randint(0, 50256, (21,), generator=g), torch.tensor([50256])])
+    qks = [None] * dims.n_text_layer
+    hooks = [b.cross_attn.register_forward_hook(lambda _, ins, outs, index=i: qks.__setitem__(index, outs[-1][0]))
+             for i, b in enumerate(im.decoder.blocks)]
+    with torch.no_grad():
+        im(mel, tokens[None])
+    for h in hooks:
+        h.remove()
+    torch.save({"variant": "tiny", "seed": 0, "pos_seed": 7, "tokens": tokens,
+                "qk_sample": torch.stack(qks)[:, :, :, ::13].clone(), "frame_step": 13,
+                "torch_version": torch.__version__}, OUT / "ref_tiny_cross_qk.pt")
+    print("ref_tiny_cross_qk.pt", tuple(torch.stack(qks).shape))
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["logmel", "model", "ref_outputs", "grad_noise", "widths"]
+    which = sys.argv[1:] or ["logmel", "model", "ref_outputs", "grad_noise", "widths", "timing_hf", "cross_qk"]
     if "logmel" in which:
         golden_logmel()
     if "model" in which:
@@ -209,3 +267,7 @@ if __name__ == "__main__":
         golden_grad_noise()
     if "widths" in which:
         golden_widths()
+    if "timing_hf" in which:
+        golden_timing_hf()
+    if "cross_qk" in which:
+        golden_cross_qk()
