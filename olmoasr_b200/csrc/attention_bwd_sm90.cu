@@ -4,9 +4,19 @@
 // (encoder self, decoder causal+length self, cross).  Given Q, K, V, O, dO and the forward's log2-domain
 // LSE it produces dQ, dK, dV without ever materialising the (Tq x Tkv) score matrix in HBM.
 //
-// One CTA per (128-key tile, head, sample), 256 threads = two warpgroups of 64 keys each, looping over the 64-query
-// tiles that can see the keys (Q / dO tiles stream through a two-stage TMA ring shared by both warpgroups).  Everything
-// is computed transposed, with the warpgroup's keys as the MMA rows, so that dK and dV stay in registers for the loop:
+// Both kernels below run two warpgroups (256 threads) and stream their operands through a three-stage TMA ring whose
+// stages carry a full and an empty mbarrier: each warpgroup releases a stage by arriving on its empty barrier, and
+// thread 0 refills it one step later, once both have (no CTA-wide barrier in the loop, so the two warpgroups drift
+// apart and cover each other's non-MMA work).  They keep 256 threads rather than adding a producer warpgroup because
+// their loops need more than the 168 registers per thread that a 384-thread launch allows (ptxas allocates the whole
+// kernel under that cap; a setmaxnreg hand-over does not lift it).  Each warpgroup's loop is software-pipelined one
+// step deep: the S / dP MMAs of step i + 1 are issued together with the accumulating MMAs of step i, and the exp2 / dS
+// math of step i + 1 runs (in place, in fp32) while those are on the tensor cores.  Tile sizes, k16 order, masks and
+// exp2 are those of an unpipelined loop, so the results are bit-for-bit the same.
+//
+// dK / dV: one CTA per (128-key tile, head, sample), each warpgroup owning 64 keys, looping over the 64-query
+// tiles that can see the keys (Q and dO stream through a three-stage ring).  Everything is computed
+// transposed, with the warpgroup's keys as the MMA rows, so that dK and dV stay in registers for the loop:
 //     S^T  = K Q^T         dP^T = V dO^T                 wgmma m64n64k16, all operands from swizzled smem
 //     P^T  = exp2(S^T c - LSE)   dS^T = P^T o (dP^T - D) thread-local: LSE / D are per query = per column
 //     dV  += P^T dO        dK  += dS^T Q                 P^T / dS^T as register A operands, dO / Q MN-major
@@ -19,16 +29,19 @@
 
 #include <stdlib.h>
 
+#include <type_traits>
+
 namespace oasr {
 namespace {
 
 constexpr int HD = 64;
 constexpr int BQ = 64;                     // queries per loop iteration
 constexpr int BKV = 128;                   // keys per CTA (64 per warpgroup)
+constexpr int STAGES = 3;                  // both rings: step i + 1 is waited on while step i - 1's stage refills
 constexpr int KV_BYTES = BKV * HD * 2;     // 16 KB
 constexpr int QT_BYTES = BQ * HD * 2;      // 8 KB
-// K, V | (Q, dO) x 2 stages
-constexpr int BWD_TILES = 2 * KV_BYTES + 2 * 2 * QT_BYTES;   // 64 KB
+// K, V | (Q, dO) per stage
+constexpr int BWD_TILES = 2 * KV_BYTES + STAGES * 2 * QT_BYTES;   // 80 KB
 constexpr int BWD_SMEM = BWD_TILES + 1024 /*barriers*/ + 1024 /*alignment slack*/;
 constexpr int BWD_THREADS = 256;
 
@@ -53,15 +66,50 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   uint8_t* smem_raw = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + BWD_TILES);
   uint64_t& bar_kv = bars[0];
-  uint64_t* bar_q = bars + 1;   // [2]: Q and dO of a query tile landed in stage s (parity: (it / 2) & 1)
+  uint64_t* bar_full = bars + 1;             // [STAGES]: Q and dO of query step it landed in stage it % STAGES
+  uint64_t* bar_empty = bar_full + STAGES;   // [STAGES]: both warpgroups are done with the stage
 
   const uint32_t sK = ptx::smem_u32(smem_raw), sV = sK + KV_BYTES;
-  const uint32_t sQ0 = sV + KV_BYTES;          // stage s: Q at sQ0 + s*16K, dO right after Q
+  const uint32_t sQ0 = sV + KV_BYTES;                        // stage s: Q at sQ0 + s*16K, dO right after Q
   const int kv_tile = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int kv0 = kv_tile * BKV;
   int kv_valid = p.Tkv;
   if (p.kv_len) kv_valid = min(kv_valid, max(1, p.kv_len[b]));
-  const int wg = threadIdx.x >> 7;
+
+  const int n_q_tiles = (p.Tq + BQ - 1) / BQ;
+  const int i_begin = p.causal ? kv0 / BQ : 0;                 // earlier queries cannot see these keys
+  const int n_iter = (kv0 < kv_valid) ? n_q_tiles - i_begin : 0;   // fully masked key tile: zero gradients
+
+  if (threadIdx.x == 0) {
+    ptx::tma_prefetch_desc(&tmQ); ptx::tma_prefetch_desc(&tmK); ptx::tma_prefetch_desc(&tmV); ptx::tma_prefetch_desc(&tmdO);
+    ptx::mbar_init(ptx::smem_u32(&bar_kv), 1);
+    for (int s = 0; s < STAGES; ++s) {
+      ptx::mbar_init(ptx::smem_u32(&bar_full[s]), 1);
+      ptx::mbar_init(ptx::smem_u32(&bar_empty[s]), 2);   // one arrival per consumer warpgroup
+    }
+    ptx::fence_barrier_init();
+  }
+  __syncthreads();
+
+  // thread 0 only: Q and dO of query step it into stage it % STAGES, once both warpgroups have released it
+  auto load_q = [&](int it) {
+    const int st = it % STAGES;
+    ptx::mbar_wait(ptx::smem_u32(&bar_empty[st]), ((it / STAGES) & 1) ^ 1);
+    const uint32_t full = ptx::smem_u32(&bar_full[st]);
+    const uint32_t dst = sQ0 + st * 2 * QT_BYTES;
+    const int q0 = (i_begin + it) * BQ;
+    ptx::mbar_arrive_expect_tx(full, 2 * QT_BYTES);
+    ptx::tma_load_2d(dst, &tmQ, full, h * HD, b * p.Tq + q0);
+    ptx::tma_load_2d(dst + QT_BYTES, &tmdO, full, h * HD, b * p.Tq + q0);
+  };
+  if (threadIdx.x == 0 && n_iter > 0) {
+    ptx::mbar_arrive_expect_tx(ptx::smem_u32(&bar_kv), 2 * KV_BYTES);
+    ptx::tma_load_2d(sK, &tmK, ptx::smem_u32(&bar_kv), h * HD, b * p.Tkv + kv0);
+    ptx::tma_load_2d(sV, &tmV, ptx::smem_u32(&bar_kv), h * HD, b * p.Tkv + kv0);
+    for (int it = 0; it < min(STAGES, n_iter); ++it) load_q(it);
+  }
+
+  const int wg = threadIdx.x >> 7;   // key half of the tile
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31;
   const int key_loc = wg * 64 + warp * 16 + (lane >> 2);   // keys key_loc and key_loc + 8 of the tile (fragment rows)
@@ -71,33 +119,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 #pragma unroll
   for (int i = 0; i < 32; ++i) { dk[i] = 0.f; dv[i] = 0.f; }
 
-  const int n_q_tiles = (p.Tq + BQ - 1) / BQ;
-  const int i_begin = p.causal ? kv0 / BQ : 0;                 // earlier queries cannot see these keys
-  const int n_iter = (kv0 < kv_valid) ? n_q_tiles - i_begin : 0;   // fully masked key tile: zero gradients
-
   if (n_iter > 0) {
-    if (threadIdx.x == 0) {
-      ptx::tma_prefetch_desc(&tmQ); ptx::tma_prefetch_desc(&tmK); ptx::tma_prefetch_desc(&tmV); ptx::tma_prefetch_desc(&tmdO);
-      ptx::mbar_init(ptx::smem_u32(&bar_kv), 1);
-      ptx::mbar_init(ptx::smem_u32(&bar_q[0]), 1);
-      ptx::mbar_init(ptx::smem_u32(&bar_q[1]), 1);
-      ptx::fence_barrier_init();
-    }
-    __syncthreads();
-    auto load_q = [&](int it) {   // thread 0 only
-      const uint32_t full = ptx::smem_u32(&bar_q[it & 1]);
-      const uint32_t dst = sQ0 + (it & 1) * 2 * QT_BYTES;
-      const int qrow = b * p.Tq + (i_begin + it) * BQ;
-      ptx::mbar_arrive_expect_tx(full, 2 * QT_BYTES);
-      ptx::tma_load_2d(dst, &tmQ, full, h * HD, qrow);
-      ptx::tma_load_2d(dst + QT_BYTES, &tmdO, full, h * HD, qrow);
-    };
-    if (threadIdx.x == 0) {
-      ptx::mbar_arrive_expect_tx(ptx::smem_u32(&bar_kv), 2 * KV_BYTES);
-      ptx::tma_load_2d(sK, &tmK, ptx::smem_u32(&bar_kv), h * HD, b * p.Tkv + kv0);
-      ptx::tma_load_2d(sV, &tmV, ptx::smem_u32(&bar_kv), h * HD, b * p.Tkv + kv0);
-      load_q(0);
-    }
     const float c = p.scale_log2;
     const uint64_t k_desc = ptx::desc_sw128(sK + wg * 8192, 16, 1024);       // A of S^T (K-major)
     const uint64_t v_desc = ptx::desc_sw128(sV + wg * 8192, 16, 1024);       // A of dP^T (K-major)
@@ -106,26 +128,12 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     for (int hh = 0; hh < 2; ++hh) key_abs[hh] = kv0 + key_loc + 8 * hh;   // absolute key index of the row
     ptx::mbar_wait(ptx::smem_u32(&bar_kv), 0);
 
-    for (int it = 0; it < n_iter; ++it) {
-      if (threadIdx.x == 0 && it + 1 < n_iter) load_q(it + 1);   // its stage was released by the __syncthreads of it - 1
-      ptx::mbar_wait(ptx::smem_u32(&bar_q[it & 1]), (it >> 1) & 1);
-      const uint32_t sQ = sQ0 + (it & 1) * 2 * QT_BYTES, sdO = sQ + QT_BYTES;
-      const int q0 = (i_begin + it) * BQ;
-
-      // lse / delta of this thread's 16 query columns (issued before the MMAs so the loads overlap them)
-      float lse_c[16], dlt_c[16];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int qn = q0 + 8 * i + qc + e;
-          const int64_t at = (static_cast<int64_t>(b) * p.H + h) * p.Tq + qn;
-          lse_c[2 * i + e] = qn < p.Tq ? __ldg(p.lse + at) : 0.f;
-          dlt_c[2 * i + e] = qn < p.Tq ? __ldg(p.delta + at) : 0.f;
-        }
-      }
-
-      float s[32], dp[32];
+    float s[32], dp[32];
+    // S^T, dP^T of query step it into s, dp (one commit group)
+    auto issue_sdp = [&](int it) {
+      const int st = it % STAGES;
+      ptx::mbar_wait(ptx::smem_u32(&bar_full[st]), (it / STAGES) & 1);
+      const uint32_t sQ = sQ0 + st * 2 * QT_BYTES, sdO = sQ + QT_BYTES;
       const uint64_t q_desc = ptx::desc_sw128(sQ, 16, 1024), do_desc = ptx::desc_sw128(sdO, 16, 1024);
       ptx::wgmma_fence();
 #pragma unroll
@@ -133,31 +141,60 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 #pragma unroll
       for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n64k16_ss<0, 0, T>(dp, ptx::desc_add(v_desc, 32 * k), ptx::desc_add(do_desc, 32 * k), k > 0);
       ptx::wgmma_commit();
-      ptx::wgmma_wait<0>();
-      ptx::fence_regs(s);
-      ptx::fence_regs(dp);
-
-      // P^T, dS^T; packed to T in the A-fragment order (k = queries)
-      uint32_t pa[4][4], da[4][4];
+    };
+    // s <- P^T, dp <- dS^T of query step it
+    auto grads = [&](int it) {
+      const int q0 = (i_begin + it) * BQ;
+      // every (key, query) pair of this thread visible: no per-element test (the common case away from the edges)
+      const bool all_vis = q0 + BQ <= p.Tq && key_abs[1] < kv_valid && (!p.causal || key_abs[1] <= q0);
+      auto run = [&](auto masked) {
+        // lse / delta of this thread's 16 query columns
+        float lse_c[16], dlt_c[16];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          float pe[2], ds[2];
+        for (int i = 0; i < 8; ++i) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int qn = q0 + 8 * i + qc + e;
-            const int key = key_abs[hh];
-            const bool vis = qn < p.Tq && key < kv_valid && (!p.causal || key <= qn);
-            const int x = 4 * i + 2 * hh + e;
-            pe[e] = vis ? fast_exp2(fmaf(s[x], c, -lse_c[2 * i + e])) : 0.f;
-            ds[e] = pe[e] * (dp[x] - dlt_c[2 * i + e]);
+            const int64_t at = (static_cast<int64_t>(b) * p.H + h) * p.Tq + qn;
+            lse_c[2 * i + e] = (!masked || qn < p.Tq) ? __ldg(p.lse + at) : 0.f;
+            dlt_c[2 * i + e] = (!masked || qn < p.Tq) ? __ldg(p.delta + at) : 0.f;
           }
-          pa[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(pe[0], pe[1]);
-          da[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(ds[0], ds[1]);
         }
-      }
-
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int qn = q0 + 8 * i + qc + e;
+              const int key = key_abs[hh];
+              const bool vis = !masked || (qn < p.Tq && key < kv_valid && (!p.causal || key <= qn));
+              const int x = 4 * i + 2 * hh + e;
+              const float pe = vis ? fast_exp2(fmaf(s[x], c, -lse_c[2 * i + e])) : 0.f;
+              dp[x] = pe * (dp[x] - dlt_c[2 * i + e]);
+              s[x] = pe;
+            }
+          }
+        }
+      };
+      if (all_vis) run(std::false_type{});
+      else run(std::true_type{});
+    };
+    // P^T, dS^T packed to T in the A-fragment order (k = queries)
+    uint32_t pa[4][4], da[4][4];
+    auto pack = [&]() {
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int x = 4 * i + 2 * hh;
+          pa[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(s[x], s[x + 1]);
+          da[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(dp[x], dp[x + 1]);
+        }
+    };
+    // dV += P^T dO, dK += dS^T Q of query step it (one commit group)
+    auto issue_dkdv = [&](int it) {
+      const uint32_t sQ = sQ0 + (it % STAGES) * 2 * QT_BYTES, sdO = sQ + QT_BYTES;
       const uint64_t qB_desc = ptx::desc_sw128(sQ, 8192, 1024), doB_desc = ptx::desc_sw128(sdO, 8192, 1024);
       ptx::wgmma_fence();
 #pragma unroll
@@ -166,11 +203,33 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         ptx::wgmma_m64n64k16_rs<1, T>(dk, da[kk], ptx::desc_add(qB_desc, 2048 * kk), 1u);
       }
       ptx::wgmma_commit();
+    };
+    auto retire_dkdv = [&](int it) {
       ptx::wgmma_wait<0>();
       ptx::fence_regs(dv);
       ptx::fence_regs(dk);
-      __syncthreads();   // both warpgroups are done with this Q / dO stage
+      if (t == 0) ptx::mbar_arrive(ptx::smem_u32(&bar_empty[it % STAGES]));   // this Q / dO stage is free
+    };
+
+    issue_sdp(0);
+    ptx::wgmma_wait<0>();
+    ptx::fence_regs(s);
+    ptx::fence_regs(dp);
+    grads(0);
+    pack();
+    for (int it = 0; it + 1 < n_iter; ++it) {
+      issue_sdp(it + 1);
+      issue_dkdv(it);
+      if (threadIdx.x == 0 && it >= 1 && it - 1 + STAGES < n_iter) load_q(it - 1 + STAGES);   // released in step it - 1
+      ptx::wgmma_wait<1>();   // S^T / dP^T of it + 1 are in; the dK / dV MMAs of it may still be running
+      ptx::fence_regs(s);
+      ptx::fence_regs(dp);
+      grads(it + 1);
+      retire_dkdv(it);
+      pack();
     }
+    issue_dkdv(n_iter - 1);
+    retire_dkdv(n_iter - 1);
   }
 
   // ---- dK (scaled), dV: key rows past Tkv are not written
@@ -189,11 +248,11 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   }
 }
 
-// dQ for one (128-query tile, head, sample): two warpgroups of 64 query rows; K / V tiles of 128 keys stream through a
-// two-stage TMA ring shared by both (the load of tile j+1 is in flight while tile j is computed), as in the forward.
+// dQ for one (128-query tile, head, sample): each warpgroup owns 64 query rows; K / V tiles of 128 keys stream
+// through a three-stage ring as in the forward.
 constexpr int DQ_BQ = 128, DQ_BKV = 128;
-constexpr int DQ_TILE = 128 * HD * 2;                            // 16 KB
-constexpr int DQ_TILES = 2 * DQ_TILE /*Q, dO*/ + 2 * 2 * DQ_TILE /*K, V x 2 stages*/;   // 96 KB
+constexpr int DQ_TILE = 128 * HD * 2;                                      // 16 KB
+constexpr int DQ_TILES = 2 * DQ_TILE /*Q, dO*/ + STAGES * 2 * DQ_TILE /*K, V per stage*/;   // 128 KB
 constexpr int DQ_SMEM = DQ_TILES + 1024 /*barriers*/ + 1024 /*alignment slack*/;
 
 template <typename T>
@@ -203,8 +262,9 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
   extern __shared__ uint8_t smem_dyn[];
   uint8_t* smem_raw = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + DQ_TILES);
-  uint64_t& bar_q = bars[0];     // Q and dO landed
-  uint64_t* bar_kv = bars + 1;   // [2]: K and V of key tile j landed in stage j & 1 (parity: (j / 2) & 1)
+  uint64_t& bar_q = bars[0];                 // Q and dO landed
+  uint64_t* bar_full = bars + 1;             // [STAGES]: K and V of key tile j landed in stage j % STAGES
+  uint64_t* bar_empty = bar_full + STAGES;   // [STAGES]: both warpgroups are done with the stage
 
   const uint32_t sQ = ptx::smem_u32(smem_raw), sdO = sQ + DQ_TILE;
   const uint32_t sKV = sdO + DQ_TILE;   // stage s: K at sKV + s*32K, V right after K
@@ -218,14 +278,20 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
   if (threadIdx.x == 0) {
     ptx::tma_prefetch_desc(&tmQ); ptx::tma_prefetch_desc(&tmK); ptx::tma_prefetch_desc(&tmV); ptx::tma_prefetch_desc(&tmdO);
     ptx::mbar_init(ptx::smem_u32(&bar_q), 1);
-    ptx::mbar_init(ptx::smem_u32(&bar_kv[0]), 1);
-    ptx::mbar_init(ptx::smem_u32(&bar_kv[1]), 1);
+    for (int s = 0; s < STAGES; ++s) {
+      ptx::mbar_init(ptx::smem_u32(&bar_full[s]), 1);
+      ptx::mbar_init(ptx::smem_u32(&bar_empty[s]), 2);   // one arrival per consumer warpgroup
+    }
     ptx::fence_barrier_init();
   }
   __syncthreads();
-  auto load_kv = [&](int j) {   // thread 0 only
-    const uint32_t full = ptx::smem_u32(&bar_kv[j & 1]);
-    const uint32_t dst = sKV + (j & 1) * 2 * DQ_TILE;
+
+  // thread 0 only: K and V of key tile j into stage j % STAGES, once both warpgroups have released it
+  auto load_kv = [&](int j) {
+    const int st = j % STAGES;
+    ptx::mbar_wait(ptx::smem_u32(&bar_empty[st]), ((j / STAGES) & 1) ^ 1);
+    const uint32_t full = ptx::smem_u32(&bar_full[st]);
+    const uint32_t dst = sKV + st * 2 * DQ_TILE;
     ptx::mbar_arrive_expect_tx(full, 2 * DQ_TILE);
     ptx::tma_load_2d(dst, &tmK, full, h * HD, b * p.Tkv + j * DQ_BKV);
     ptx::tma_load_2d(dst + DQ_TILE, &tmV, full, h * HD, b * p.Tkv + j * DQ_BKV);
@@ -234,10 +300,10 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
     ptx::mbar_arrive_expect_tx(ptx::smem_u32(&bar_q), 2 * DQ_TILE);
     ptx::tma_load_2d(sQ, &tmQ, ptx::smem_u32(&bar_q), h * HD, b * p.Tq + q_base);
     ptx::tma_load_2d(sdO, &tmdO, ptx::smem_u32(&bar_q), h * HD, b * p.Tq + q_base);
-    load_kv(0);
+    for (int j = 0; j < min(STAGES, n_kv); ++j) load_kv(j);
   }
 
-  const int wg = threadIdx.x >> 7;
+  const int wg = threadIdx.x >> 7;   // query-row half of the tile
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31;
   const int r_loc = wg * 64 + warp * 16 + (lane >> 2);   // rows r_loc and r_loc + 8 of the query tile
@@ -259,14 +325,12 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
   float dq[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) dq[i] = 0.f;
-  ptx::mbar_wait(ptx::smem_u32(&bar_q), 0);
-
-  for (int j = 0; j < n_kv; ++j) {
-    if (threadIdx.x == 0 && j + 1 < n_kv) load_kv(j + 1);   // its stage was released by the __syncthreads of j - 1
-    ptx::mbar_wait(ptx::smem_u32(&bar_kv[j & 1]), (j >> 1) & 1);
-    const uint32_t sK = sKV + (j & 1) * 2 * DQ_TILE, sV = sK + DQ_TILE;
-
-    float s[64], dp[64];
+  float s[64], dp[64];
+  // S = Q K_j^T, dP = dO V_j^T into s, dp (one commit group)
+  auto issue_sdp = [&](int j) {
+    const int st = j % STAGES;
+    ptx::mbar_wait(ptx::smem_u32(&bar_full[st]), (j / STAGES) & 1);
+    const uint32_t sK = sKV + st * 2 * DQ_TILE, sV = sK + DQ_TILE;
     const uint64_t k_desc = ptx::desc_sw128(sK, 16, 1024), v_desc = ptx::desc_sw128(sV, 16, 1024);
     ptx::wgmma_fence();
 #pragma unroll
@@ -274,40 +338,78 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
 #pragma unroll
     for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n128k16_ss<0, 0, T>(dp, ptx::desc_add(do_desc, 32 * k), ptx::desc_add(v_desc, 32 * k), k > 0);
     ptx::wgmma_commit();
-    ptx::wgmma_wait<0>();
-    ptx::fence_regs(s);
-    ptx::fence_regs(dp);
-
-    // dS = P o (dP - D), P = 2^(S c - LSE) on the visible keys [0, limit); packed to T in the A-fragment order (k = keys)
+  };
+  // dp <- dS = P o (dP - D), P = 2^(S c - LSE) on the visible keys [0, limit) of key tile j
+  auto grads = [&](int j) {
     const int k0 = j * DQ_BKV;
-    uint32_t da[8][4];
+    int limit[2];
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int qi = q_base + r_loc + 8 * hh;
-      int limit = kv_valid - k0;
-      if (p.causal) limit = min(limit, qi - k0 + 1);
-      if (!q_ok[hh]) limit = 0;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        float ds[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int x = 4 * i + 2 * hh + e;
-          const float pe = (8 * i + kc + e < limit) ? fast_exp2(fmaf(s[x], c, -lse_r[hh])) : 0.f;
-          ds[e] = pe * (dp[x] - dlt_r[hh]);
-        }
-        da[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(ds[0], ds[1]);
-      }
+      limit[hh] = kv_valid - k0;
+      if (p.causal) limit[hh] = min(limit[hh], qi - k0 + 1);
+      if (!q_ok[hh]) limit[hh] = 0;
     }
-    const uint64_t kB_desc = ptx::desc_sw128(sK, DQ_BKV * 128, 1024);   // K as the MN-major B operand (keys are k)
+    // every key of the tile visible to both of this thread's rows: no per-element test
+    auto run = [&](auto masked) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int x = 4 * i + 2 * hh + e;
+            const float pe = (!masked || 8 * i + kc + e < limit[hh]) ? fast_exp2(fmaf(s[x], c, -lse_r[hh])) : 0.f;
+            dp[x] = pe * (dp[x] - dlt_r[hh]);
+          }
+        }
+      }
+    };
+    if (min(limit[0], limit[1]) >= DQ_BKV) run(std::false_type{});
+    else run(std::true_type{});
+  };
+  // dS packed to T in the A-fragment order (k = keys)
+  uint32_t da[8][4];
+  auto pack = [&]() {
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) da[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(dp[4 * i + 2 * hh], dp[4 * i + 2 * hh + 1]);
+  };
+  // dQ += dS K_j (one commit group); K as the MN-major B operand (keys are k)
+  auto issue_dq = [&](int j) {
+    const uint64_t kB_desc = ptx::desc_sw128(sKV + (j % STAGES) * 2 * DQ_TILE, DQ_BKV * 128, 1024);
     ptx::wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < DQ_BKV / 16; ++kk) ptx::wgmma_m64n64k16_rs<1, T>(dq, da[kk], ptx::desc_add(kB_desc, 2048 * kk), 1u);
     ptx::wgmma_commit();
+  };
+  auto retire_dq = [&](int j) {
     ptx::wgmma_wait<0>();
     ptx::fence_regs(dq);
-    __syncthreads();   // both warpgroups are done with this stage: it may be refilled
+    if (t == 0) ptx::mbar_arrive(ptx::smem_u32(&bar_empty[j % STAGES]));   // K_j and V_j are no longer read
+  };
+
+  ptx::mbar_wait(ptx::smem_u32(&bar_q), 0);
+  issue_sdp(0);
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(s);
+  ptx::fence_regs(dp);
+  grads(0);
+  pack();
+  for (int j = 0; j + 1 < n_kv; ++j) {
+    issue_sdp(j + 1);
+    issue_dq(j);
+    if (threadIdx.x == 0 && j >= 1 && j - 1 + STAGES < n_kv) load_kv(j - 1 + STAGES);   // released in step j - 1
+    ptx::wgmma_wait<1>();   // S / dP of tile j + 1 are in; dQ += dS_j K_j may still be running
+    ptx::fence_regs(s);
+    ptx::fence_regs(dp);
+    grads(j + 1);
+    retire_dq(j);
+    pack();
   }
+  issue_dq(n_kv - 1);
+  retire_dq(n_kv - 1);
 
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {

@@ -6,14 +6,18 @@
 //   encoder self-attention (no mask), decoder self-attention (causal + per-sample key length, derived
 //   from the dense additive mask the reference passes, model.py:740-743) and cross-attention (no mask).
 //
-// One CTA per (128-query tile, head, sample), 256 threads = two warpgroups of 64 query rows each.  K / V tiles of 128
-// keys stream through a two-stage TMA ring shared by both warpgroups (the load of tile j+1 is in flight while tile j is
-// computed).  Per key tile a warpgroup runs
+// One CTA per (128-query tile, head, sample), 384 threads = three warpgroups.  In warpgroup 0 one thread is the TMA
+// producer: it loads Q and streams the K / V tiles of 128 keys through a three-stage ring (full / empty mbarrier per
+// stage; no CTA-wide barrier in the loop).  Warpgroups 1 and 2 consume, 64 query rows each.  There is no setmaxnreg
+// hand-over: ptxas allocates the whole kernel under the 168-register cap of a 384-thread launch, the consumers fit in
+// it, and a producer cut below what ptxas gave it would lose live registers.  Per key tile a consumer runs
 //     S = Q K^T          4 x wgmma m64n128k16, Q and K from 128B-swizzled smem, fp32 S in registers
 //     online softmax     thread owns rows lane/4 and lane/4 + 8 of its warp's 16: row max / sum over the 4-lane quad
-//     O += P V           8 x wgmma m64n64k16 with P as the register A operand (the S fragment re-packed to bf16) and
+//     O += P V           8 x wgmma m64n64k16 with P as the register A operand (the S fragment re-packed to 16 bits) and
 //                        V MN-major from its TMA tile
-// and the output leaves straight from the O fragment.
+// software-pipelined one tile deep: S_{j+1} and O += P_j V_j are issued together and the exponentials of tile j + 1 run
+// (in place, in fp32) while P_j V_j is still on the tensor cores; P_{j+1} is packed to 16 bits once P_j V_j retires.  The arithmetic (tile sizes, k16 order, masks, exp2) is that of the
+// unpipelined loop, so the results are bit-for-bit the same.  The output leaves straight from the O fragment.
 #include "common.cuh"
 #include "ptx_sm90.cuh"
 
@@ -23,12 +27,13 @@ namespace oasr {
 namespace {
 
 constexpr int HD = 64;
-constexpr int BQ = 128;                      // query rows per CTA (64 per warpgroup)
+constexpr int BQ = 128;                      // query rows per CTA (64 per consumer warpgroup)
 constexpr int BKV = 128;
-constexpr int TILE_BYTES = 128 * HD * 2;     // 16 KB: a [128 rows][64 bf16] swizzled tile
-constexpr int ATT_TILES = TILE_BYTES /*Q*/ + 2 * 2 * TILE_BYTES /*K,V x 2 stages*/;   // 80 KB
+constexpr int STAGES = 3;                    // K/V ring: tile j + 1 is waited on while tile j - 1's stage refills
+constexpr int TILE_BYTES = 128 * HD * 2;     // 16 KB: a [128 rows][64 16-bit] swizzled tile
+constexpr int ATT_TILES = TILE_BYTES /*Q*/ + STAGES * 2 * TILE_BYTES /*K,V per stage*/;   // 112 KB
 constexpr int ATT_SMEM = ATT_TILES + 1024 /*barriers*/ + 1024 /*alignment slack*/;
-constexpr int THREADS = 256;
+constexpr int THREADS = 384;
 
 struct AttnParams {
   void* o;
@@ -57,7 +62,8 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   uint8_t* smem_raw = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + ATT_TILES);
   uint64_t& bar_q = bars[0];
-  uint64_t* bar_kv = bars + 1;   // [2]: K and V of a key tile landed in stage s (parity: (j / 2) & 1)
+  uint64_t* bar_full = bars + 1;             // [STAGES]: K and V of key tile j landed in stage j % STAGES
+  uint64_t* bar_empty = bar_full + STAGES;   // [STAGES]: both consumers are done with the stage
 
   const uint32_t sQ = ptx::smem_u32(smem_raw);
   const uint32_t sKV = sQ + TILE_BYTES;   // stage s: K at sKV + s*32K, V right after K
@@ -71,28 +77,38 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   if (threadIdx.x == 0) {
     ptx::tma_prefetch_desc(&tmQ); ptx::tma_prefetch_desc(&tmK); ptx::tma_prefetch_desc(&tmV);
     ptx::mbar_init(ptx::smem_u32(&bar_q), 1);
-    ptx::mbar_init(ptx::smem_u32(&bar_kv[0]), 1);
-    ptx::mbar_init(ptx::smem_u32(&bar_kv[1]), 1);
+    for (int s = 0; s < STAGES; ++s) {
+      ptx::mbar_init(ptx::smem_u32(&bar_full[s]), 1);
+      ptx::mbar_init(ptx::smem_u32(&bar_empty[s]), 2);   // one arrival per consumer warpgroup
+    }
     ptx::fence_barrier_init();
   }
   __syncthreads();
-  auto load_kv = [&](int j) {   // thread 0 only
-    const uint32_t full = ptx::smem_u32(&bar_kv[j & 1]);
-    const uint32_t dst = sKV + (j & 1) * 2 * TILE_BYTES;
-    ptx::mbar_arrive_expect_tx(full, 2 * TILE_BYTES);
-    ptx::tma_load_2d(dst, &tmK, full, h * HD, b * p.Tkv + j * BKV);
-    ptx::tma_load_2d(dst + TILE_BYTES, &tmV, full, h * HD, b * p.Tkv + j * BKV);
-  };
-  if (threadIdx.x == 0) {
-    ptx::mbar_arrive_expect_tx(ptx::smem_u32(&bar_q), TILE_BYTES);
-    ptx::tma_load_2d(sQ, &tmQ, ptx::smem_u32(&bar_q), h * HD, b * p.Tq + q_base);
-    load_kv(0);
+
+  if (threadIdx.x < 128) {
+    // ===================== TMA producer =====================
+    if (threadIdx.x == 0) {
+      ptx::mbar_arrive_expect_tx(ptx::smem_u32(&bar_q), TILE_BYTES);
+      ptx::tma_load_2d(sQ, &tmQ, ptx::smem_u32(&bar_q), h * HD, b * p.Tq + q_base);
+      for (int j = 0; j < n_kv; ++j) {
+        const int st = j % STAGES;
+        ptx::mbar_wait(ptx::smem_u32(&bar_empty[st]), ((j / STAGES) & 1) ^ 1);
+        const uint32_t full = ptx::smem_u32(&bar_full[st]);
+        const uint32_t dst = sKV + st * 2 * TILE_BYTES;
+        ptx::mbar_arrive_expect_tx(full, 2 * TILE_BYTES);
+        ptx::tma_load_2d(dst, &tmK, full, h * HD, b * p.Tkv + j * BKV);
+        ptx::tma_load_2d(dst + TILE_BYTES, &tmV, full, h * HD, b * p.Tkv + j * BKV);
+      }
+    }
+    return;
   }
 
-  const int wg = threadIdx.x >> 7;
+  // ===================== consumers =====================
+  const int wg = (threadIdx.x >> 7) - 1;   // query-row half of the tile
   const int t = threadIdx.x & 127;
   const int warp = t >> 5, lane = t & 31;
   const int r_loc = wg * 64 + warp * 16 + (lane >> 2);   // rows r_loc and r_loc + 8 of the CTA's query tile
+  const int kc = 2 * (lane & 3);
   const float c = p.scale_log2;
   const uint64_t q_desc = ptx::desc_sw128(sQ + wg * 8192, 16, 1024);
 
@@ -100,25 +116,22 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // l: this thread's share of the row sum
-  ptx::mbar_wait(ptx::smem_u32(&bar_q), 0);
+  float s[64];
 
-  for (int j = 0; j < n_kv; ++j) {
-    if (threadIdx.x == 0 && j + 1 < n_kv) load_kv(j + 1);   // its stage was released by the __syncthreads of j - 1
-    ptx::mbar_wait(ptx::smem_u32(&bar_kv[j & 1]), (j >> 1) & 1);
-    const uint32_t sK = sKV + (j & 1) * 2 * TILE_BYTES, sV = sK + TILE_BYTES;
-
-    float s[64];
-    const uint64_t k_desc = ptx::desc_sw128(sK, 16, 1024);
+  // S = Q K_j^T into s (one commit group)
+  auto issue_s = [&](int j) {
+    const int st = j % STAGES;
+    ptx::mbar_wait(ptx::smem_u32(&bar_full[st]), (j / STAGES) & 1);
+    const uint64_t k_desc = ptx::desc_sw128(sKV + st * 2 * TILE_BYTES, 16, 1024);
     ptx::wgmma_fence();
 #pragma unroll
     for (int k = 0; k < HD / 16; ++k) ptx::wgmma_m64n128k16_ss<0, 0, T>(s, ptx::desc_add(q_desc, 32 * k), ptx::desc_add(k_desc, 32 * k), k > 0);
     ptx::wgmma_commit();
-    ptx::wgmma_wait<0>();
-    ptx::fence_regs(s);
-
+  };
+  // masks tile j of s, updates m / l and overwrites s with p = 2^(s c - m c)
+  auto softmax = [&](int j, float (&alpha)[2]) {
     // mask: keys [0, limit) of this tile are visible to a row
     const int k0 = j * BKV;
-    const int kc = 2 * (lane & 3);
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int qi = q_base + r_loc + 8 * hh;
@@ -132,7 +145,7 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         }
       }
     }
-    float alpha[2], neg[2];
+    float neg[2];
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       float mx = -INFINITY;
@@ -145,8 +158,6 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       m[hh] = m_new;
       l[hh] *= alpha[hh];
     }
-    // p = 2^(s c - m c); P packed to T in the A-fragment order of the P V MMA
-    uint32_t pa[8][4];
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
 #pragma unroll
@@ -154,23 +165,57 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         const float p0 = fast_exp2(fmaf(s[4 * i + 2 * hh], c, neg[hh]));
         const float p1 = fast_exp2(fmaf(s[4 * i + 2 * hh + 1], c, neg[hh]));
         l[hh] += p0 + p1;
-        pa[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(p0, p1);
+        s[4 * i + 2 * hh] = p0;
+        s[4 * i + 2 * hh + 1] = p1;
       }
     }
+  };
+  // P packed to T in the A-fragment order of the P V MMA
+  uint32_t pa[8][4];
+  auto pack_p = [&]() {
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) pa[i >> 1][(i & 1) * 2 + hh] = Act16<T>::pack2(s[4 * i + 2 * hh], s[4 * i + 2 * hh + 1]);
+  };
+
+  float alpha[2];
+  ptx::mbar_wait(ptx::smem_u32(&bar_q), 0);
+  issue_s(0);
+  ptx::wgmma_wait<0>();
+  ptx::fence_regs(s);
+  softmax(0, alpha);
+  pack_p();
+
+  // O = O alpha + P_j V_j (one commit group)
+  auto issue_pv = [&](int j) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       o[4 * i] *= alpha[0]; o[4 * i + 1] *= alpha[0];
       o[4 * i + 2] *= alpha[1]; o[4 * i + 3] *= alpha[1];
     }
-    const uint64_t v_desc = ptx::desc_sw128(sV, BKV * 128, 1024);
+    const uint64_t v_desc = ptx::desc_sw128(sKV + (j % STAGES) * 2 * TILE_BYTES + TILE_BYTES, BKV * 128, 1024);
     ptx::wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < BKV / 16; ++kk) ptx::wgmma_m64n64k16_rs<1, T>(o, pa[kk], ptx::desc_add(v_desc, 2048 * kk), 1u);
     ptx::wgmma_commit();
+  };
+  auto retire_pv = [&](int j) {
     ptx::wgmma_wait<0>();
     ptx::fence_regs(o);
-    __syncthreads();   // both warpgroups are done with this stage: it may be refilled
+    if (t == 0) ptx::mbar_arrive(ptx::smem_u32(&bar_empty[j % STAGES]));   // K_j and V_j are no longer read
+  };
+  for (int j = 0; j + 1 < n_kv; ++j) {
+    issue_s(j + 1);
+    issue_pv(j);
+    ptx::wgmma_wait<1>();   // S_{j+1} is in; P_j V_j may still be running
+    ptx::fence_regs(s);
+    softmax(j + 1, alpha);
+    retire_pv(j);
+    pack_p();
   }
+  issue_pv(n_kv - 1);
+  retire_pv(n_kv - 1);
 
   // ---- output: O / l -> T, rows past Tq are not written; lse in the log2 domain
 #pragma unroll
