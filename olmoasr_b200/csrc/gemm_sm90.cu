@@ -86,28 +86,31 @@ __device__ __forceinline__ void quad_transpose(const uint32_t (&w)[4], uint32_t 
   }
 }
 
-// 16-bit epilogues: 8 consecutive columns col .. col+7 of one row, v[k] = T(acc + bias) of columns col+2k, col+2k+1
-template <typename T, int EPI>
-__device__ __forceinline__ void store_16x8(const GemmParams& p, int row, int col, const uint32_t (&v)[4], bool vec_c,
-                                             bool vec_aux) {
-  const bool full = col + 8 <= p.N;
-  uint32_t a[4];
-  if constexpr (reads_aux(EPI)) {   // plain loads: aux may be the output itself (in-place residual)
-    using A = Act16<T>;
-    const T* ap = reinterpret_cast<const T*>(p.aux) + static_cast<int64_t>(row) * p.ldaux + col;
-    if (full && vec_aux) {
-      const uint4 t = *reinterpret_cast<const uint4*>(ap);
-      a[0] = t.x; a[1] = t.y; a[2] = t.z; a[3] = t.w;
-    } else {
-      const uint16_t* ah = reinterpret_cast<const uint16_t*>(ap);
+// aux of 8 consecutive columns col .. col+7 of one row, a[k] = columns col+2k, col+2k+1 (0 past N).  Plain loads: aux
+// may be the output itself (in-place residual).
+template <typename T>
+__device__ __forceinline__ void load_aux_16x8(const GemmParams& p, int row, int col, uint32_t (&a)[4], bool vec_aux) {
+  const T* ap = reinterpret_cast<const T*>(p.aux) + static_cast<int64_t>(row) * p.ldaux + col;
+  if (col + 8 <= p.N && vec_aux) {
+    const uint4 t = *reinterpret_cast<const uint4*>(ap);
+    a[0] = t.x; a[1] = t.y; a[2] = t.z; a[3] = t.w;
+  } else {
+    const uint16_t* ah = reinterpret_cast<const uint16_t*>(ap);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const uint32_t lo = col + 2 * k < p.N ? ah[2 * k] : 0u;
-        const uint32_t hi = col + 2 * k + 1 < p.N ? ah[2 * k + 1] : 0u;
-        a[k] = lo | (hi << 16);
-      }
+    for (int k = 0; k < 4; ++k) {
+      const uint32_t lo = col + 2 * k < p.N ? ah[2 * k] : 0u;
+      const uint32_t hi = col + 2 * k + 1 < p.N ? ah[2 * k + 1] : 0u;
+      a[k] = lo | (hi << 16);
     }
   }
+}
+
+// 16-bit epilogues: 8 consecutive columns col .. col+7 of one row, v[k] = T(acc + bias) of columns col+2k, col+2k+1,
+// a = their aux (load_aux_16x8) for the epilogues that read it
+template <typename T, int EPI>
+__device__ __forceinline__ void store_16x8(const GemmParams& p, int row, int col, const uint32_t (&v)[4],
+                                           const uint32_t (&a)[4], bool vec_c) {
+  const bool full = col + 8 <= p.N;
   using A = Act16<T>;
   uint32_t o[4], g[4];
 #pragma unroll
@@ -287,30 +290,58 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     } else {
-      // T(acc + T(bias)) per column pair, then a quad transpose so that each lane stores 8 consecutive columns
+      // T(acc + T(bias)) per column pair, then a quad transpose so that each lane stores 8 consecutive columns.  The
+      // bias and aux loads of 128 columns are issued together before any of their arithmetic and stores: one round trip
+      // to memory per 128 columns instead of one per 32 (a store may alias a later aux load, so the compiler cannot
+      // hoist those loads itself).  Loading before storing keeps the in-place residual right: every element is read and
+      // written by the same thread.  (Whole 256-column rows at once measured no faster, and slower on the tied logits.)
+      constexpr int JC = BN / 32 < 4 ? BN / 32 : 4;   // 32-column steps per chunk
 #pragma unroll
-      for (int j = 0; j < BN / 32; ++j) {
-        if (ncol0 + 32 * j >= p.N) break;   // warp-uniform: the quad shuffles below need every lane
-        uint32_t w[2][4];
+      for (int j0 = 0; j0 < BN / 32; j0 += JC) {
+        if (ncol0 + 32 * j0 >= p.N) break;
+        float b[JC][4][2];
+        uint32_t a[JC][2][4];
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int i = 4 * j + k;
-          const int col = ncol0 + 8 * i + 2 * (lane & 3);
-          float b0 = 0.f, b1 = 0.f;
-          if (p.bias != nullptr) {   // rounded to T like bias.to(x.dtype)
-            if (col < p.N) b0 = Act16<T>::round(__ldg(p.bias + col));
-            if (col + 1 < p.N) b1 = Act16<T>::round(__ldg(p.bias + col + 1));
+        for (int jj = 0; jj < JC; ++jj) {
+          const int j = j0 + jj;
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int col = ncol0 + 8 * (4 * j + k) + 2 * (lane & 3);
+            b[jj][k][0] = b[jj][k][1] = 0.f;
+            if (p.bias != nullptr) {   // rounded to T like bias.to(x.dtype)
+              if (col < p.N) b[jj][k][0] = Act16<T>::round(__ldg(p.bias + col));
+              if (col + 1 < p.N) b[jj][k][1] = Act16<T>::round(__ldg(p.bias + col + 1));
+            }
           }
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
-            w[h][k] = Act16<T>::pack2(__fadd_rn(acc[4 * i + 2 * h], b0), __fadd_rn(acc[4 * i + 2 * h + 1], b1));
+          for (int h = 0; h < 2; ++h) {
+            a[jj][h][0] = a[jj][h][1] = a[jj][h][2] = a[jj][h][3] = 0u;
+            if constexpr (reads_aux(EPI)) {
+              const int row = row0 + 8 * h, col = ncol0 + 32 * j + 8 * (lane & 3);
+              if (row < p.M && col < p.N) load_aux_16x8<T>(p, row, col, a[jj][h], vec_aux);
+            }
+          }
         }
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t v[4];
-          quad_transpose(w[h], v, lane);
-          const int row = row0 + 8 * h;
-          if (row < p.M) store_16x8<T, EPI>(p, row, ncol0 + 32 * j + 8 * (lane & 3), v, vec_c, vec_aux);
+        for (int jj = 0; jj < JC; ++jj) {
+          const int j = j0 + jj;
+          if (ncol0 + 32 * j >= p.N) break;   // warp-uniform: the quad shuffles below need every lane
+          uint32_t w[2][4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int i = 4 * j + k;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              w[h][k] = Act16<T>::pack2(__fadd_rn(acc[4 * i + 2 * h], b[jj][k][0]),
+                                        __fadd_rn(acc[4 * i + 2 * h + 1], b[jj][k][1]));
+          }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            uint32_t v[4];
+            quad_transpose(w[h], v, lane);
+            const int row = row0 + 8 * h;
+            if (row < p.M) store_16x8<T, EPI>(p, row, ncol0 + 32 * j + 8 * (lane & 3), v, a[jj][h], vec_c);
+          }
         }
       }
     }
