@@ -1,11 +1,14 @@
 // Persistent, warp-specialised bf16 GEMM for sm_90a: TMA -> 128B-swizzled smem ring -> wgmma (fp32 accumulators in
-// registers) -> fused epilogue stored straight from the accumulator fragments.
+// registers) -> fused epilogue, staged through shared memory and stored by TMA for the 16-bit outputs.
 //
 //   D[M,N] = epi( sum_k A[m,k] B[n,k] )
 //
 // One CTA per SM (at most gemm_sm_budget() CTAs), walking over 128 x BN output tiles with stride gridDim.x.  384 threads:
-//   warpgroup 0    TMA producer (one thread issues; the ring keeps running across tiles, so the next tile's operands
-//                  arrive while this tile's epilogue runs).  It gives its registers up (setmaxnreg 40) ...
+//   warpgroup 0    producers, which give their registers up (setmaxnreg 40) ...
+//                  warp 0: one thread streams A / B through the ring (the ring keeps running across tiles, so the next
+//                  tile's operands arrive while this tile's epilogue runs);
+//                  warp 1: the 16-bit epilogues' bias slice and aux tile (residual, GELU pre-activation), loaded into
+//                  shared memory during the tile's mainloop
 //   warpgroups 1-2 ... to the consumers (setmaxnreg 232): warpgroup c owns rows 64c .. 64c+63 of the tile, issues its
 //                  m64 x BN x 16 wgmmas and runs the epilogue for those rows
 // Tile = 128 x BN (BN = 64, 128 or 256; 256 keeps 128 fp32 accumulators per consumer thread), BK = 64 bf16 (= one
@@ -18,6 +21,7 @@
 
 #include <stdio.h>
 #include <stdlib.h>
+#include <string.h>
 
 namespace oasr {
 namespace {
@@ -28,6 +32,11 @@ constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
 constexpr int THREADS = 384;
 constexpr int PRODUCER_REGS = 40;    // 40 * 128 + 232 * 256 <= 64 K registers of the SM
 constexpr int CONSUMER_REGS = 232;
+// The 16-bit epilogues stage their results in boxes of 64 rows x 64 columns (8 KB, one consumer warpgroup's rows),
+// 128-byte swizzled like the TMA boxes they are loaded and stored as: 16-byte chunk j of row r sits at
+// r * 128 + (j ^ (r % 8)) * 16.
+constexpr int BOX = 64;
+constexpr int BOX_BYTES = BOX * BOX * 2;
 
 struct GemmParams {
   void* C;
@@ -38,18 +47,29 @@ struct GemmParams {
   int64_t ldaux;
   int M, N, K;
   int tiles_m, tiles_n, splits;
+  int num_tiles;   // tiles_m * tiles_n * splits (a parameter, so the tile loops need no register for it)
   int kblocks_total, kblocks_per_split;
   int raster_m;  // 1: consecutive tiles walk M first (B tile stays hot in L2) -- used when B is the larger operand
   int64_t split_stride;   // split-K: split s stores its fp32 partial at C + s * split_stride (0: one split)
+  // 16-bit epilogues: C (and C2) / aux move by TMA (16-byte aligned base and row stride), else by plain bounded copies
+  int tma_out, tma_aux;
 };
 
-template <int BN>
+constexpr bool is_f32_epi(int epi) { return epi == OASR_EPI_F32 || epi == OASR_EPI_F32_ATOMIC_ADD; }
+constexpr bool reads_aux(int epi) { return epi == OASR_EPI_BF16_RESIDUAL || epi == OASR_EPI_BF16_GELU_BWD; }
+
+template <int BN, int EPI>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int BUDGET = 232448 - 1024;   // 227 KB of dynamic smem per block, minus the barrier area
+  // Epilogue buffer after the ring: the aux epilogues hold the whole 128 x BN aux tile (each result is written over its
+  // own aux and stored from there); BF16 and GELU cycle two output boxes per consumer warpgroup.  Then BN fp32 of bias.
+  static constexpr int EPI_BYTES = is_f32_epi(EPI) ? 0 : (reads_aux(EPI) ? BM * BN * 2 : 2 * 2 * BOX_BYTES);
+  static constexpr int BIAS_BYTES = is_f32_epi(EPI) ? 0 : BN * 4;
+  static constexpr int BUDGET = 232448 - 1024 - EPI_BYTES - BIAS_BYTES;   // 227 KB per block, minus the barrier area
   static constexpr int STAGES = (BUDGET / STAGE_BYTES) > 8 ? 8 : (BUDGET / STAGE_BYTES);
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;   // 1024-aligned base: tiles first, barriers last
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + BIAS_BYTES + 1024;   // 1024-aligned base, barriers last
+  static_assert(STAGES >= 3, "gemm: shared-memory ring too shallow");
 };
 
 // tile index -> (m block, n block, k split).  Default order walks N fastest: the CTAs running together share A row
@@ -65,96 +85,55 @@ __device__ __forceinline__ void decode_tile(int tile, const GemmParams& p, int& 
   split = tile / (p.tiles_n * p.tiles_m);
 }
 
-constexpr bool is_f32_epi(int epi) { return epi == OASR_EPI_F32 || epi == OASR_EPI_F32_ATOMIC_ADD; }
-constexpr bool reads_aux(int epi) { return epi == OASR_EPI_BF16_RESIDUAL || epi == OASR_EPI_BF16_GELU_BWD; }
-
-__device__ __forceinline__ uint32_t pick4(const uint32_t (&w)[4], int i) {
-  return i == 0 ? w[0] : (i == 1 ? w[1] : (i == 2 ? w[2] : w[3]));
-}
-
-// 4 x 4 word transpose inside each quad of lanes: lane q holds w[k] = bf16 columns 8k + 2q, 8k + 2q + 1 (k = 0..3) of
-// one row; afterwards it holds v[k] = columns 8q + 2k, 8q + 2k + 1, i.e. 8 consecutive columns (one 16-byte store).
-__device__ __forceinline__ void quad_transpose(const uint32_t (&w)[4], uint32_t (&v)[4], int lane) {
-  const int q = lane & 3;
-#pragma unroll
-  for (int r = 0; r < 4; ++r) {   // round r: lane p sends its w[(p + r) % 4], lane q receives from lane (q - r) % 4
-    const int src = (q - r) & 3;
-    const uint32_t x = __shfl_sync(0xffffffffu, pick4(w, (q + r) & 3), (lane & ~3) | src);
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      if (src == k) v[k] = x;
-  }
-}
-
-// aux of 8 consecutive columns col .. col+7 of one row, a[k] = columns col+2k, col+2k+1 (0 past N).  Plain loads: aux
-// may be the output itself (in-place residual).
+// Plain copies of one box between global (rows row0.., columns col0.., bounded by M and N; zeros past them on the way
+// in) and its swizzled shared-memory image, 8 columns per step: the path for tensors TMA cannot address.
 template <typename T>
-__device__ __forceinline__ void load_aux_16x8(const GemmParams& p, int row, int col, uint32_t (&a)[4], bool vec_aux) {
-  const T* ap = reinterpret_cast<const T*>(p.aux) + static_cast<int64_t>(row) * p.ldaux + col;
-  if (col + 8 <= p.N && vec_aux) {
-    const uint4 t = *reinterpret_cast<const uint4*>(ap);
-    a[0] = t.x; a[1] = t.y; a[2] = t.z; a[3] = t.w;
-  } else {
-    const uint16_t* ah = reinterpret_cast<const uint16_t*>(ap);
+__device__ __forceinline__ void box_from_global(uint8_t* box, const void* src, int64_t ld, int row0, int col0, const GemmParams& p,
+                                                int tid, int nthreads) {
+  for (int k = tid; k < BOX * BOX / 8; k += nthreads) {
+    const int r = k >> 3, j = k & 7, row = row0 + r, col = col0 + 8 * j;
+    uint16_t v[8];
+    const uint16_t* s = reinterpret_cast<const uint16_t*>(src) + static_cast<int64_t>(row) * ld + col;
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const uint32_t lo = col + 2 * k < p.N ? ah[2 * k] : 0u;
-      const uint32_t hi = col + 2 * k + 1 < p.N ? ah[2 * k + 1] : 0u;
-      a[k] = lo | (hi << 16);
-    }
+    for (int e = 0; e < 8; ++e) v[e] = (row < p.M && col + e < p.N) ? s[e] : uint16_t(0);
+    *reinterpret_cast<uint4*>(box + r * 128 + ((j ^ (r & 7)) << 4)) =
+        make_uint4(v[0] | (uint32_t(v[1]) << 16), v[2] | (uint32_t(v[3]) << 16), v[4] | (uint32_t(v[5]) << 16),
+                   v[6] | (uint32_t(v[7]) << 16));
   }
 }
-
-// 16-bit epilogues: 8 consecutive columns col .. col+7 of one row, v[k] = T(acc + bias) of columns col+2k, col+2k+1,
-// a = their aux (load_aux_16x8) for the epilogues that read it
-template <typename T, int EPI>
-__device__ __forceinline__ void store_16x8(const GemmParams& p, int row, int col, const uint32_t (&v)[4],
-                                           const uint32_t (&a)[4], bool vec_c) {
-  const bool full = col + 8 <= p.N;
-  using A = Act16<T>;
-  uint32_t o[4], g[4];
+template <typename T>
+__device__ __forceinline__ void box_to_global(const uint8_t* box, void* dst, int64_t ld, int row0, int col0, const GemmParams& p,
+                                              int tid) {
+  for (int k = tid; k < BOX * BOX / 8; k += 128) {
+    const int r = k >> 3, j = k & 7, row = row0 + r, col = col0 + 8 * j;
+    if (row >= p.M || col >= p.N) continue;
+    const uint16_t* s = reinterpret_cast<const uint16_t*>(box + r * 128 + ((j ^ (r & 7)) << 4));
+    uint16_t* d = reinterpret_cast<uint16_t*>(dst) + static_cast<int64_t>(row) * ld + col;
 #pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    o[k] = v[k];
-    if constexpr (EPI == OASR_EPI_BF16_GELU) {   // h = bf16(acc + b), g = bf16(gelu(h))
-      const float2 x = gelu_erf2(A::unpack2(v[k]));
-      g[k] = A::pack2(x.x, x.y);
-    } else if constexpr (EPI == OASR_EPI_BF16_RESIDUAL) {   // C = bf16(aux + bf16(acc + b))
-      const float2 x = fadd2(A::unpack2(a[k]), A::unpack2(v[k]));
-      o[k] = A::pack2(x.x, x.y);
-    } else if constexpr (EPI == OASR_EPI_BF16_GELU_BWD) {   // C = bf16(bf16(acc) * gelu'(aux))
-      const float2 x = fmul2(A::unpack2(v[k]), gelu_erf_grad2(A::unpack2(a[k])));
-      o[k] = A::pack2(x.x, x.y);
-    }
-  }
-  const int64_t off = static_cast<int64_t>(row) * p.ldc + col;
-#pragma unroll
-  for (int out = 0; out < (EPI == OASR_EPI_BF16_GELU ? 2 : 1); ++out) {
-    const uint32_t* src = out ? g : o;
-    T* dst = reinterpret_cast<T*>(out ? p.C2 : p.C) + off;
-    if (full && vec_c) {
-      *reinterpret_cast<uint4*>(dst) = make_uint4(src[0], src[1], src[2], src[3]);
-    } else {
-      uint16_t* dh = reinterpret_cast<uint16_t*>(dst);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if (col + 2 * k < p.N) dh[2 * k] = static_cast<uint16_t>(src[k]);
-        if (col + 2 * k + 1 < p.N) dh[2 * k + 1] = static_cast<uint16_t>(src[k] >> 16);
-      }
-    }
+    for (int e = 0; e < 8; ++e)
+      if (col + e < p.N) d[e] = s[e];
   }
 }
 
 template <typename T, int BN, int A_MN, int B_MN, int EPI>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  using C = Cfg<BN>;
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2,
+                  const __grid_constant__ CUtensorMap tmAux, const GemmParams p) {
+  using C = Cfg<BN, EPI>;
   constexpr int STAGES = C::STAGES;
   constexpr int NACC = BN / 2;   // accumulator registers per thread (64 x BN fp32 over 128 threads)
+  constexpr bool EPI16 = !is_f32_epi(EPI);
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem_raw + STAGES * C::STAGE_BYTES);
+  uint8_t* epi_buf = smem_raw + STAGES * C::STAGE_BYTES;
+  float* bias_s = reinterpret_cast<float*>(epi_buf + C::EPI_BYTES);
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(epi_buf + C::EPI_BYTES + C::BIAS_BYTES);
   uint64_t* bar_empty = bar_full + STAGES;
+  // 16-bit epilogues: the epilogue producer fills bias (and aux) for a tile -> epi_full; both consumer warpgroups are
+  // done with them -> epi_empty
+  const uint32_t epi_full = ptx::smem_u32(bar_empty + STAGES);
+  const uint32_t epi_empty = epi_full + 8;
 
   const uint32_t smem_base = ptx::smem_u32(smem_raw);
   if (smem_base & 1023u) __trap();
@@ -163,23 +142,28 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (threadIdx.x == 0) {
     ptx::tma_prefetch_desc(&tmA);
     ptx::tma_prefetch_desc(&tmB);
+    if (EPI16 && p.tma_out) {
+      ptx::tma_prefetch_desc(&tmC);
+      if (EPI == OASR_EPI_BF16_GELU) ptx::tma_prefetch_desc(&tmC2);
+    }
+    if (reads_aux(EPI) && p.tma_aux) ptx::tma_prefetch_desc(&tmAux);
     for (int s = 0; s < STAGES; ++s) {
       ptx::mbar_init(ptx::smem_u32(&bar_full[s]), 1);
       ptx::mbar_init(ptx::smem_u32(&bar_empty[s]), 2);   // one arrival per consumer warpgroup
     }
+    ptx::mbar_init(epi_full, 32);    // every lane of the epilogue producer warp
+    ptx::mbar_init(epi_empty, 2);    // one arrival per consumer warpgroup
     ptx::fence_barrier_init();
   }
   __syncthreads();
 
-  const int num_tiles = p.tiles_m * p.tiles_n * p.splits;
-
   if (wg == 0) {
-    // ===================== TMA producer =====================
     ptx::setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
+      // ===================== operand producer =====================
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         int m_blk, n_blk, split;
         decode_tile(tile, p, m_blk, n_blk, split);
         const int kb0 = split * p.kblocks_per_split;
@@ -205,6 +189,40 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
+    } else if (EPI16 && (threadIdx.x >> 5) == 1) {
+      // ===================== epilogue producer: bias slice and aux tile of each tile =====================
+      // Its own barriers: the operand producer never waits on the epilogue's buffers.
+      const int lane = threadIdx.x & 31;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, phase ^= 1) {
+        int m_blk, n_blk, split;
+        decode_tile(tile, p, m_blk, n_blk, split);
+        const int m0 = m_blk * BM, n0 = n_blk * BN;
+        ptx::mbar_wait(epi_empty, phase ^ 1);   // both consumer warpgroups are done with the previous tile's
+        for (int j = lane; j < BN; j += 32)     // rounded to T like bias.to(x.dtype); 0 past N
+          bias_s[j] = (p.bias != nullptr && n0 + j < p.N) ? Act16<T>::round(__ldg(p.bias + n0 + j)) : 0.f;
+        if (reads_aux(EPI) && p.tma_aux) {
+          if (lane == 0) {   // the boxes that hold rows < M and columns < N; TMA zero-fills past the edges
+            const int halves = p.M - m0 > 64 ? 2 : 1;
+            const int boxes = min(BN / BOX, (p.N - n0 + BOX - 1) / BOX);
+            ptx::mbar_arrive_expect_tx(epi_full, halves * boxes * BOX_BYTES);
+            for (int h = 0; h < halves; ++h)
+              for (int b = 0; b < boxes; ++b)
+                ptx::tma_load_2d(ptx::smem_u32(epi_buf) + (h * (BN / BOX) + b) * BOX_BYTES, &tmAux, epi_full, n0 + BOX * b,
+                                 m0 + 64 * h);
+          } else {
+            ptx::mbar_arrive(epi_full);
+          }
+        } else {
+          if (reads_aux(EPI)) {
+            for (int h = 0; h < 2; ++h)
+              for (int b = 0; b < BN / BOX; ++b)
+                box_from_global<T>(epi_buf + (h * (BN / BOX) + b) * BOX_BYTES, p.aux, p.ldaux, m0 + 64 * h, n0 + BOX * b, p,
+                                   lane, 32);
+          }
+          ptx::mbar_arrive(epi_full);
+        }
+      }
     }
     return;
   }
@@ -220,15 +238,14 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   constexpr uint32_t b_kstep = B_MN ? 16 * 128 : 16 * 2;
   const uint64_t a_desc0 = ptx::desc_sw128(smem_base + c * 8192, A_MN ? BK * 128 : 16, 1024);
   const uint64_t b_desc0 = ptx::desc_sw128(smem_base + A_STAGE_BYTES, B_MN ? BK * 128 : 16, 1024);
-  const bool vec_c = is_f32_epi(EPI) ? ((p.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 7) == 0)
-                                     : ((p.ldc & 7) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 15) == 0 &&
-                                        (p.C2 == nullptr || (reinterpret_cast<uintptr_t>(p.C2) & 15) == 0));
-  const bool vec_aux = (p.ldaux & 7) == 0 && (reinterpret_cast<uintptr_t>(p.aux) & 15) == 0;
+  const bool vec_c = is_f32_epi(EPI) && (p.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(p.C) & 7) == 0;
+  // this warpgroup's half of the epilogue buffer
+  const uint32_t epi_wg = ptx::smem_u32(epi_buf) + c * (C::EPI_BYTES / 2);
 
   int stage = 0;
-  uint32_t phase = 0;
+  uint32_t phase = 0, epi_phase = 0;
   float acc[NACC];
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
     int m_blk, n_blk, split;
     decode_tile(tile, p, m_blk, n_blk, split);
     const int kb0 = split * p.kblocks_per_split;
@@ -248,6 +265,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         else ptx::wgmma_m64n64k16_ss<A_MN, B_MN, T>(acc, da, db, accumulate);
       }
       ptx::wgmma_commit();
+      if (EPI16 && kb == kb0 && tile != static_cast<int>(blockIdx.x) && t == 0) {
+        // The previous tile's epilogue is over (its last box barrier came after every read of bias and aux); with the
+        // MMAs of this tile under way, hand its buffers back once the TMA engine has read the stores' sources.
+        if (reads_aux(EPI) && p.tma_out) ptx::bulk_wait_group_read<0>();
+        ptx::mbar_arrive(epi_empty);
+      }
       ptx::wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot may be refilled
       if (prev >= 0 && t == 0) ptx::mbar_arrive(ptx::smem_u32(&bar_empty[prev]));
       prev = stage;
@@ -257,11 +280,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     ptx::fence_regs(acc);
     if (t == 0) ptx::mbar_arrive(ptx::smem_u32(&bar_empty[prev]));
 
-    // ---- epilogue straight from the fragments: row 16*warp + lane/4 (+8), columns 8i + 2*(lane%4) (+1)
-    const int row0 = m_blk * BM + c * 64 + warp * 16 + (lane >> 2);
-    const int ncol0 = n_blk * BN;
     if constexpr (is_f32_epi(EPI)) {
-      const int col0 = ncol0 + 2 * (lane & 3);
+      // ---- straight from the fragments: row 16*warp + lane/4 (+8), columns 8i + 2*(lane%4) (+1)
+      const int row0 = m_blk * BM + c * 64 + warp * 16 + (lane >> 2);
+      const int col0 = n_blk * BN + 2 * (lane & 3);
 #pragma unroll
       for (int i = 0; i < BN / 8; ++i) {
         const int col = col0 + 8 * i;
@@ -290,62 +312,77 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     } else {
-      // T(acc + T(bias)) per column pair, then a quad transpose so that each lane stores 8 consecutive columns.  The
-      // bias and aux loads of 128 columns are issued together before any of their arithmetic and stores: one round trip
-      // to memory per 128 columns instead of one per 32 (a store may alias a later aux load, so the compiler cannot
-      // hoist those loads itself).  Loading before storing keeps the in-place residual right: every element is read and
-      // written by the same thread.  (Whole 256-column rows at once measured no faster, and slower on the tied logits.)
-      constexpr int JC = BN / 32 < 4 ? BN / 32 : 4;   // 32-column steps per chunk
+      // ---- 16-bit: T(acc + T(bias)) per column pair (then GELU / residual / GELU backward) into 64 x 64 boxes in shared
+      // memory, each stored by one TMA while the warpgroup goes on.  Fragment rows r = 16*warp + lane/4 and r + 8
+      // (r % 8 = lane / 4), columns 8i + 2*(lane%4) (+1): one 4-byte word per row of 16-byte chunk i % 8 of box i / 8,
+      // and the 8 rows a warp writes at once fall in 8 different chunks, i.e. all 32 banks.
+      ptx::mbar_wait(epi_full, epi_phase);
+      epi_phase ^= 1;
+      const int row0 = m_blk * BM + c * 64;   // first row of this warpgroup's boxes
+      if (row0 < p.M) {
+        const uint32_t word = (16 * warp + (lane >> 2)) * 128 + 4 * (lane & 3);
+        const uint32_t bias_q = ptx::smem_u32(bias_s) + 8 * (lane & 3);
 #pragma unroll
-      for (int j0 = 0; j0 < BN / 32; j0 += JC) {
-        if (ncol0 + 32 * j0 >= p.N) break;
-        float b[JC][4][2];
-        uint32_t a[JC][2][4];
+        for (int b = 0; b < BN / BOX; ++b) {
+          const int col0 = n_blk * BN + BOX * b;
+          if (col0 >= p.N) break;   // warpgroup-uniform
 #pragma unroll
-        for (int jj = 0; jj < JC; ++jj) {
-          const int j = j0 + jj;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int col = ncol0 + 8 * (4 * j + k) + 2 * (lane & 3);
-            b[jj][k][0] = b[jj][k][1] = 0.f;
-            if (p.bias != nullptr) {   // rounded to T like bias.to(x.dtype)
-              if (col < p.N) b[jj][k][0] = Act16<T>::round(__ldg(p.bias + col));
-              if (col + 1 < p.N) b[jj][k][1] = Act16<T>::round(__ldg(p.bias + col + 1));
-            }
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            a[jj][h][0] = a[jj][h][1] = a[jj][h][2] = a[jj][h][3] = 0u;
+          for (int out = 0; out < (EPI == OASR_EPI_BF16_GELU ? 2 : 1); ++out) {
+            uint32_t box;
             if constexpr (reads_aux(EPI)) {
-              const int row = row0 + 8 * h, col = ncol0 + 32 * j + 8 * (lane & 3);
-              if (row < p.M && col < p.N) load_aux_16x8<T>(p, row, col, a[jj][h], vec_aux);
+              box = epi_wg + b * BOX_BYTES;   // the aux box: each result goes over its own aux
+            } else {   // two slots in turn; the store that last read this one is done with it
+              constexpr int NOUT = EPI == OASR_EPI_BF16_GELU ? 2 : 1;
+              box = epi_wg + ((b * NOUT + out) & 1) * BOX_BYTES;
+              if (t == 0) {   // (a tile's first box: the previous tile's stores went out a whole mainloop ago)
+                if (b == 0 && out == 0) ptx::bulk_wait_group_read<0>();
+                else ptx::bulk_wait_group_read<1>();
+              }
+              ptx::named_bar_sync(1 + c, 128);
             }
-          }
-        }
 #pragma unroll
-        for (int jj = 0; jj < JC; ++jj) {
-          const int j = j0 + jj;
-          if (ncol0 + 32 * j >= p.N) break;   // warp-uniform: the quad shuffles below need every lane
-          uint32_t w[2][4];
+            for (int j = 0; j < BOX / 8; ++j) {
+              const int i = (BOX / 8) * b + j;
+              const float2 bb = ptx::ld_shared_f32x2(bias_q + 32 * i);
+              const uint32_t wa = box + word + ((j ^ (lane >> 2)) << 4);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int i = 4 * j + k;
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-              w[h][k] = Act16<T>::pack2(__fadd_rn(acc[4 * i + 2 * h], b[jj][k][0]),
-                                        __fadd_rn(acc[4 * i + 2 * h + 1], b[jj][k][1]));
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint32_t v[4];
-            quad_transpose(w[h], v, lane);
-            const int row = row0 + 8 * h;
-            if (row < p.M) store_16x8<T, EPI>(p, row, ncol0 + 32 * j + 8 * (lane & 3), v, a[jj][h], vec_c);
+              for (int h = 0; h < 2; ++h) {
+                using A = Act16<T>;
+                const uint32_t v = A::pack2(__fadd_rn(acc[4 * i + 2 * h], bb.x), __fadd_rn(acc[4 * i + 2 * h + 1], bb.y));
+                uint32_t o = v;
+                if constexpr (EPI == OASR_EPI_BF16_GELU) {   // h = T(acc + b), g = T(gelu(h))
+                  if (out) {
+                    const float2 x = gelu_erf2(A::unpack2(v));
+                    o = A::pack2(x.x, x.y);
+                  }
+                } else if constexpr (EPI == OASR_EPI_BF16_RESIDUAL) {   // C = T(aux + T(acc + b))
+                  const float2 x = fadd2(A::unpack2(ptx::ld_shared_u32(wa + 1024 * h)), A::unpack2(v));
+                  o = A::pack2(x.x, x.y);
+                } else if constexpr (EPI == OASR_EPI_BF16_GELU_BWD) {   // C = T(T(acc) * gelu'(aux))
+                  const float2 x = fmul2(A::unpack2(v), gelu_erf_grad2(A::unpack2(ptx::ld_shared_u32(wa + 1024 * h))));
+                  o = A::pack2(x.x, x.y);
+                }
+                ptx::st_shared_u32(wa + 1024 * h, o);   // row r + 8h: 1024 bytes on, same swizzle
+              }
+            }
+            if (p.tma_out) {
+              ptx::fence_proxy_async_smem();
+              ptx::named_bar_sync(1 + c, 128);
+              if (t == 0) {
+                ptx::tma_store_2d(out ? &tmC2 : &tmC, box, col0, row0);
+                ptx::bulk_commit_group();
+              }
+            } else {
+              ptx::named_bar_sync(1 + c, 128);
+              box_to_global<T>(smem_raw + (box - smem_base), out ? p.C2 : p.C, p.ldc, row0, col0, p, t);
+              ptx::named_bar_sync(1 + c, 128);
+            }
           }
         }
       }
     }
   }
+  if (EPI16 && t == 0) ptx::bulk_wait_group<0>();   // the stores read shared memory until they complete
 }
 
 // split-K: out[m, n] += sum_s ws[s][m][n], splits in order (fp32 atomics would round differently from run to run)
@@ -358,18 +395,22 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, int splits, i
   }
 }
 
+// operand maps (A, B) and the 16-bit epilogues' maps (C, C2, aux; zero when unused)
+struct Maps {
+  CUtensorMap a, b, c, c2, aux;
+};
+
 template <typename T, int BN, int A_MN, int B_MN, int EPI>
-int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
-  using C = Cfg<BN>;
+int launch(const Maps& m, const GemmParams& p, cudaStream_t st) {
+  using C = Cfg<BN, EPI>;
   auto kern = gemm_wgmma_kernel<T, BN, A_MN, B_MN, EPI>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     OASR_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     attr_set = true;
   }
-  const int tiles = p.tiles_m * p.tiles_n * p.splits;
-  const int grid = tiles < gemm_sm_budget() ? tiles : gemm_sm_budget();
-  kern<<<grid, THREADS, C::SMEM_BYTES, st>>>(tmA, tmB, p);
+  const int grid = p.num_tiles < gemm_sm_budget() ? p.num_tiles : gemm_sm_budget();
+  kern<<<grid, THREADS, C::SMEM_BYTES, st>>>(m.a, m.b, m.c, m.c2, m.aux, p);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
@@ -380,30 +421,35 @@ int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, 
 //   A MN-major, B MN-major (wgrad):                                F32, F32_ATOMIC_ADD
 // (split-K launches store fp32 partials: they run the F32 kernel).  Any other pair is rejected.
 template <typename T, int BN>
-int dispatch(int a_mn, int b_mn, int epi, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
+int dispatch(int a_mn, int b_mn, int epi, const Maps& m, const GemmParams& p, cudaStream_t st) {
   if (!a_mn && !b_mn) {
     switch (epi) {
-      case OASR_EPI_BF16: return launch<T, BN, 0, 0, OASR_EPI_BF16>(tmA, tmB, p, st);
-      case OASR_EPI_BF16_GELU: return launch<T, BN, 0, 0, OASR_EPI_BF16_GELU>(tmA, tmB, p, st);
-      case OASR_EPI_BF16_RESIDUAL: return launch<T, BN, 0, 0, OASR_EPI_BF16_RESIDUAL>(tmA, tmB, p, st);
-      case OASR_EPI_BF16_GELU_BWD: return launch<T, BN, 0, 0, OASR_EPI_BF16_GELU_BWD>(tmA, tmB, p, st);
-      case OASR_EPI_F32: return launch<T, BN, 0, 0, OASR_EPI_F32>(tmA, tmB, p, st);
+      case OASR_EPI_BF16: return launch<T, BN, 0, 0, OASR_EPI_BF16>(m, p, st);
+      case OASR_EPI_BF16_GELU: return launch<T, BN, 0, 0, OASR_EPI_BF16_GELU>(m, p, st);
+      case OASR_EPI_BF16_RESIDUAL: return launch<T, BN, 0, 0, OASR_EPI_BF16_RESIDUAL>(m, p, st);
+      case OASR_EPI_BF16_GELU_BWD: return launch<T, BN, 0, 0, OASR_EPI_BF16_GELU_BWD>(m, p, st);
+      case OASR_EPI_F32: return launch<T, BN, 0, 0, OASR_EPI_F32>(m, p, st);
     }
   } else if (!a_mn && b_mn) {
     switch (epi) {
-      case OASR_EPI_BF16: return launch<T, BN, 0, 1, OASR_EPI_BF16>(tmA, tmB, p, st);
-      case OASR_EPI_BF16_RESIDUAL: return launch<T, BN, 0, 1, OASR_EPI_BF16_RESIDUAL>(tmA, tmB, p, st);
-      case OASR_EPI_BF16_GELU_BWD: return launch<T, BN, 0, 1, OASR_EPI_BF16_GELU_BWD>(tmA, tmB, p, st);
-      case OASR_EPI_F32: return launch<T, BN, 0, 1, OASR_EPI_F32>(tmA, tmB, p, st);
+      case OASR_EPI_BF16: return launch<T, BN, 0, 1, OASR_EPI_BF16>(m, p, st);
+      case OASR_EPI_BF16_RESIDUAL: return launch<T, BN, 0, 1, OASR_EPI_BF16_RESIDUAL>(m, p, st);
+      case OASR_EPI_BF16_GELU_BWD: return launch<T, BN, 0, 1, OASR_EPI_BF16_GELU_BWD>(m, p, st);
+      case OASR_EPI_F32: return launch<T, BN, 0, 1, OASR_EPI_F32>(m, p, st);
     }
   } else if (a_mn && b_mn) {
     switch (epi) {
-      case OASR_EPI_F32: return launch<T, BN, 1, 1, OASR_EPI_F32>(tmA, tmB, p, st);
-      case OASR_EPI_F32_ATOMIC_ADD: return launch<T, BN, 1, 1, OASR_EPI_F32_ATOMIC_ADD>(tmA, tmB, p, st);
+      case OASR_EPI_F32: return launch<T, BN, 1, 1, OASR_EPI_F32>(m, p, st);
+      case OASR_EPI_F32_ATOMIC_ADD: return launch<T, BN, 1, 1, OASR_EPI_F32_ATOMIC_ADD>(m, p, st);
     }
   }
   set_last_error("gemm: no kernel for a_layout=%d b_layout=%d epilogue=%d", a_mn, b_mn, epi);
   return OASR_ERR_UNSUPPORTED;
+}
+
+// TMA addresses a 16-bit matrix whose base and row stride are multiples of 16 bytes
+bool tma_addressable(const void* base, int64_t ld) {
+  return (reinterpret_cast<uintptr_t>(base) & 15) == 0 && (ld & 7) == 0;
 }
 
 template <typename T>
@@ -436,21 +482,38 @@ int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, i
   p.kblocks_per_split = (int)ceil_div(p.kblocks_total, split_k);
   p.splits = (int)ceil_div(p.kblocks_total, p.kblocks_per_split);
   p.raster_m = (N > M) ? 1 : 0;
+  p.num_tiles = p.tiles_m * p.tiles_n * p.splits;
   p.split_stride = 0;
 
-  CUtensorMap tmA, tmB;
+  Maps m;
+  memset(&m, 0, sizeof(m));
   constexpr bool f16 = Act16<T>::is_fp16;
   int rc;
   if (a_layout == OASR_K_MAJOR)
-    rc = make_tmap_2d(&tmA, A, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BK, BM, true, f16);
+    rc = make_tmap_2d(&m.a, A, 2, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, BK, BM, true, f16);
   else
-    rc = make_tmap_2d(&tmA, A, 2, (uint64_t)M, (uint64_t)K, (uint64_t)lda * 2, 64, BK, true, f16);
+    rc = make_tmap_2d(&m.a, A, 2, (uint64_t)M, (uint64_t)K, (uint64_t)lda * 2, 64, BK, true, f16);
   if (rc) return rc;
   if (b_layout == OASR_K_MAJOR)
-    rc = make_tmap_2d(&tmB, B, 2, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, BK, block_n, true, f16);
+    rc = make_tmap_2d(&m.b, B, 2, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, BK, block_n, true, f16);
   else
-    rc = make_tmap_2d(&tmB, B, 2, (uint64_t)N, (uint64_t)K, (uint64_t)ldb * 2, 64, BK, true, f16);
+    rc = make_tmap_2d(&m.b, B, 2, (uint64_t)N, (uint64_t)K, (uint64_t)ldb * 2, 64, BK, true, f16);
   if (rc) return rc;
+
+  // 16-bit epilogues: outputs and aux move by TMA in 64 x 64 boxes where TMA can address them (clipped at M and N by
+  // the maps), by plain bounded copies otherwise
+  const bool epi16 = !is_f32_epi(epilogue);
+  p.tma_out = epi16 && tma_addressable(Cout, ldc) && (epilogue != OASR_EPI_BF16_GELU || tma_addressable(C2, ldc));
+  p.tma_aux = reads_aux(epilogue) && tma_addressable(aux, ldaux);
+  if (p.tma_out) {
+    if ((rc = make_tmap_2d(&m.c, Cout, 2, (uint64_t)N, (uint64_t)M, (uint64_t)ldc * 2, BOX, BOX, true, f16))) return rc;
+    if (epilogue == OASR_EPI_BF16_GELU &&
+        (rc = make_tmap_2d(&m.c2, C2, 2, (uint64_t)N, (uint64_t)M, (uint64_t)ldc * 2, BOX, BOX, true, f16)))
+      return rc;
+  }
+  if (p.tma_aux &&
+      (rc = make_tmap_2d(&m.aux, aux, 2, (uint64_t)N, (uint64_t)M, (uint64_t)ldaux * 2, BOX, BOX, true, f16)))
+    return rc;
 
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   float* ws = nullptr;
@@ -459,9 +522,9 @@ int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, i
     if (!ws) return OASR_ERR_CUDA;
     p.C = ws; p.ldc = N; epilogue = OASR_EPI_F32; p.split_stride = M * N;
   }
-  rc = block_n == 256 ? dispatch<T, 256>(a_layout, b_layout, epilogue, tmA, tmB, p, st)
-     : block_n == 128 ? dispatch<T, 128>(a_layout, b_layout, epilogue, tmA, tmB, p, st)
-                      : dispatch<T, 64>(a_layout, b_layout, epilogue, tmA, tmB, p, st);
+  rc = block_n == 256 ? dispatch<T, 256>(a_layout, b_layout, epilogue, m, p, st)
+     : block_n == 128 ? dispatch<T, 128>(a_layout, b_layout, epilogue, m, p, st)
+                      : dispatch<T, 64>(a_layout, b_layout, epilogue, m, p, st);
   if (ws) {
     if (rc == OASR_OK) {
       int64_t blocks = ceil_div(M * N, 256);
