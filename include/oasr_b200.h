@@ -308,15 +308,34 @@ OASR_API int oasr_dec_beam_reorder(void* k_cache, void* v_cache, int64_t layer_s
  *   c0 = cost[i-1][j-1], c1 = cost[i-1][j], c2 = cost[i][j-1]: t = 0 if c0 < c1 and c0 < c2, else 1 if c1 < c0 and
  *   c1 < c2, else 2; cost[i][j] = x[i-1][j-1] + c rounded to float32.  trace: (rows + 1) x (cols + 1) byte workspace.
  *   Writes the path (text_idx, time_idx) (int32, room for rows + cols entries) in path order and its length to
- *   *path_len.  One CTA; rows <= 17065. */
+ *   *path_len.  One CTA; rows <= 17065.
+ * oasr_align_cost_batched / oasr_dtw_batched: the same computations for n_windows windows of any sizes in one call each
+ *   (the windows of one transcribe_batch() round).  `windows` is a DEVICE table of one descriptor per window; the kernels
+ *   trust its entries, so the caller keeps every n_tok <= max_tok, n_frames <= max_frames and rows <= max_rows (the host
+ *   sizes the grid and the shared memory from these maxima).  Each window's arithmetic is exactly that of the
+ *   single-window entry point (which is the one-window case of the same kernels): the results are bit-identical.
+ *   oasr_align_window: heads -> a device table of n_heads oasr_align_head entries; row_stats -> offset in floats of the
+ *   window's (n_heads, n_tok, 2) workspace inside `row_stats`; cost (n_tok - 2, n_frames) with row stride ld_cost.
+ *   oasr_dtw_window: x (rows, cols) with row stride ldx, a (rows + 1) x (cols + 1) byte trace, the path slots. */
 typedef struct oasr_align_head {
   const void* q; const void* k; int64_t ldq; int64_t ldk;
 } oasr_align_head;
+typedef struct oasr_align_window {
+  const oasr_align_head* heads; float* cost; int64_t ld_cost; int64_t row_stats; int32_t n_tok; int32_t n_frames;
+} oasr_align_window;
+typedef struct oasr_dtw_window {
+  const float* x; int64_t ldx; uint8_t* trace; int32_t* text_idx; int32_t* time_idx; int32_t* path_len;
+  int32_t rows; int32_t cols;
+} oasr_dtw_window;
 OASR_API int oasr_align_cost(const oasr_align_head* heads, int32_t n_heads, int32_t head_dim, int32_t n_tok,
                              int32_t n_frames, int32_t medfilt_width, float* row_stats, float* cost, int64_t ld_cost,
                              int dtype, void* stream);
 OASR_API int oasr_dtw(const float* x, int64_t ldx, int32_t rows, int32_t cols, uint8_t* trace, int32_t* text_idx,
                       int32_t* time_idx, int32_t* path_len, void* stream);
+OASR_API int oasr_align_cost_batched(const oasr_align_window* windows, int32_t n_windows, int32_t n_heads,
+                                     int32_t head_dim, int32_t max_tok, int32_t max_frames, int32_t medfilt_width,
+                                     float* row_stats, int dtype, void* stream);
+OASR_API int oasr_dtw_batched(const oasr_dtw_window* windows, int32_t n_windows, int32_t max_rows, void* stream);
 
 /* elementwise dtype conversion (weights fp32 -> T once per engine; bf16 encoder output / cross K,V -> fp16) */
 OASR_API int oasr_convert(const void* src, int src_dtype, void* dst, int dst_dtype, int64_t n, void* stream);

@@ -159,6 +159,9 @@ _SIGNATURES = {
     # word-level timestamps: heads table of oasr_align_head {q, k, ldq, ldk}
     "oasr_align_cost": [c_void_p, c_i32, c_i32, c_i32, c_i32, c_i32, c_void_p, c_void_p, c_i64, c_int, c_void_p],
     "oasr_dtw": [c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    # the same for many windows: device tables of oasr_align_window / oasr_dtw_window
+    "oasr_align_cost_batched": [c_void_p, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_void_p, c_int, c_void_p],
+    "oasr_dtw_batched": [c_void_p, c_i32, c_i32, c_void_p],
 }
 _RESTYPES = {"oasr_last_error": ctypes.c_char_p}
 
@@ -222,7 +225,7 @@ _LAUNCHES_PER_CALL = {"oasr_logmel": 3, "oasr_attention_bwd": 3, "oasr_dec_atten
                       "oasr_dec_sample_rules": 2, "oasr_dec_attention_grouped": 2, "oasr_dec_beam_select": 2,
                       "oasr_ce_fwd": 2, "oasr_colsum_bf16": 2, "oasr_layernorm_bwd": 3, "oasr_grad_sqnorm": 2,
                       "oasr_grad_sqnorm_flat": 2, "oasr_attention_bwd16": 3, "oasr_ce_fwd16": 2, "oasr_colsum16": 2,
-                      "oasr_layernorm_bwd16": 3, "oasr_align_cost": 2}
+                      "oasr_layernorm_bwd16": 3, "oasr_align_cost": 2, "oasr_align_cost_batched": 2}
 LAUNCH_COUNT = 0
 
 

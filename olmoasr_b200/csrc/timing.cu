@@ -1,6 +1,9 @@
 // Word-level timestamps: the cross-attention alignment matrix and its dynamic time warping (whisper/timing.py
 // find_alignment and dtw, restated in the header next to oasr_align_cost / oasr_dtw).
 //
+// Each kernel reads its window from a descriptor (oasr_align_window / oasr_dtw_window): one CTA grid dimension walks the
+// windows of a batched call, and a single-window call is the one-window case with the descriptor passed by value.
+//
 // Everything is fp32 after the 16-bit q / k are read.  Every sum has one fixed order (a thread's own loop, then
 // xor-butterfly shuffles, then a fixed block merge), there are no float atomics, so results are bit-identical from run
 // to run.
@@ -23,6 +26,14 @@ constexpr int KPAD = HD + 1;  // padded k / q rows (no bank conflicts on column 
 template <typename T>
 __device__ __forceinline__ float ld16(const T* p) { return Act16<T>::to_f(*p); }
 
+// The windows of a call: a device table, or (table == nullptr) the one window of a single-window entry point.
+template <typename W>
+struct Windows {
+  const W* table;
+  W one;
+  __device__ __forceinline__ W get(int i) const { return table ? table[i] : one; }
+};
+
 // QK value of one (row, frame): the dot product in d order, then the exact 1/8 = hd^-1/2 scale (qk_scale = 1).  Both
 // passes use this loop, so the row maxima of pass 1 are values pass 2 recomputes bit for bit.
 __device__ __forceinline__ float qk_dot(const float* q, const float* k) {
@@ -32,17 +43,21 @@ __device__ __forceinline__ float qk_dot(const float* q, const float* k) {
   return acc * 0.125f;
 }
 
-// grid (ceil(n_tok / RS_ROWS), n_heads), 256 threads: thread (r, c) owns rows r and r + 16 of the CTA's block and the
-// frames c, c + 16, c + 32, c + 48 of every tile; its online (max, sum-exp) pairs are merged over c by a butterfly.
+// grid (ceil(max n_tok / RS_ROWS), n_heads, n_windows), 256 threads: thread (r, c) owns rows r and r + 16 of the CTA's
+// block and the frames c, c + 16, c + 32, c + 48 of every tile; its online (max, sum-exp) pairs are merged over c by a
+// butterfly.
 template <typename T>
-__global__ void __launch_bounds__(256) align_rowstats_kernel(const oasr_align_head* heads, int n_tok, int n_frames,
-                                                             float* row_stats) {
+__global__ void __launch_bounds__(256) align_rowstats_kernel(Windows<oasr_align_window> windows, float* row_stats_base) {
   __shared__ float qs[RS_ROWS * KPAD];
   __shared__ float ks[RS_FR * KPAD];
-  const oasr_align_head hd = heads[blockIdx.y];
+  const oasr_align_window win = windows.get(blockIdx.z);
+  const int n_tok = win.n_tok, n_frames = win.n_frames;
+  const int row0 = blockIdx.x * RS_ROWS;
+  if (row0 >= n_tok) return;   // a shorter window of a batched call
+  float* row_stats = row_stats_base + win.row_stats;
+  const oasr_align_head hd = win.heads[blockIdx.y];
   const T* q = (const T*)hd.q;
   const T* k = (const T*)hd.k;
-  const int row0 = blockIdx.x * RS_ROWS;
   const int tid = threadIdx.x, r = tid >> 4, c = tid & 15;
   for (int i = tid; i < RS_ROWS * HD; i += 256) {
     const int rr = i / HD, d = i % HD;
@@ -116,13 +131,19 @@ __device__ __forceinline__ int reflect(int g, int n) {   // F.pad(mode="reflect"
   return g;
 }
 
-// grid ceil(n_frames / CT_F) CTAs; heads are processed one after the other in table order, so the head sum adds them
-// in ascending (layer, head) order for a table built that way.
+// grid (ceil(max n_frames / CT_F), n_windows) CTAs; heads are processed one after the other in table order, so the head
+// sum adds them in ascending (layer, head) order for a table built that way.
 template <typename T>
-__global__ void __launch_bounds__(CT_THREADS, 1) align_cost_kernel(const oasr_align_head* heads, int n_heads, int n_tok,
-                                                                int n_frames, int medfilt_width, const float* row_stats,
-                                                                float* cost, int64_t ld_cost) {
+__global__ void __launch_bounds__(CT_THREADS, 1) align_cost_kernel(Windows<oasr_align_window> windows, int n_heads,
+                                                                int medfilt_width, const float* row_stats_base) {
   extern __shared__ float sm[];
+  const oasr_align_window win = windows.get(blockIdx.y);
+  const int n_tok = win.n_tok, n_frames = win.n_frames;
+  if ((int)blockIdx.x * CT_F >= n_frames) return;   // a shorter window of a batched call
+  const oasr_align_head* heads = win.heads;
+  const float* row_stats = row_stats_base + win.row_stats;
+  float* cost = win.cost;
+  const int64_t ld_cost = win.ld_cost;
   float* P = sm;
   float* acc = P + (size_t)n_tok * CT_PLD;
   float* ks = acc + (size_t)(n_tok - 2) * CT_F;
@@ -225,13 +246,19 @@ __global__ void __launch_bounds__(CT_THREADS, 1) align_cost_kernel(const oasr_al
 }
 
 // ---- dynamic time warping ------------------------------------------------------------------------------------------
-// One CTA walks the anti-diagonals d = i + j of the (rows + 1) x (cols + 1) cost table; three diagonals live in shared
-// memory (indexed by i), the trace goes to global memory, then thread 0 backtracks.
+// One CTA per window walks the anti-diagonals d = i + j of the (rows + 1) x (cols + 1) cost table; three diagonals live
+// in shared memory (indexed by i), the trace goes to global memory, then thread 0 backtracks.
 constexpr int DTW_THREADS = 1024;
 
-__global__ void __launch_bounds__(DTW_THREADS) dtw_kernel(const float* x, int64_t ldx, int rows, int cols, uint8_t* trace,
-                                                           int32_t* text_idx, int32_t* time_idx, int32_t* path_len) {
+__global__ void __launch_bounds__(DTW_THREADS) dtw_kernel(Windows<oasr_dtw_window> windows) {
   extern __shared__ float diag[];   // 3 x (rows + 1)
+  const oasr_dtw_window win = windows.get(blockIdx.x);
+  const float* x = win.x;
+  const int64_t ldx = win.ldx;
+  const int rows = win.rows, cols = win.cols;
+  uint8_t* trace = win.trace;
+  int32_t* text_idx = win.text_idx;
+  int32_t* time_idx = win.time_idx;
   const int R = rows + 1;
   const int64_t tld = cols + 1;
   for (int i = threadIdx.x; i < 3 * R; i += DTW_THREADS) diag[i] = INFINITY;
@@ -278,7 +305,7 @@ __global__ void __launch_bounds__(DTW_THREADS) dtw_kernel(const float* x, int64_
         --j;
       }
     }
-    *path_len = n;
+    *win.path_len = n;
     diag[0] = __int_as_float(n);
   }
   __syncthreads();
@@ -294,37 +321,64 @@ __global__ void __launch_bounds__(DTW_THREADS) dtw_kernel(const float* x, int64_
 }
 
 template <typename T>
-int launch_align(const oasr_align_head* heads, int n_heads, int n_tok, int n_frames, int medfilt_width, float* row_stats,
-                 float* cost, int64_t ld_cost, cudaStream_t st) {
-  align_rowstats_kernel<T><<<dim3((unsigned)ceil_div(n_tok, RS_ROWS), (unsigned)n_heads), 256, 0, st>>>(heads, n_tok, n_frames,
-                                                                                                        row_stats);
+int launch_align(Windows<oasr_align_window> windows, int n_windows, int n_heads, int max_tok, int max_frames,
+                 int medfilt_width, float* row_stats, cudaStream_t st) {
+  const dim3 rs_grid((unsigned)ceil_div(max_tok, RS_ROWS), (unsigned)n_heads, (unsigned)n_windows);
+  align_rowstats_kernel<T><<<rs_grid, 256, 0, st>>>(windows, row_stats);
   OASR_LAUNCH_CHECK();
-  const size_t smem = cost_smem_floats(n_tok) * sizeof(float);
+  const size_t smem = cost_smem_floats(max_tok) * sizeof(float);
   OASR_CUDA_OK(cudaFuncSetAttribute(align_cost_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  align_cost_kernel<T><<<(unsigned)ceil_div(n_frames, CT_F), CT_THREADS, smem, st>>>(heads, n_heads, n_tok, n_frames,
-                                                                                   medfilt_width, row_stats, cost, ld_cost);
+  const dim3 ct_grid((unsigned)ceil_div(max_frames, CT_F), (unsigned)n_windows);
+  align_cost_kernel<T><<<ct_grid, CT_THREADS, smem, st>>>(windows, n_heads, medfilt_width, row_stats);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
+
+int launch_dtw(Windows<oasr_dtw_window> windows, int n_windows, int max_rows, cudaStream_t st) {
+  const size_t smem = (size_t)3 * (max_rows + 1) * sizeof(float);
+  if (smem > 48 * 1024) OASR_CUDA_OK(cudaFuncSetAttribute(dtw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  dtw_kernel<<<(unsigned)n_windows, DTW_THREADS, smem, st>>>(windows);
+  OASR_LAUNCH_CHECK();
+  return OASR_OK;
+}
+
+constexpr int DTW_MAX_ROWS = (int)(200 * 1024 / 12) - 1;   // three diagonals of rows + 1 floats in 200 KB
+constexpr int MAX_WINDOWS = 65535;                          // the grid dimension that walks the windows
 
 }  // namespace
 }  // namespace oasr
 
 using namespace oasr;
 
+#define OASR_REQUIRE_ALIGN_SHAPE(n_heads, head_dim, n_tok, n_frames, medfilt_width)                                      \
+  OASR_REQUIRE(head_dim == HD, "align_cost: head_dim must be %d (got %d)", HD, head_dim);                               \
+  OASR_REQUIRE(n_heads >= 1, "align_cost: need at least one head (got %d)", n_heads);                                  \
+  OASR_REQUIRE(n_tok >= 3 && n_tok <= ALIGN_MAX_TOK, "align_cost: 3 <= n_tok <= %d (got %d)", ALIGN_MAX_TOK, n_tok);   \
+  OASR_REQUIRE(n_frames >= 1 && n_frames <= 1500, "align_cost: 1 <= n_frames <= 1500 (got %d)", n_frames);             \
+  OASR_REQUIRE(medfilt_width >= 1 && medfilt_width <= MAX_MEDFILT && (medfilt_width & 1),                              \
+               "align_cost: medfilt_width must be odd and <= %d (got %d)", MAX_MEDFILT, medfilt_width)
+
 extern "C" int oasr_align_cost(const oasr_align_head* heads, int32_t n_heads, int32_t head_dim, int32_t n_tok,
                                int32_t n_frames, int32_t medfilt_width, float* row_stats, float* cost, int64_t ld_cost,
                                int dtype, void* stream) {
   OASR_REQUIRE(heads && row_stats && cost, "align_cost: null tensor");
-  OASR_REQUIRE(head_dim == HD, "align_cost: head_dim must be %d (got %d)", HD, head_dim);
-  OASR_REQUIRE(n_heads >= 1, "align_cost: need at least one head (got %d)", n_heads);
-  OASR_REQUIRE(n_tok >= 3 && n_tok <= ALIGN_MAX_TOK, "align_cost: 3 <= n_tok <= %d (got %d)", ALIGN_MAX_TOK, n_tok);
-  OASR_REQUIRE(n_frames >= 1 && n_frames <= 1500, "align_cost: 1 <= n_frames <= 1500 (got %d)", n_frames);
-  OASR_REQUIRE(medfilt_width >= 1 && medfilt_width <= MAX_MEDFILT && (medfilt_width & 1),
-               "align_cost: medfilt_width must be odd and <= %d (got %d)", MAX_MEDFILT, medfilt_width);
+  OASR_REQUIRE_ALIGN_SHAPE(n_heads, head_dim, n_tok, n_frames, medfilt_width);
   OASR_REQUIRE(ld_cost >= n_frames, "align_cost: ld_cost < n_frames");
-  cudaStream_t st = (cudaStream_t)stream;
-  return OASR_BY_DTYPE16(dtype, launch_align, heads, n_heads, n_tok, n_frames, medfilt_width, row_stats, cost, ld_cost, st);
+  Windows<oasr_align_window> one{nullptr, {heads, cost, ld_cost, 0, n_tok, n_frames}};
+  return OASR_BY_DTYPE16(dtype, launch_align, one, 1, n_heads, n_tok, n_frames, medfilt_width, row_stats,
+                         (cudaStream_t)stream);
+}
+
+extern "C" int oasr_align_cost_batched(const oasr_align_window* windows, int32_t n_windows, int32_t n_heads,
+                                       int32_t head_dim, int32_t max_tok, int32_t max_frames, int32_t medfilt_width,
+                                       float* row_stats, int dtype, void* stream) {
+  OASR_REQUIRE(windows && row_stats, "align_cost_batched: null tensor");
+  OASR_REQUIRE(n_windows >= 1 && n_windows <= MAX_WINDOWS, "align_cost_batched: 1 <= n_windows <= %d (got %d)",
+               MAX_WINDOWS, n_windows);
+  OASR_REQUIRE_ALIGN_SHAPE(n_heads, head_dim, max_tok, max_frames, medfilt_width);
+  Windows<oasr_align_window> table{windows, {}};
+  return OASR_BY_DTYPE16(dtype, launch_align, table, n_windows, n_heads, max_tok, max_frames, medfilt_width, row_stats,
+                         (cudaStream_t)stream);
 }
 
 extern "C" int oasr_dtw(const float* x, int64_t ldx, int32_t rows, int32_t cols, uint8_t* trace, int32_t* text_idx,
@@ -332,10 +386,16 @@ extern "C" int oasr_dtw(const float* x, int64_t ldx, int32_t rows, int32_t cols,
   OASR_REQUIRE(x && trace && text_idx && time_idx && path_len, "dtw: null tensor");
   OASR_REQUIRE(rows >= 1 && cols >= 1, "dtw: empty matrix (%d x %d)", rows, cols);
   OASR_REQUIRE(ldx >= cols, "dtw: ldx < cols");
-  const size_t smem = (size_t)3 * (rows + 1) * sizeof(float);
-  OASR_REQUIRE(smem <= 200 * 1024, "dtw: rows <= %d (got %d)", (int)(200 * 1024 / 12) - 1, rows);
-  if (smem > 48 * 1024) OASR_CUDA_OK(cudaFuncSetAttribute(dtw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  dtw_kernel<<<1, DTW_THREADS, smem, (cudaStream_t)stream>>>(x, ldx, rows, cols, trace, text_idx, time_idx, path_len);
-  OASR_LAUNCH_CHECK();
-  return OASR_OK;
+  OASR_REQUIRE(rows <= DTW_MAX_ROWS, "dtw: rows <= %d (got %d)", DTW_MAX_ROWS, rows);
+  Windows<oasr_dtw_window> one{nullptr, {x, ldx, trace, text_idx, time_idx, path_len, rows, cols}};
+  return launch_dtw(one, 1, rows, (cudaStream_t)stream);
+}
+
+extern "C" int oasr_dtw_batched(const oasr_dtw_window* windows, int32_t n_windows, int32_t max_rows, void* stream) {
+  OASR_REQUIRE(windows, "dtw_batched: null tensor");
+  OASR_REQUIRE(n_windows >= 1 && n_windows <= MAX_WINDOWS, "dtw_batched: 1 <= n_windows <= %d (got %d)", MAX_WINDOWS,
+               n_windows);
+  OASR_REQUIRE(max_rows >= 1 && max_rows <= DTW_MAX_ROWS, "dtw_batched: 1 <= max_rows <= %d (got %d)", DTW_MAX_ROWS,
+               max_rows);
+  return launch_dtw(Windows<oasr_dtw_window>{windows, {}}, n_windows, max_rows, (cudaStream_t)stream);
 }

@@ -28,6 +28,7 @@ cases (their bf16 outputs are converted to fp16 for an fp16 decoder).
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import math
 from typing import Dict, Optional, Sequence, Tuple
@@ -62,6 +63,13 @@ def sample_row_key(seed: int, clip: int, sample: int) -> int:
     """The 64-bit Philox key of sample `sample` of clip `clip` (counted over the whole decode() call) under `seed`: a
     clip's draws do not depend on how the call is split into engine batches."""
     return _mix64(_mix64(_mix64(seed & _M64) ^ clip) ^ sample)
+
+
+def window_clip_id(recording: int, seek: int, temperature_index: int) -> int:
+    """The clip id of one transcribe_batch() window (passed to `DecodeEngine.sample` as `clip_ids`): the recording's
+    index in the call, the window's seek frame and the temperature's index in the fallback tuple, mixed like
+    `sample_row_key`, so a window's draws do not depend on which windows share its engine call."""
+    return _mix64(_mix64(_mix64(recording & _M64) ^ (seek & _M64)) ^ (temperature_index & _M64))
 
 
 def _convert(src: Tensor, dst: Tensor) -> Tensor:
@@ -131,6 +139,7 @@ class DecodeEngine:
         self._w_sig = None
         self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}
         self._sample_cfg = None
+        self.split_rows: Optional[int] = None   # see splits_of()
         self.launches_per_step = 0
 
     # ---- weights ----------------------------------------------------------------------------------------------
@@ -210,6 +219,17 @@ class DecodeEngine:
         """Key-range splits of the cross-attention so that n x H x splits CTAs cover the SMs about twice."""
         return max(1, min(self.max_splits, math.ceil(2 * _lib.lib().oasr_device_sm_count() / (n * self.H))))
 
+    @contextlib.contextmanager
+    def splits_of(self, rows: int):
+        """Inside, every step splits the cross-attention key range as a step of `rows` rows would, whatever its row count.
+        The fp32 partial sums of a sequence then group alike in calls of any size, so its logits have the same bits
+        alone and inside a batch (transcribe_batch() windows equal transcribe()'s)."""
+        prev, self.split_rows = self.split_rows, rows
+        try:
+            yield
+        finally:
+            self.split_rows = prev
+
     def _enqueue_step(self, n: int):
         """One decoder step for sequences [0, n): per layer 6 fused Linear launches, 1 self-attention launch and 1 (unsplit key
         range) or 2 (split) cross-attention launches; plus the embedding, the logits head and the 2 sampling launches."""
@@ -217,7 +237,7 @@ class DecodeEngine:
         c0 = _lib.LAUNCH_COUNT
         call("oasr_dec_embed", ptr(self.tokens), self.tokens.stride(0), ptr(self.pos), ptr(w["emb"]), ptr(w["pos"]), ptr(self.x),
              n, d, self.V, self.dt, stream())
-        sc = self.cross_splits(n)
+        sc = self.cross_splits(self.split_rows or n)
         seq_self, seq_cross = self.n_ctx * d, self.n_audio_ctx * 2 * d
         x, q, h = self.x[:n], self.q[:n], self.h[:n]
         # the attention kernels lay their fp32 partial outputs out as (splits, n, d): views with exactly that geometry
@@ -273,7 +293,7 @@ class DecodeEngine:
         call("oasr_dec_sample_rules", ctypes.byref(s), stream())
 
     def _graph(self, n: int) -> torch.cuda.CUDAGraph:
-        key = (n, self._sample_cfg, self._beam_cfg, self._rules_cfg, self._group)
+        key = (n, self._sample_cfg, self._beam_cfg, self._rules_cfg, self._group, self.split_rows)
         g = self._graphs.get(key)
         if g is None:
             # one eager run first (kernel modules are loaded lazily on first launch, which must not happen under capture),
@@ -384,10 +404,11 @@ class DecodeEngine:
     def sample(self, audio_features: Tensor, initial_tokens: Sequence[int], sample_len: int, temperature: float,
                best_of: int = 1, seed: int = 0, clip_offset: int = 0, suppress: Sequence[int] = (), suppress_blank: bool = True,
                sot_index: int = 0, timestamps: bool = False, max_initial_timestamp_index: Optional[int] = None,
-               blank: int = 220, eot: int = 50256, no_speech: int = 50361, check_every: int = 8):
+               blank: int = 220, eot: int = 50256, no_speech: int = 50361, check_every: int = 8,
+               clip_ids: Optional[Sequence[int]] = None):
         """Temperature sampling with `best_of` samples per clip (DecodingTask._main_loop with GreedyDecoder at temperature
         > 0, and ApplyTimestampRules when `timestamps`).  Row c * best_of + j draws with the key sample_row_key(seed,
-        clip_offset + c, j).  Cross K/V is projected once per clip and shared by its samples.  Returns (candidates,
+        clip_offset + c, j), or sample_row_key(seed, clip_ids[c], j) when `clip_ids` (one per clip) are given.  Cross K/V is projected once per clip and shared by its samples.  Returns (candidates,
         no_speech_probs (n_clips,), number of graph replays): candidates[c] is the list of best_of (token ids incl. the
         initial tokens and the final eot, sum_logprob), as `beam_search` returns them."""
         G = int(best_of)
@@ -406,7 +427,10 @@ class DecodeEngine:
         mi = -1 if max_initial_timestamp_index is None else int(max_initial_timestamp_index)
         self._rules_cfg = (int(bool(timestamps)), mi, 1)
         self._group = G
-        keys = [sample_row_key(seed, clip_offset + c, j) for c in range(C) for j in range(G)]
+        if clip_ids is not None and len(clip_ids) != C:
+            raise ValueError(f"sample: {len(clip_ids)} clip ids for {C} clips")
+        ids = list(clip_ids) if clip_ids is not None else [clip_offset + c for c in range(C)]
+        keys = [sample_row_key(seed, ids[c], j) for c in range(C) for j in range(G)]
         self.row_keys[:n] = torch.tensor([k - (1 << 64) if k >> 63 else k for k in keys], dtype=torch.int64)
         self.temperature.fill_(float(temperature))
         toks, lps, nsp, replays = self._run(n, n_init, sample_len, check_every)

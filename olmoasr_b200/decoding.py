@@ -31,6 +31,7 @@ from torch import Tensor
 if TYPE_CHECKING:
     from ._core import OLMoASRBase
 
+import contextlib
 import os
 
 # OASR_DECODE_ENGINE=0 forces the generic hook-based loop below for every configuration (A/B runs, debugging)
@@ -198,13 +199,22 @@ class DecodingTask:
             self.ts_rules = _TimestampRules(self.sample_begin, mi)
 
     @torch.no_grad()
-    def run(self, mel: Tensor, tokenizer=None) -> List[DecodingResult]:
+    def run(self, mel: Tensor, tokenizer=None, sample_keys: Optional[Tuple[int, List[int]]] = None) -> List[DecodingResult]:
+        """`sample_keys` = (seed, one clip id per clip) replaces the per-call seed and the clips' indices in the sampling
+        keys of the device decoder, and its steps split the cross-attention as a one-clip call does (transcribe_batch():
+        a window's draws and bits then do not depend on the other windows of its call).  The hook loop
+        (OASR_DECODE_ENGINE=0) draws from torch's generator and makes no such promise."""
         from ._core import bf16_compute
 
-        with bf16_compute():     # decoding computes in bf16 / its engine's type, also inside an fp16 autocast region
-            return self._run(mel, tokenizer)
+        with bf16_compute(), self._window_splits(sample_keys):   # bf16 / the engine's type, also inside fp16 autocast
+            return self._run(mel, tokenizer, sample_keys)
 
-    def _run(self, mel: Tensor, tokenizer=None) -> List[DecodingResult]:
+    def _window_splits(self, sample_keys):
+        if sample_keys is None or not (USE_ENGINE and hasattr(self.model, "decode_engine")):
+            return contextlib.nullcontext()
+        return self.model.decode_engine(torch.float16 if self.options.fp16 else torch.bfloat16).splits_of(self.n_group)
+
+    def _run(self, mel: Tensor, tokenizer=None, sample_keys=None) -> List[DecodingResult]:
         model, opt = self.model, self.options
         if mel.shape[-2:] == (model.dims.n_audio_ctx, model.dims.n_audio_state):
             audio_features = mel  # encoded features were passed in (DecodingTask._get_audio_features)
@@ -219,7 +229,7 @@ class DecodingTask:
             if opt.temperature == 0:
                 return self._run_on_device(audio_features, tokenizer, eng)
             if self.n_group <= eng.max_batch:
-                return self._run_sampling_on_device(audio_features, tokenizer, eng)
+                return self._run_sampling_on_device(audio_features, tokenizer, eng, sample_keys)
         G = self.n_group                           # best_of samples per clip (temperature > 0), rows clip-major
         xa = audio_features.repeat_interleave(G, dim=0) if G > 1 else audio_features
         n_rows = n_audio * G
@@ -303,19 +313,22 @@ class DecodingTask:
                                           temperature=opt.temperature))
         return results
 
-    def _run_sampling_on_device(self, audio_features: Tensor, tokenizer, eng):
+    def _run_sampling_on_device(self, audio_features: Tensor, tokenizer, eng, sample_keys=None):
         """Temperature sampling, best_of samples per clip (every fallback temperature of transcribe()), on the device
         decoder: up to max_batch // best_of clips per call, ranked like the hook loop.  One seed per decode() call from
-        torch's default generator; each clip's draws depend on it and on the clip's index in this call only."""
+        torch's default generator; each clip's draws depend on it and on the clip's index in this call only.  With
+        `sample_keys` = (seed, clip ids) the given seed and each clip's own id key the draws instead."""
         opt, G = self.options, self.n_group
         per = eng.max_batch // G
         ts = self.ts_rules is not None
         mi = self.ts_rules.max_initial_timestamp_index if ts else None
-        seed = int(torch.randint(2 ** 62, (1,)))
+        seed = int(torch.randint(2 ** 62, (1,))) if sample_keys is None else sample_keys[0]
         candidates, nsp = [], []
         for s in range(0, audio_features.shape[0], per):
+            ids = {} if sample_keys is None else dict(clip_ids=list(sample_keys[1][s:s + per]))
             c, ns, _ = eng.sample(audio_features[s:s + per], self.initial_tokens, self.sample_len, opt.temperature, G, seed, s,
-                                  self.suppress, opt.suppress_blank, self.sot_index, timestamps=ts, max_initial_timestamp_index=mi)
+                                  self.suppress, opt.suppress_blank, self.sot_index, timestamps=ts, max_initial_timestamp_index=mi,
+                                  **ids)
             candidates += c
             nsp += ns.tolist()
         return self._ranked(audio_features, candidates, nsp, tokenizer)
@@ -363,6 +376,14 @@ def decode(model: "OLMoASRBase", mel: Tensor, options: DecodingOptions = Decodin
         options = replace(options, **kwargs)
     result = DecodingTask(model, options).run(mel, tokenizer)
     return result[0] if single else result
+
+
+@torch.no_grad()
+def decode_windows(model: "OLMoASRBase", features: Tensor, options: DecodingOptions, tokenizer=None,
+                   sample_keys: Optional[Tuple[int, List[int]]] = None) -> List[DecodingResult]:
+    """decode() of (W, n_audio_ctx, n_audio_state) encoded features with per-window sampling keys (see
+    `DecodingTask.run`): the route of transcribe_batch()."""
+    return DecodingTask(model, options).run(features, tokenizer, sample_keys)
 
 
 @torch.no_grad()

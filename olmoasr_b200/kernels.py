@@ -330,3 +330,85 @@ def dtw(x):
     length = torch.empty(1, device=x.device, dtype=torch.int32)
     call("oasr_dtw", ptr(x), x.stride(0), rows, cols, ptr(trace), ptr(path[0]), ptr(path[1]), ptr(length), stream())
     return path, length
+
+
+def _device_table(dev, fill):
+    """An int64 device table whose entries may hold addresses inside itself: `fill(base)` gets the table's device address
+    and returns its host rows; one host-to-device copy."""
+    rows = fill(0)
+    table = torch.empty(sum(len(r) for r in rows), device=dev, dtype=torch.int64)
+    host = torch.tensor([v for r in fill(table.data_ptr()) for v in r], dtype=torch.int64)
+    table.copy_(host, non_blocking=True)
+    return table
+
+
+def align_cost_batched(windows, medfilt_width=7):
+    """`align_cost` for many windows in one oasr_align_cost_batched call: `windows` lists (heads, n_frames), each as
+    `align_cost` takes them, with the same number of heads and one 16-bit type throughout.  Returns one cost
+    (n_tok - 2, n_frames) fp32 per window, bit-identical to `align_cost` on the same inputs (views of one buffer)."""
+    _req(len(windows) >= 1, "align_cost_batched: need at least one window")
+    n_heads = len(windows[0][0])
+    _req(n_heads >= 1, "align_cost_batched: need at least one head")
+    dt, dev = windows[0][0][0][0].dtype, windows[0][0][0][0].device
+    shapes = []
+    for heads, n_frames in windows:
+        _req(len(heads) == n_heads, "align_cost_batched: every window has the same number of heads")
+        n_tok = heads[0][0].shape[0]
+        for q, k in heads:
+            _req(q.is_cuda and k.is_cuda and q.dtype == dt and k.dtype == dt and dt in ACT16,
+                 "align_cost_batched: q and k must be CUDA tensors of one 16-bit type")
+            _req(q.dim() == 2 and k.dim() == 2 and q.shape == (n_tok, 64) and k.shape[1] == 64 and k.shape[0] >= n_frames,
+                 "align_cost_batched: q (n_tok, 64) and k (>= n_frames, 64) per head")
+            _req(q.stride(1) == 1 and k.stride(1) == 1, "align_cost_batched: unit inner stride")
+        _req(3 <= n_tok <= 448 and 1 <= n_frames <= 1500, "align_cost_batched: 3 <= n_tok <= 448, 1 <= n_frames <= 1500")
+        shapes.append((n_tok, n_frames))
+    cost_off = [0]
+    stats_off = [0]
+    for n_tok, n_frames in shapes:
+        cost_off.append(cost_off[-1] + (n_tok - 2) * n_frames)
+        stats_off.append(stats_off[-1] + n_heads * n_tok * 2)
+    cost = torch.empty(cost_off[-1], device=dev, dtype=torch.float32)
+    stats = torch.empty(stats_off[-1], device=dev, dtype=torch.float32)
+    n_w = len(windows)
+    head_rows = [[q.data_ptr(), k.data_ptr(), q.stride(0), k.stride(0)] for heads, _ in windows for q, k in heads]
+
+    def fill(base):      # n_w * n_heads oasr_align_head entries (4 int64), then n_w oasr_align_window entries (5 int64)
+        rows = list(head_rows)
+        for w, (n_tok, n_frames) in enumerate(shapes):
+            rows.append([base + 32 * w * n_heads, cost.data_ptr() + 4 * cost_off[w], n_frames, stats_off[w],
+                         n_tok | (n_frames << 32)])
+        return rows
+
+    table = _device_table(dev, fill)
+    max_tok, max_frames = max(s[0] for s in shapes), max(s[1] for s in shapes)
+    call("oasr_align_cost_batched", ptr(table) + 32 * n_w * n_heads, n_w, n_heads, 64, max_tok, max_frames, medfilt_width,
+         ptr(stats), _DTYPE_CODE[dt], stream())
+    return [cost[cost_off[w]:cost_off[w + 1]].view(n_tok - 2, n_frames) for w, (n_tok, n_frames) in enumerate(shapes)]
+
+
+def dtw_batched(xs):
+    """`dtw` for many matrices in one oasr_dtw_batched call (one CTA each).  Returns (paths, lengths): paths (n, 2, max
+    rows + cols) int32 whose window w holds its path in the first lengths[w] columns, lengths (n,) int32, both on the
+    device and bit-identical to `dtw` on each matrix."""
+    _req(len(xs) >= 1, "dtw_batched: need at least one matrix")
+    dev = xs[0].device
+    for x in xs:
+        _req(x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1,
+             "dtw_batched: 2-D fp32 CUDA matrices, unit inner stride")
+        _req(x.shape[0] >= 1 and x.shape[1] >= 1, "dtw_batched: empty matrix")
+    n = len(xs)
+    width = max(x.shape[0] + x.shape[1] for x in xs)
+    trace_off = [0]
+    for x in xs:
+        trace_off.append(trace_off[-1] + (x.shape[0] + 1) * (x.shape[1] + 1))
+    trace = torch.empty(trace_off[-1], device=dev, dtype=torch.uint8)
+    paths = torch.empty((n, 2, width), device=dev, dtype=torch.int32)
+    lengths = torch.empty(n, device=dev, dtype=torch.int32)
+
+    def fill(_base):     # oasr_dtw_window: x, ldx, trace, text_idx, time_idx, path_len, rows | cols << 32
+        return [[x.data_ptr(), x.stride(0), trace.data_ptr() + trace_off[w], paths[w, 0].data_ptr(), paths[w, 1].data_ptr(),
+                 lengths[w:].data_ptr(), x.shape[0] | (x.shape[1] << 32)] for w, x in enumerate(xs)]
+
+    table = _device_table(dev, fill)
+    call("oasr_dtw_batched", ptr(table), n, max(x.shape[0] for x in xs), stream())
+    return paths, lengths

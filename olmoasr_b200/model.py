@@ -25,6 +25,10 @@ class OLMoASR(OLMoASRBase):
         from .transcribe import transcribe as transcribe_function
         return transcribe_function(self, audio, **kwargs)
 
+    def transcribe_batch(self, audios, **kwargs):
+        from .transcribe import transcribe_batch as transcribe_batch_function
+        return transcribe_batch_function(self, audios, **kwargs)
+
 
 __all__ = ["LayerNorm", "Linear", "Conv1d", "sinusoids", "MultiHeadAttention", "ResidualAttentionBlock", "AudioEncoder",
            "TextDecoder", "OLMoASR", "ModelDimensions"]

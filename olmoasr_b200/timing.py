@@ -39,9 +39,11 @@ class WordTiming:
 
 
 # ---- device part ---------------------------------------------------------------------------------------------------
-def alignment_cost(model, text_tokens: List[int], mel: torch.Tensor, num_frames: int, medfilt_width: int = 7):
-    """Steps 1-2 for one window: (cost (n_text + 1, num_frames // 2) fp32, text-token probabilities (n_text,) fp32),
-    both on the device.  `mel` is a mel segment (n_mels, 3000) or encoded features (n_audio_ctx, n_audio_state)."""
+def alignment_forward(model, text_tokens: List[int], mel: torch.Tensor, num_frames: int):
+    """Step 1 for one window: the decoder forward over [SOT, NO_TIMESTAMPS, *text_tokens, EOT].  Returns (pairs,
+    text-token probabilities (n_text,) fp32): pairs lists the alignment heads' (query rows (n_tok, 64), cross keys
+    (1500, 64)) 16-bit column slices in ascending (layer, head) order, as `kernels.align_cost` takes them.  `mel` is a mel
+    segment (n_mels, 3000) or encoded features (n_audio_ctx, n_audio_state)."""
     dims = model.dims
     n_frames = num_frames // 2
     if not 1 <= n_frames <= dims.n_audio_ctx:
@@ -66,14 +68,26 @@ def alignment_cost(model, text_tokens: List[int], mel: torch.Tensor, num_frames:
             hd = dims.n_text_state // dims.n_text_head
             pairs = [(queries[l][0][:, h * hd:(h + 1) * hd], cache[blocks[l].cross_attn.key][0][:, h * hd:(h + 1) * hd])
                      for l, h in heads]
-            cost = K.align_cost(pairs, n_frames, medfilt_width)
             n_text = len(text_tokens)
             probs = logits[1:n_text + 1, :EOT].float().softmax(dim=-1)
             text_probs = probs[torch.arange(n_text, device=dev), tokens[2:2 + n_text]]
     finally:
         for h in hooks + kv_hooks:
             h.remove()
-    return cost, text_probs
+    return pairs, text_probs
+
+
+def alignment_cost(model, text_tokens: List[int], mel: torch.Tensor, num_frames: int, medfilt_width: int = 7):
+    """Steps 1-2 for one window: (cost (n_text + 1, num_frames // 2) fp32, text-token probabilities (n_text,) fp32),
+    both on the device.  `mel` is a mel segment (n_mels, 3000) or encoded features (n_audio_ctx, n_audio_state)."""
+    pairs, text_probs = alignment_forward(model, text_tokens, mel, num_frames)
+    return K.align_cost(pairs, num_frames // 2, medfilt_width), text_probs
+
+
+def _split_host_path(host: np.ndarray, width: int):
+    """(text_indices, time_indices) of one window's [length, text_idx (width), time_idx (width)] as copied to the host."""
+    n = int(host[0])
+    return host[1:1 + n].astype(np.int64), host[1 + width:1 + width + n].astype(np.int64)
 
 
 def _device_alignment(model, text_tokens: List[int], mel: torch.Tensor, num_frames: int, medfilt_width: int = 7):
@@ -81,10 +95,30 @@ def _device_alignment(model, text_tokens: List[int], mel: torch.Tensor, num_fram
     cost, probs = alignment_cost(model, text_tokens, mel, num_frames, medfilt_width)
     path, length = K.dtw(cost)
     host = torch.cat([length.float(), path.flatten().float(), probs]).cpu().numpy()
-    n, width = int(host[0]), path.shape[1]
-    text_indices = host[1:1 + n].astype(np.int64)
-    time_indices = host[1 + width:1 + width + n].astype(np.int64)
+    width = path.shape[1]
+    text_indices, time_indices = _split_host_path(host, width)
     return text_indices, time_indices, host[1 + 2 * width:].astype(np.float64).tolist()
+
+
+def device_alignments(model, windows, medfilt_width: int = 7):
+    """Steps 1-3 for many windows (a transcribe_batch() round): `windows` lists (text_tokens, mel or encoded features,
+    num_frames), each with at least one text token.  The per-window decoder forwards run one after the other (the code
+    of `alignment_cost`), then one oasr_align_cost_batched and one oasr_dtw_batched call cover every window, and one copy
+    brings every path and probability to the host.  Returns (text_indices, time_indices, probabilities) per window, equal
+    to `_device_alignment` of each window."""
+    forwards = [alignment_forward(model, list(text), mel, num_frames) for text, mel, num_frames in windows]
+    costs = K.align_cost_batched([(pairs, num_frames // 2) for (pairs, _), (_, _, num_frames) in zip(forwards, windows)],
+                                 medfilt_width)
+    paths, lengths = K.dtw_batched(costs)
+    n, width = paths.shape[0], paths.shape[2]
+    flat = torch.cat([lengths.float()[:, None], paths.view(n, 2 * width).float()], dim=1).flatten()
+    host = torch.cat([flat] + [probs for _, probs in forwards]).cpu().numpy()
+    out, at = [], n * (1 + 2 * width)
+    for w, (text, _, _) in enumerate(windows):
+        text_indices, time_indices = _split_host_path(host[w * (1 + 2 * width):], width)
+        out.append((text_indices, time_indices, host[at:at + len(text)].astype(np.float64).tolist()))
+        at += len(text)
+    return out
 
 
 # ---- host part -----------------------------------------------------------------------------------------------------
@@ -190,6 +224,10 @@ def merge_punctuations(alignment: List[WordTiming], prepended: str, appended: st
         j += 1
 
 
+def segment_text_tokens(segments: List[dict]) -> List[List[int]]:
+    return [[token for token in segment["tokens"] if token < EOT] for segment in segments]
+
+
 def add_word_timestamps(*, segments: List[dict], model, tokenizer, mel: torch.Tensor, num_frames: int,
                         prepend_punctuations: str = "\"'“¿([{-", append_punctuations: str = "\"'.。,，!！?？:：”)]}、",
                         last_speech_timestamp: float, **kwargs):
@@ -197,9 +235,16 @@ def add_word_timestamps(*, segments: List[dict], model, tokenizer, mel: torch.Te
     start / end in place."""
     if len(segments) == 0:
         return
-    text_tokens_per_segment = [[token for token in segment["tokens"] if token < EOT] for segment in segments]
-    text_tokens = list(itertools.chain.from_iterable(text_tokens_per_segment))
+    text_tokens = list(itertools.chain.from_iterable(segment_text_tokens(segments)))
     alignment = find_alignment(model, tokenizer, text_tokens, mel, num_frames, **kwargs)
+    apply_word_timings(segments, alignment, prepend_punctuations=prepend_punctuations,
+                       append_punctuations=append_punctuations, last_speech_timestamp=last_speech_timestamp)
+
+
+def apply_word_timings(segments: List[dict], alignment: List[WordTiming], *, prepend_punctuations: str,
+                       append_punctuations: str, last_speech_timestamp: float):
+    """The part of add_word_timestamps after find_alignment: durations, punctuation and the segments' words."""
+    text_tokens_per_segment = segment_text_tokens(segments)
     word_durations = np.array([t.end - t.start for t in alignment])
     word_durations = word_durations[word_durations.nonzero()]
     median_duration = np.median(word_durations) if len(word_durations) > 0 else 0.0

@@ -68,6 +68,16 @@ def main():
         eng.sample(xa, [50257, 50362], 4, 0.6, best_of=5, seed=1, suppress=(7, 9))
         eng.sample(xa[:2], [50257], 4, 1.0, best_of=3, seed=2, clip_offset=5, suppress=(7, 9), timestamps=True,
                    max_initial_timestamp_index=50)
+    # word alignment: single-window and batched cost and DTW over ragged windows (edge tiles, one frame, 448 tokens)
+    for dtype in (torch.float16, torch.bfloat16):
+        windows = []
+        for n_tok, n_frames in ((3, 1), (448, 37), (37, 750), (5, 3)):
+            q, k = torch.randn(n_tok, 128, device=dev).to(dtype), torch.randn(800, 128, device=dev).to(dtype)
+            windows.append(([(q[:, :64], k[:, :64]), (q[:, 64:], k[:, 64:])], n_frames))
+        K.align_cost(*windows[1])
+        costs = K.align_cost_batched(windows)
+    K.dtw(costs[2])
+    K.dtw_batched([costs[1], costs[2], costs[3], torch.randn(1, 1, device=dev), torch.randn(9, 1, device=dev)])
     torch.cuda.synchronize()
     print("sanitize run complete; loss", float(loss))
 
