@@ -98,7 +98,9 @@ OASR_API int oasr_layernorm_bwd(const void* dy, const void* x, const float* weig
  * Replaces F.scaled_dot_product_attention in MultiHeadAttention.forward (olmoasr/model.py:331-340) and its
  * autograd.  q: (B*Tq, ldq) bf16 with head h at columns [64h, 64h+64); k, v: (B*Tkv, ld*) likewise; o like q.
  * causal != 0 applies key <= query; kv_len (B,) int32 (nullable) hides keys >= kv_len[b] -- together they are
- * the reference's `padding_mask + causal mask` (model.py:740-743, train_timestamps.py:314-315).
+ * the reference's `padding_mask + causal mask` (model.py:740-743, train_timestamps.py:314-315).  kv_len[b] is clamped
+ * to [1, Tkv]: a sample with kv_len[b] <= 0 sees key 0 alone (no softmax row is ever empty), one with kv_len[b] > Tkv
+ * sees every key.
  * lse: (B,H,Tq) f32, log2 domain: log2(sum_k 2^(s_k * scale * log2 e)).
  * Backward: delta (B,H,Tq) f32 is scratch. */
 OASR_API int oasr_attention_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,

@@ -463,6 +463,8 @@ int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const 
   OASR_REQUIRE((reinterpret_cast<uintptr_t>(dq) & 3) == 0 && (reinterpret_cast<uintptr_t>(dk) & 3) == 0 &&
                    (reinterpret_cast<uintptr_t>(dv) & 3) == 0,
                "attention_bwd: dQ / dK / dV must be 4-byte aligned");
+  // attention_delta_kernel reads O with 16-byte loads; dO is checked by its TMA descriptor
+  OASR_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0, "attention_bwd: O must be 16-byte aligned");
   OASR_REQUIRE(!causal || Tq == Tkv, "attention_bwd: causal needs Tq == Tkv");
   OASR_REQUIRE(B <= 65535 && H <= 65535, "attention_bwd: B and H must fit the grid");
   cudaStream_t st = (cudaStream_t)stream;

@@ -29,6 +29,22 @@ def main():
     # mask -> key counts
     _, _, pm, _ = synth.text_batch(3)
     _core.kv_len_from_padding_mask(pm.to(dev))
+    # attention forward / backward at the mask edges, both dtypes: ragged T, kv_len on and next to the 64-query / 128-key
+    # tile edges (the backward's all-visible fast paths switch there), kv_len clamps, strided inputs and outputs
+    for dtype in (torch.bfloat16, torch.float16):
+        for B, T, Tkv, causal, lens in ((2, 65, 65, True, [65, 1]), (1, 191, 383, False, None),
+                                        (6, 257, 257, True, [0, 63, 64, 128, 129, 300]), (2, 129, 300, False, [256, 257])):
+            H, d = 2, 128
+            qkv = torch.randn(B * T, 3 * d, device=dev).to(dtype)
+            kv = torch.randn(B * Tkv, 2 * d, device=dev).to(dtype)
+            q, k, v = (qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:]) if causal else (qkv[:, :d], kv[:, :d], kv[:, d:])
+            kv_len = torch.tensor(lens, device=dev, dtype=torch.int32) if lens else None
+            obuf = torch.zeros(B * T + 1, d + 64, device=dev, dtype=dtype)
+            o, lse = K.attention_fwd(q, k, v, B, H, T, Tkv, causal=causal, kv_len=kv_len, out=obuf[1:, 64:])
+            gq = torch.zeros(B * T + 1, d + 64, device=dev, dtype=dtype)
+            gkv = torch.zeros(B * Tkv + 1, 2 * d + 64, device=dev, dtype=dtype)
+            K.attention_bwd(q, k, v, o, torch.randn_like(o), lse, B, H, T, Tkv, causal=causal, kv_len=kv_len,
+                            dq=gq[1:, 64:], dk=gkv[1:, :d], dv=gkv[1:, d:2 * d])
     # slab training step on a narrow model (direct gradients, flat optimizer, shadow write)
     dims = ModelDimensions(80, 1500, 64, 1, 1, 51864, 448, 64, 1, 1)
     m = OLMoASR(dims).to(dev)
