@@ -14,6 +14,7 @@ import pytest
 import torch
 
 from tests import attention_reference as ar
+from tests.decode_reference import dec_out_ref, dec_scores_ref, ulp
 
 pytestmark = pytest.mark.gpu
 
@@ -344,24 +345,6 @@ def test_backward_rejects_misaligned_o(dtype):
 
 
 # ---------------------------------------------------------------------------------------------------- decode
-def _rnd(x, dtype):
-    return x.to(dtype).double()
-
-
-def _dec_scores_ref(q, kc, dtype, scale):
-    """Per (n, h, key): round_T(sum_c round_T(q_c s) round_T(k_c s)) in fp64, and sum_c |q_c s k_c s| (the scale of the
-    kernel's fp32 summation error).  q (n, H, 64), kc (n, keys, H, 64)."""
-    qs = (q.float() * scale).to(dtype).double()
-    ks = (kc.float() * scale).to(dtype).double()
-    return _rnd(torch.einsum("nhc,njhc->nhj", qs, ks), dtype), torch.einsum("nhc,njhc->nhj", qs.abs(), ks.abs())
-
-
-def _dec_out_ref(scores, vc, dtype):
-    """softmax of the rounded scores (n, H, keys), P rounded to T, then sum_j p_j v_j in fp64 -> (n, H, 64)."""
-    p = _rnd(torch.softmax(scores.double(), dim=-1), dtype)
-    return torch.einsum("nhj,njhc->nhc", p, vc.double())
-
-
 def _dec_call(q, k, v, seq_stride, row_stride, n, H, splits, dtype, pos=None, n_keys=0, kv_group=1):
     from olmoasr_b200._lib import DTYPE_BF16, DTYPE_F16, DecAttnArgs, call, ptr, stream
 
@@ -387,13 +370,6 @@ def _dec_call(q, k, v, seq_stride, row_stride, n, H, splits, dtype, pos=None, n_
     return scores, out
 
 
-def _ulp(x, dtype):
-    """Spacing of the 16-bit type at |x| (at 0: the smallest subnormal)."""
-    e = torch.frexp(x.abs().double())[1] - 1
-    e = torch.where(x == 0, torch.full_like(e, -1000), e)   # frexp(0) has exponent 0; the clamp below takes over
-    return torch.exp2((e - (7 if dtype == torch.bfloat16 else 10)).clamp_min(-24 if dtype == torch.float16 else -133).double())
-
-
 def _check_scores(got, ref, dtype, what):
     """Kernel scores against the fp64 statement's: at most 1% of them (or 2) differ at all, each by at most one T ulp
     -- its fp32 sum and the exact one fall on either side of a rounding boundary -- plus the fp32 sum's own error
@@ -401,7 +377,7 @@ def _check_scores(got, ref, dtype, what):
     ref, mag = ref
     got = got.double()
     diff = (got - ref).abs()
-    bound = _ulp(torch.maximum(got.abs(), ref.abs()), dtype) + 2.0 ** -18 * mag
+    bound = ulp(torch.maximum(got.abs(), ref.abs()), dtype) + 2.0 ** -18 * mag
     assert bool((diff <= bound).all()), f"{what}: worst score error {float((diff / bound).max()):.3g} x the bound"
     n_off = int((diff > 0).sum())
     assert n_off <= max(2, 0.01 * diff.numel()), f"{what}: {n_off} of {diff.numel()} scores differ"
@@ -441,8 +417,8 @@ def test_decode_self_attention(H, dtype):
                 _, out1 = _dec_call(*args, 1, dtype, pos=pos)
                 kh = kc[:, :keys].view(n, keys, H, HD)
                 vh = vc[:, :keys].view(n, keys, H, HD)
-                _check_scores(sc2[:, :, :keys], _dec_scores_ref(q.view(n, H, HD), kh, dtype, 64 ** -0.25), dtype, what)
-                ref = _dec_out_ref(sc2[:, :, :keys], vh, dtype)
+                _check_scores(sc2[:, :, :keys], dec_scores_ref(q.view(n, H, HD), kh, dtype, 64 ** -0.25), dtype, what)
+                ref = dec_out_ref(sc2[:, :, :keys], vh, dtype)
                 _check_out(out2, ref, dtype, what + " split")
                 _check_out(out1, ref, dtype, what + " fused")
 
@@ -463,7 +439,7 @@ def test_decode_cross_attention(kv_group, dtype):
         kv = kv.to(dtype)
         kh = kv[..., :d].reshape(n_kv, T, H, HD).repeat_interleave(kv_group, dim=0)
         vh = kv[..., d:].reshape(n_kv, T, H, HD).repeat_interleave(kv_group, dim=0)
-        sref = _dec_scores_ref(q.view(n, H, HD), kh, dtype, 64 ** -0.25)
+        sref = dec_scores_ref(q.view(n, H, HD), kh, dtype, 64 ** -0.25)
         args = (q, kv, kv[..., d:], T * 2 * d, 2 * d, n, H)
         sc2, _ = _dec_call(*args, 2, dtype, n_keys=T, kv_group=kv_group)
         for splits in (1, 2, 3, 7, 8):
@@ -472,4 +448,4 @@ def test_decode_cross_attention(kv_group, dtype):
             if splits > 1:
                 _check_scores(sc[:, :, :T], sref, dtype, what)
                 assert torch.equal(sc[:, :, :T], sc2[:, :, :T]), what   # split count does not change a score
-            _check_out(out, _dec_out_ref(sc2[:, :, :T], vh, dtype), dtype, what)
+            _check_out(out, dec_out_ref(sc2[:, :, :T], vh, dtype), dtype, what)

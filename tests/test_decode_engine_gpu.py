@@ -233,61 +233,3 @@ def test_sampling_kernel_bookkeeping():
     s.n_slices = 1
     call("oasr_dec_sample", ctypes.byref(s), stream())
     assert torch.equal(eng.tokens[:n, 2].cpu(), out) and torch.allclose(eng.sum_logprobs[:3].cpu(), lp[:3].cpu(), rtol=1e-4, atol=1e-4)
-
-
-@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("M", [1, 7, 16, 33, 64])
-def test_skinny_linear_modes(dtype, M):
-    """oasr_dec_linear: every prologue / epilogue against torch with the same rounding points."""
-    from olmoasr_b200.decode_engine import (EPI_GELU, EPI_LOGITS_F32, EPI_RESIDUAL, EPI_STORE, X_LAYERNORM, X_PARTIAL_SUM,
-                                            DecodeEngine)
-
-    class _Shell:   # the engine's launch helper without a model
-        dt = {torch.float16: 1, torch.bfloat16: 0}[dtype]
-        n_ctx = 448
-    sh = _Shell()
-    sh.pos = torch.zeros(1, device="cuda", dtype=torch.int32)
-    lin = lambda *a, **k: DecodeEngine._linear(sh, *a, **k)
-    torch.manual_seed(5)
-    Kd, N = 768, 1000                       # N not a multiple of the 16-column CTA tile
-    x = torch.randn(M, Kd, device="cuda").to(dtype)
-    W = (torch.randn(N, Kd, device="cuda") / math.sqrt(Kd)).to(dtype)
-    b = torch.randn(N, device="cuda")
-    rT = lambda t: t.to(dtype).float()
-    acc = x.float() @ W.float().t()
-    y = rT(acc + rT(b))
-    tol = dict(rtol=0, atol=2.0 ** (-9 if dtype == torch.float16 else -6) * float(y.abs().max()))
-    out = torch.zeros(M, N, device="cuda", dtype=dtype)
-    lin(M, x, W, b, out)
-    assert torch.allclose(out.float(), y, **tol)
-    lin(M, x, W, b, out, epi=EPI_GELU)
-    assert torch.allclose(out.float(), rT(F.gelu(y)), **tol)
-    res = torch.randn(M, N, device="cuda").to(dtype)
-    out2 = res.clone()
-    lin(M, x, W, b, out2, epi=EPI_RESIDUAL, res=out2)                     # in place, as the engine uses it
-    assert torch.allclose(out2.float(), rT(res.float() + y), **tol)
-    lg = torch.zeros(M, N, device="cuda")
-    lin(M, x, W, None, lg, epi=EPI_LOGITS_F32)
-    assert torch.allclose(lg, rT(acc), **tol)
-    gam, bet = torch.randn(Kd, device="cuda"), torch.randn(Kd, device="cuda")
-    xn = rT(F.layer_norm(x.float(), (Kd,), gam, bet, 1e-5))
-    lin(M, x, W, b, out, x_mode=X_LAYERNORM, ln=(gam, bet, 1e-5))
-    want = rT(xn @ W.float().t() + rT(b))
-    assert float((out.float() - want).norm() / want.norm()) <= (2e-3 if dtype == torch.float16 else 1.5e-2)
-    parts = torch.randn(3, M, Kd, device="cuda")
-    lin(M, parts, W, b, out, x_mode=X_PARTIAL_SUM, n_partials=3)
-    want = rT(rT(parts.sum(0)) @ W.float().t() + rT(b))
-    assert float((out.float() - want).norm() / want.norm()) <= (2e-3 if dtype == torch.float16 else 1.5e-2)
-    # K = 3072 (fc2): several k rounds per warp through the prefetch ring; at 64 rows the x tile is staged in K chunks
-    x4 = torch.randn(M, 3072, device="cuda").to(dtype)
-    W4 = (torch.randn(N, 3072, device="cuda") / math.sqrt(3072)).to(dtype)
-    lin(M, x4, W4, b, out)
-    want = rT(x4.float() @ W4.float().t() + rT(b))
-    assert torch.allclose(out.float(), want, **tol)
-    # a wide output (like the 51864-column logits head): several 16-column groups per CTA, LayerNorm prologue staged once
-    Nw = 16 * 700 + 5
-    Ww = (torch.randn(Nw, Kd, device="cuda") / math.sqrt(Kd)).to(dtype)
-    lgw = torch.zeros(M, Nw, device="cuda")
-    lin(M, x, Ww, None, lgw, x_mode=X_LAYERNORM, ln=(gam, bet, 1e-5), epi=EPI_LOGITS_F32)
-    want = rT(xn @ Ww.float().t())
-    assert float((lgw - want).norm() / want.norm()) <= (2e-3 if dtype == torch.float16 else 1.5e-2)
