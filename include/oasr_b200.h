@@ -63,7 +63,7 @@ OASR_API int oasr_gemm_set_sm_budget(int n_sms);
 #define OASR_EPI_BF16_RESIDUAL 2 /* C = bf16(aux + bf16(acc + bias))                            */
 #define OASR_EPI_BF16_GELU_BWD 3 /* C = bf16(bf16(acc) * gelu_erf'(aux))   aux = pre-activation  */
 #define OASR_EPI_F32 4           /* C(f32) = acc + bias                                         */
-#define OASR_EPI_F32_ATOMIC_ADD 5 /* C(f32) += acc   (split_k >= 1, C pre-initialised; one add per element) */
+#define OASR_EPI_F32_ATOMIC_ADD 5 /* C(f32) += acc   (split_k >= 1, C pre-initialised; one add per element; no bias) */
 
 OASR_API int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, int b_layout,
                    void* C, int64_t ldc, void* C2, const float* bias, const void* aux, int64_t ldaux,

@@ -43,9 +43,11 @@ ce_fwd_kernel(const T* __restrict__ logits, const int64_t* __restrict__ targets,
     float mx = f[0];
 #pragma unroll
     for (int j = 1; j < 8; ++j) mx = fmaxf(mx, f[j]);
-    float s = 0.f;
+    float s = 0.f;   // a group of eight -inf logits adds nothing (f - mx would be NaN)
+    if (mx != -INFINITY) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) s += __expf(f[j] - mx);
+      for (int j = 0; j < 8; ++j) s += __expf(f[j] - mx);
+    }
     acc = ms_merge(acc, MS{mx, s});
   }
   for (int c = (nvec << 3) + threadIdx.x; c < V; c += blockDim.x) acc = ms_merge(acc, MS{Act16<T>::to_f(x[c]), 1.f});

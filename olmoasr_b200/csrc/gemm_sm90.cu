@@ -326,6 +326,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int b = 0; b < BN / BOX; ++b) {
           const int col0 = n_blk * BN + BOX * b;
           if (col0 >= p.N) break;   // warpgroup-uniform
+          // TMA stores whole 16-byte chunks: with N % 8 != 0 the box that holds column N - 1 would also write zeros to
+          // columns N .. round8(N) - 1, outside the output, so that box goes out by plain bounded copies
+          const bool tma_box = p.tma_out && (col0 + BOX <= p.N || (p.N & 7) == 0);
 #pragma unroll
           for (int out = 0; out < (EPI == OASR_EPI_BF16_GELU ? 2 : 1); ++out) {
             uint32_t box;
@@ -335,7 +338,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
               constexpr int NOUT = EPI == OASR_EPI_BF16_GELU ? 2 : 1;
               box = epi_wg + ((b * NOUT + out) & 1) * BOX_BYTES;
               if (t == 0) {   // (a tile's first box: the previous tile's stores went out a whole mainloop ago)
-                if (b == 0 && out == 0) ptx::bulk_wait_group_read<0>();
+                // (a plain-copy box commits no store group, so the latest group may be reading this slot)
+                if ((b == 0 && out == 0) || !tma_box) ptx::bulk_wait_group_read<0>();
                 else ptx::bulk_wait_group_read<1>();
               }
               ptx::named_bar_sync(1 + c, 128);
@@ -365,7 +369,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 ptx::st_shared_u32(wa + 1024 * h, o);   // row r + 8h: 1024 bytes on, same swizzle
               }
             }
-            if (p.tma_out) {
+            if (tma_box) {
               ptx::fence_proxy_async_smem();
               ptx::named_bar_sync(1 + c, 128);
               if (t == 0) {
@@ -469,6 +473,8 @@ int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, i
     OASR_REQUIRE(aux != nullptr, "gemm: epilogue %d needs aux", epilogue);
   if (split_k < 1) split_k = 1;
   OASR_REQUIRE(split_k == 1 || epilogue == OASR_EPI_F32_ATOMIC_ADD, "gemm: split_k needs the accumulating fp32 epilogue");
+  // C += acc: a bias would be added once per split (each split's partial runs the F32 epilogue)
+  OASR_REQUIRE(bias == nullptr || epilogue != OASR_EPI_F32_ATOMIC_ADD, "gemm: the accumulating fp32 epilogue takes no bias");
   if (block_n == 0) block_n = (N > 128) ? 256 : (N > 64 ? 128 : 64);
   OASR_REQUIRE(block_n == 64 || block_n == 128 || block_n == 256, "gemm: block_n must be 64/128/256");
 
@@ -501,7 +507,8 @@ int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, i
   if (rc) return rc;
 
   // 16-bit epilogues: outputs and aux move by TMA in 64 x 64 boxes where TMA can address them (clipped at M and N by
-  // the maps), by plain bounded copies otherwise
+  // the maps; an output box past N with N % 8 != 0 is stored by plain copies, see the consumer), by plain bounded
+  // copies otherwise
   const bool epi16 = !is_f32_epi(epilogue);
   p.tma_out = epi16 && tma_addressable(Cout, ldc) && (epilogue != OASR_EPI_BF16_GELU || tma_addressable(C2, ldc));
   p.tma_aux = reads_aux(epilogue) && tma_addressable(aux, ldaux);

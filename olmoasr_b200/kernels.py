@@ -69,6 +69,7 @@ def gemm(a, b, M, N, K, *, a_mn=False, b_mn=False, out=None, out2=None, bias=Non
         _req(aux.dtype == dt and aux.stride(1) == 1 and aux.shape[0] == M, "gemm: aux")
     if bias is not None:
         _req(bias.dtype == torch.float32 and bias.numel() >= N and bias.is_contiguous(), "gemm: bias must be f32")
+        _req(epi != EPI_F32_ATOMIC_ADD, "gemm: the accumulating fp32 epilogue (out += acc) takes no bias")
     prof = GEMM_PROFILE
     if prof is not None:
         e0 = torch.cuda.Event(enable_timing=True)

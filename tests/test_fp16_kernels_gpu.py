@@ -144,24 +144,6 @@ def test_attention_fwd_bwd(K, use):
         assert _rel(got, r.transpose(1, 2).reshape(got.shape)) < 16 * EPS
 
 
-def test_layernorm_fwd_bwd(K):
-    torch.manual_seed(4)
-    rows, d = 1000, 384
-    x = torch.randn(rows, d, device="cuda").to(H16)
-    w, b = 1 + 0.1 * torch.randn(d, device="cuda"), 0.1 * torch.randn(d, device="cuda")
-    y, mean, rstd = K.layernorm_fwd(x, w, b)
-    xr = x.float().requires_grad_()
-    wr, br = w.clone().requires_grad_(), b.clone().requires_grad_()
-    ref = F.layer_norm(xr, (d,), wr, br, 1e-5)
-    assert y.dtype == H16 and _rel(y, _h(ref)) < 2 * EPS
-    dy, dres = (torch.randn(rows, d, device="cuda").to(H16) for _ in range(2))
-    ref.backward(dy.float())
-    dw, db = torch.zeros(d, device="cuda"), torch.zeros(d, device="cuda")
-    dx = K.layernorm_bwd(dy, x, w, mean, rstd, dw, db, dresidual=dres)
-    assert _rel(dx, _h(dres.float() + _h(xr.grad))) < 4 * EPS
-    assert _rel(dw, wr.grad) < 1e-5 and _rel(db, br.grad) < 1e-5
-
-
 def test_cross_entropy_and_logits(K):
     torch.manual_seed(5)
     rows, V, ld = 100, 51865, 51968

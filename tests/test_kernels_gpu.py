@@ -39,28 +39,6 @@ def test_gemm_layouts(K, M, N, Kd, bn, a_mn, b_mn):
     _close(out, A.float() @ B.float().t(), rtol=1e-4)
 
 
-def test_gemm_epilogues(K):
-    torch.manual_seed(1)
-    M, N, Kd = 512, 384, 320
-    A = torch.randn(M, Kd, device="cuda").bfloat16()
-    B = (torch.randn(N, Kd, device="cuda") / math.sqrt(Kd)).bfloat16()
-    bias = torch.randn(N, device="cuda")
-    aux = torch.randn(M, N, device="cuda").bfloat16()
-    ref = A.float() @ B.float().t()
-    rb = (ref + bias.bfloat16().float()).bfloat16().float()
-    _close(K.gemm(A, B, M, N, Kd, bias=bias), rb)
-    h, g = K.gemm(A, B, M, N, Kd, bias=bias, epi=K.EPI_BF16_GELU)
-    _close(h, rb)
-    _close(g, F.gelu(h.float()), rtol=1.0 / 200)
-    _close(K.gemm(A, B, M, N, Kd, bias=bias, aux=aux, epi=K.EPI_BF16_RESIDUAL), aux.float() + rb)
-    x = aux.float().requires_grad_(True)
-    F.gelu(x).backward(ref.bfloat16().float())
-    _close(K.gemm(A, B, M, N, Kd, aux=aux, epi=K.EPI_BF16_GELU_BWD), x.grad)
-    acc = torch.full((M, N), 2.0, device="cuda")
-    K.gemm(A, B, M, N, Kd, out=acc, epi=K.EPI_F32_ATOMIC_ADD, split_k=3)
-    _close(acc, ref + 2.0, rtol=1e-4)
-
-
 # Production shapes of the headline benchmark (medium model).  The unit shapes above never make a persistent CTA process a
 # second tile: these do (many tiles per CTA), which exercises the stage ring wrapping across tiles, the epilogue of one
 # tile overlapping the loads of the next, M-fastest rasterisation and split-K.
@@ -101,7 +79,7 @@ def test_gemm_production_tied_logits_raster_m(K):
         ref = x[r0:r0 + 1024].float() @ E.float().t()
         assert _rel_l2(buf[r0:r0 + 1024, :V], ref) < 3e-3, r0
     pad = buf[:, V:]
-    assert bool(((pad == 7.0) | (pad == 0.0)).all())             # padding columns: untouched or zero-filled, never garbage
+    assert bool((pad == 7.0).all())                              # padding columns: untouched
 
 
 def test_gemm_production_wgrad_split_k(K):
@@ -164,30 +142,6 @@ def test_gemm_rejects_bad_arguments(K):
 
 
 # ------------------------------------------------------------------------------------------------ LayerNorm
-@pytest.mark.parametrize("d", [384, 512, 768, 1024, 1280])
-def test_layernorm_fwd_bwd(K, d):
-    torch.manual_seed(2)
-    rows = 777
-    x = (torch.randn(rows, d, device="cuda") * 2 + 0.5).bfloat16()
-    w = torch.randn(d, device="cuda")
-    b = torch.randn(d, device="cuda")
-    y, mean, rstd = K.layernorm_fwd(x, w, b)
-    xr = x.float().requires_grad_(True)
-    wr, br = w.clone().requires_grad_(True), b.clone().requires_grad_(True)
-    yr = F.layer_norm(xr, (d,), wr, br, 1e-5)
-    _close(y, yr.detach())
-    dy = torch.randn(rows, d, device="cuda").bfloat16()
-    dres = torch.randn(rows, d, device="cuda").bfloat16()
-    yr.backward(dy.float())
-    dw = torch.zeros(d, device="cuda"); db = torch.zeros(d, device="cuda")
-    dx = K.layernorm_bwd(dy, x, w, mean, rstd, dw, db, dresidual=dres)
-    _close(dx, dres.float() + xr.grad.bfloat16().float())
-    _close(dw, wr.grad, rtol=2e-3)
-    _close(db, br.grad, rtol=2e-3)
-    dx2 = K.layernorm_bwd(dy, x, w, mean, rstd, torch.zeros_like(dw), torch.zeros_like(db))
-    _close(dx2, xr.grad)
-
-
 # ------------------------------------------------------------------------------------------------ attention
 def _sdpa_ref(q, k, v, B, H, Tq, Tkv, causal, kv_len):
     qh = q.float().view(B, Tq, H, 64).permute(0, 2, 1, 3)
@@ -290,27 +244,6 @@ def test_cross_block_reductions_repeat_bit_for_bit(K):
 
 
 # ------------------------------------------------------------------------------------------------ CE / embedding
-def test_cross_entropy_fwd_bwd(K):
-    torch.manual_seed(4)
-    rows, V, ld = 96, 51865, 51968
-    logits = torch.zeros(rows, ld, device="cuda", dtype=torch.bfloat16)
-    logits[:, :V] = (torch.randn(rows, V, device="cuda") * 3).bfloat16()
-    y = torch.randint(0, 50257, (rows,), device="cuda")
-    y[::5] = 51864
-    ref_in = logits[:, :V].float().requires_grad_(True)
-    loss_ref = F.cross_entropy(ref_in, y, ignore_index=51864)
-    lse, lsc = K.ce_fwd(logits, y, V, 51864)
-    loss = K.ce_finalize(lsc)
-    assert abs(loss.item() - loss_ref.item()) <= 1e-4 * abs(loss_ref.item())
-    assert lsc[1].item() == float((y != 51864).sum()) and lsc[2].item() == 0.0
-    y_bad = y.clone(); y_bad[1] = 60000; y_bad[2] = -3           # out-of-range targets are counted (F.cross_entropy raises)
-    assert K.ce_fwd(logits, y_bad, V, 51864)[1][2].item() == 2.0
-    (loss_ref * 7.0).backward()
-    K.ce_bwd_(logits, y, lse, lsc, torch.tensor([7.0], device="cuda"), V, 51864)
-    _close(logits[:, :V], ref_in.grad, rtol=1.0 / 128)
-    assert logits[::5, :V].abs().max().item() == 0.0
-
-
 def test_embedding_fwd_bwd(K):
     torch.manual_seed(5)
     B, S, d, V = 3, 448, 384, 51865
