@@ -386,6 +386,40 @@ OASR_API int oasr_add_pos16(const void* x, const float* pos, void* out, int64_t 
                             void* stream);
 OASR_API int oasr_gelu_bwd16(const void* dy, const void* pre, void* out, int64_t n, int dtype, void* stream);
 OASR_API int oasr_colsum16(const void* dy, float* db, int64_t M, int64_t N, int64_t ld, int dtype, void* stream);
+/* ---- packed (variable-length) decoder batches ----------------------------------------------------------------
+ * A training batch whose sample b holds its first len_b tokens (the reference loader pads every transcript to n_text_ctx
+ * with 51864 and masks the rest, train_timestamps.py:314-329) runs the decoder on its N = sum len_b real rows only:
+ * sample b owns packed rows [cu_seqlens[b], cu_seqlens[b+1]) (int32, B+1 entries, cu_seqlens[0] = 0).
+ *
+ * oasr_attention_*_varlen16: the attention kernels above over packed query rows q / o / dq (N rows; lse and delta are
+ * (H, N) f32).  tiles lists n_tiles (b, j) int32 pairs, one per 128-row query tile j of sample b that holds a row: only
+ * those tiles are launched.  Two forms:
+ *   kv_cu_seqlens == cu_seqlens: causal self-attention; k / v / dk / dv are packed like q and sample b sees its own
+ *                                len_b keys (the reference's causal + padding mask); Tkv is ignored.
+ *   kv_cu_seqlens == NULL:       cross-attention; k / v / dk / dv are dense (B*Tkv rows, sample b at row b*Tkv).
+ * For each sample the results are bit-for-bit those of oasr_attention_fwd16 / _bwd16 on that sample alone (B = 1,
+ * Tq = len_b).  No row of another sample is written.
+ *
+ * oasr_embed_fwd_packed16: out (N, d) = T(emb[ids[src_rows[r]]] + pos[src_rows[r] % S]), src_rows (N,) int32 holding
+ * b*S + t of each packed row of ids (B, S).  oasr_embed_bwd_packed16 ACCUMULATES the packed gradient dx (N, d) into
+ * demb / dpos with oasr_embed_bwd16's summation order (padded rows, whose gradient is zero, left out). */
+OASR_API int oasr_attention_fwd_varlen16(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                         int64_t ldv, void* o, int64_t ldo, float* lse, int64_t B, int64_t H, int64_t N,
+                                         int64_t Tkv, int64_t head_dim, const int32_t* cu_seqlens,
+                                         const int32_t* kv_cu_seqlens, const int32_t* tiles, int64_t n_tiles, float scale,
+                                         int dtype, void* stream);
+OASR_API int oasr_attention_bwd_varlen16(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                         int64_t ldv, const void* o, int64_t ldo, const void* dout, int64_t lddo,
+                                         const float* lse, float* delta, void* dq, int64_t lddq, void* dk, int64_t lddk,
+                                         void* dv, int64_t lddv, int64_t B, int64_t H, int64_t N, int64_t Tkv,
+                                         int64_t head_dim, const int32_t* cu_seqlens, const int32_t* kv_cu_seqlens,
+                                         const int32_t* tiles, int64_t n_tiles, float scale, int dtype, void* stream);
+OASR_API int oasr_embed_fwd_packed16(const int64_t* ids, const float* emb, const float* pos, void* out,
+                                     const int32_t* src_rows, int64_t N, int64_t S, int64_t d, int64_t n_rows_emb, int dtype,
+                                     void* stream);
+OASR_API int oasr_embed_bwd_packed16(const int64_t* ids, const void* dx, float* demb, float* dpos, const int32_t* src_rows,
+                                     const int32_t* cu_seqlens, int64_t B, int64_t N, int64_t S, int64_t d,
+                                     int64_t padding_idx, int64_t n_rows_emb, int dtype, void* stream);
 /* The flat AdamW update refreshing a shadow slab of type `dtype` (bf16 or fp16; see oasr_adamw_flat). */
 OASR_API int oasr_adamw_flat16(float* p, const float* g, float* m, float* v, void* shadow, int64_t numel,
                                const float* state, float lr, float beta1, float beta2, float eps, float weight_decay,

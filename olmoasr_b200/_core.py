@@ -315,6 +315,69 @@ def kv_len_from_padding_mask(padding_mask: Tensor) -> Tensor:
     return kv
 
 
+class PackedBatch:
+    """The decoder rows of a batch whose sample b holds its first lens[b] tokens, stacked in (b, t) order: N rows
+    instead of B*S.  One int32 device buffer, filled by one pinned non-blocking copy, carries what the kernels read:
+        cu     (B+1,)        sample b owns packed rows [cu[b], cu[b+1])
+        tiles  (n_tiles, 2)  (b, j) for every 128-row tile j of sample b that holds a row: the attention grids
+        rows   (N,)          dense index b*S + t of each packed row: the embedding gather, the target gather
+    Every decoder layer reads the same buffer in forward and backward."""
+
+    TILE = 128   # query / key rows per attention tile (csrc/attention_*_sm90.cu)
+
+    def __init__(self, lens, S: int, device):
+        self.lens = [int(n) for n in lens]
+        self.B, self.S = len(self.lens), int(S)
+        cu = np.zeros(self.B + 1, dtype=np.int32)
+        cu[1:] = np.cumsum(self.lens)
+        self.N = int(cu[-1])
+        tiles = [(b, j) for b, n in enumerate(self.lens) for j in range((n + self.TILE - 1) // self.TILE)]
+        self.n_tiles = len(tiles)
+        rows = np.concatenate([b * self.S + np.arange(n, dtype=np.int32) for b, n in enumerate(self.lens)])
+        host = torch.from_numpy(np.concatenate([cu, np.asarray(tiles, dtype=np.int32).reshape(-1), rows]))
+        device = torch.device(device)
+        if device.type == "cuda":
+            buf = torch.empty(host.shape, device=device, dtype=torch.int32)
+            buf.copy_(host.pin_memory(), non_blocking=True)
+        else:
+            buf = host
+        n_cu, n_t = self.B + 1, 2 * self.n_tiles
+        self.cu, self.tiles, self.rows = buf[:n_cu], buf[n_cu:n_cu + n_t].view(-1, 2), buf[n_cu + n_t:]
+
+
+def packed_text_lens(text_lens, tokens: Tensor, targets: Optional[Tensor], padding_mask: Optional[Tensor]) -> list:
+    """Validate the `text_lens=` argument of the loss calls and return it as a list of ints.  It is host data by design:
+    reading a CUDA tensor would put a device-to-host sync into every step."""
+    if targets is None:
+        raise ValueError("text_lens packs the loss route only: pass targets= as well (the logits route is dense)")
+    if padding_mask is not None:
+        raise ValueError("pass either text_lens or padding_mask, not both: text_lens already defines the key counts")
+    if isinstance(text_lens, Tensor):
+        if text_lens.is_cuda:
+            raise ValueError("text_lens must be host data (a CPU tensor or a sequence of ints): reading a CUDA tensor "
+                             "would synchronise with the device on every step")
+        if text_lens.is_floating_point() or text_lens.is_complex() or text_lens.dtype == torch.bool or text_lens.dim() != 1:
+            raise ValueError(f"text_lens must be a 1-D integer tensor, got {text_lens.dtype} {tuple(text_lens.shape)}")
+        lens = [int(n) for n in text_lens.tolist()]
+    else:
+        try:
+            lens = list(text_lens)
+        except TypeError:
+            raise ValueError("text_lens must be a CPU integer tensor or a sequence of ints") from None
+        if not all(isinstance(n, (int, np.integer)) and not isinstance(n, bool) for n in lens):
+            raise ValueError("text_lens must be a CPU integer tensor or a sequence of ints")
+        lens = [int(n) for n in lens]
+    B, S = tokens.shape
+    if tuple(targets.shape) != (B, S):
+        raise ValueError(f"targets {tuple(targets.shape)} must have the shape of tokens {(B, S)} with text_lens")
+    if len(lens) != B:
+        raise ValueError(f"text_lens has {len(lens)} entries for a batch of {B}")
+    bad = [n for n in lens if not 1 <= n <= S]
+    if bad:
+        raise ValueError(f"text_lens entries must lie in [1, {S}], got {bad[0]}")
+    return lens
+
+
 class _ShadowCache:
     """16-bit copies of fp32 master weights (+ fused biases), rebuilt only when a master or the wanted type changed."""
 
@@ -520,15 +583,28 @@ class MultiHeadAttention(nn.Module):
 # =====================================================================================================
 # fused training blocks
 # =====================================================================================================
+def _self_attn_fwd(q, k, v, B, H, T, causal, kv_len, pk):
+    if pk is not None:
+        return K.attention_fwd_varlen(q, k, v, pk, H)
+    return K.attention_fwd(q, k, v, B, H, T, T, causal=causal, kv_len=kv_len)
+
+
+def _cross_attn_fwd(q, k, v, B, H, T, Ta, pk):
+    if pk is not None:
+        return K.attention_fwd_varlen(q, k, v, pk, H, Tkv=Ta)
+    return K.attention_fwd(q, k, v, B, H, T, Ta)
+
+
 class _BlockFn(torch.autograd.Function):
     """ResidualAttentionBlock.forward (model.py:485-528) for a (B*T, d) bf16 or fp16 residual stream (x's type is the
-    block's compute type).
+    block's compute type), or for the (N, d) rows of a packed decoder batch `pk` (PackedBatch; then B, T are its batch
+    size and dense length, the self-attention is causal over each sample's own rows and kv_len is None).
 
     inputs: x, xa (or None), kv_len (or None), then the block's parameters in `ResidualAttentionBlock._param_list`
     order.  Saves every GEMM input it needs for wgrad; recomputes nothing."""
 
     @staticmethod
-    def forward(ctx, blk, B, T, Ta, causal, kv_len, xa_state, x, xa, *params):
+    def forward(ctx, blk, B, T, Ta, causal, kv_len, xa_state, pk, x, xa, *params):
         ctx.xa_state = xa_state
         H = blk.attn.n_head
         d = x.shape[1]
@@ -540,14 +616,14 @@ class _BlockFn(torch.autograd.Function):
             side.run(lambda: linear_fwd(xa, sh["wckv"], sh["bckv"], out=kvc))
         ln1, mean1, rstd1 = K.layernorm_fwd(x, sh["ln1w"], sh["ln1b"])
         qkv = linear_fwd(ln1, sh["wqkv"], sh["bqkv"])
-        ao, lse = K.attention_fwd(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], B, H, T, T, causal=causal, kv_len=kv_len)
+        ao, lse = _self_attn_fwd(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], B, H, T, causal, kv_len, pk)
         x1 = linear_fwd(ao, sh["wo"], sh["bo"], epi=K.EPI_BF16_RESIDUAL, aux=x)
         saved = [x, mean1, rstd1, ln1, qkv, ao, lse, x1]
         if xa is not None:
             lnc, meanc, rstdc = K.layernorm_fwd(x1, sh["lncw"], sh["lncb"])
             qc = linear_fwd(lnc, sh["wcq"], sh["bcq"])
             side.join()
-            co, lsec = K.attention_fwd(qc, kvc[:, :d], kvc[:, d:], B, H, T, Ta)
+            co, lsec = _cross_attn_fwd(qc, kvc[:, :d], kvc[:, d:], B, H, T, Ta, pk)
             x2 = linear_fwd(co, sh["wco"], sh["bco"], epi=K.EPI_BF16_RESIDUAL, aux=x1)
             saved += [xa, meanc, rstdc, lnc, qc, kvc, co, lsec, x2]
         else:
@@ -559,7 +635,7 @@ class _BlockFn(torch.autograd.Function):
         if kv_len is not None:
             saved.append(kv_len)
         ctx.save_for_backward(*saved)
-        ctx.blk, ctx.dims, ctx.sh = blk, (B, T, Ta, H, d, causal, xa is not None, kv_len is not None), sh
+        ctx.blk, ctx.dims, ctx.sh, ctx.pk = blk, (B, T, Ta, H, d, causal, xa is not None, kv_len is not None), sh, pk
         return x3
 
     @staticmethod
@@ -569,6 +645,7 @@ class _BlockFn(torch.autograd.Function):
         if not _is_master(blk.attn.query.weight):
             sh = blk._shadows(sv[0].dtype)   # FSDP frees and re-gathers the unsharded parameters between forward and backward
         B, T, Ta, H, d, causal, cross, has_len = ctx.dims
+        pk = ctx.pk
         kv_len = sv.pop() if has_len else None
         x, mean1, rstd1, ln1, qkv, ao, lse, x1 = sv[:8]
         if cross:
@@ -595,7 +672,11 @@ class _BlockFn(torch.autograd.Function):
             dco = linear_dgrad(dx2, sh["wco"])
             dqc = torch.empty_like(qc)
             dkvc = torch.empty_like(kvc)
-            K.attention_bwd(qc, kvc[:, :d], kvc[:, d:], co, dco, lsec, B, H, T, Ta, dq=dqc, dk=dkvc[:, :d], dv=dkvc[:, d:])
+            if pk is not None:
+                K.attention_bwd_varlen(qc, kvc[:, :d], kvc[:, d:], co, dco, lsec, pk, H, Tkv=Ta, dq=dqc, dk=dkvc[:, :d],
+                                       dv=dkvc[:, d:])
+            else:
+                K.attention_bwd(qc, kvc[:, :d], kvc[:, d:], co, dco, lsec, B, H, T, Ta, dq=dqc, dk=dkvc[:, :d], dv=dkvc[:, d:])
             grads.linear("cross_attn.query", dqc, lnc)
             grads.linear("cross_attn.kv", dkvc, xa)         # [dWk; dWv] in one GEMM
             # d(loss)/d(xa): every decoder layer contributes one (B*1500, d) term.  Instead of 24 separate tensors that
@@ -626,15 +707,19 @@ class _BlockFn(torch.autograd.Function):
         grads.linear("attn.out", dx1, ao)
         dao = linear_dgrad(dx1, sh["wo"])
         dqkv = torch.empty_like(qkv)
-        K.attention_bwd(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ao, dao, lse, B, H, T, T, causal=causal, kv_len=kv_len,
-                        dq=dqkv[:, :d], dk=dqkv[:, d:2 * d], dv=dqkv[:, 2 * d:])
+        if pk is not None:
+            K.attention_bwd_varlen(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ao, dao, lse, pk, H,
+                                   dq=dqkv[:, :d], dk=dqkv[:, d:2 * d], dv=dqkv[:, 2 * d:])
+        else:
+            K.attention_bwd(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ao, dao, lse, B, H, T, T, causal=causal, kv_len=kv_len,
+                            dq=dqkv[:, :d], dk=dqkv[:, d:2 * d], dv=dqkv[:, 2 * d:])
         grads.linear("attn.qkv", dqkv, ln1)                 # [dWq; dWk; dWv] in one GEMM
         dln1 = linear_dgrad(dqkv, sh["wqkv"])
         dx = K.layernorm_bwd(dln1, x, sh["ln1w"], mean1, rstd1, grads.vec("attn_ln.weight", d), grads.vec("attn_ln.bias", d),
                              dresidual=dx1)
         side.join()
         grads.done()
-        return (None, None, None, None, None, None, None, dx, dxa, *grads.grads_for(blk._param_names))
+        return (None, None, None, None, None, None, None, None, dx, dxa, *grads.grads_for(blk._param_names))
 
 
 class ResidualAttentionBlock(nn.Module):
@@ -689,9 +774,14 @@ class ResidualAttentionBlock(nn.Module):
         return self._shadow.get([p for _, p in self.named_parameters()], lambda: self._build_shadows(dtype), dtype)
 
     def forward(self, x: Tensor, xa: Optional[Tensor] = None, mask: Optional[Tensor] = None,
-                kv_cache: Optional[dict] = None, verbose: bool = False, _xa_state: Optional[dict] = None):
+                kv_cache: Optional[dict] = None, verbose: bool = False, _xa_state: Optional[dict] = None,
+                _packed: Optional[PackedBatch] = None):
         if kv_cache is not None:
             return self._forward_cached(x, xa, mask, kv_cache)
+        if _packed is not None:      # x: the (N, d) rows of a packed decoder batch (TextDecoder.hidden)
+            params = [_attr_by_path(self, n) for n in self._param_names]
+            xa2 = _as16_2d(xa, x.dtype)
+            return _BlockFn.apply(self, _packed.B, _packed.S, xa.shape[1], True, None, _xa_state, _packed, x, xa2, *params)
         B, T, d = x.shape
         causal, kv_len = False, None
         if mask is not None:
@@ -703,7 +793,7 @@ class ResidualAttentionBlock(nn.Module):
         xa2 = _as16_2d(xa, dt) if xa is not None else None
         # attribute walk, not get_parameter(): under FSDP the attributes are plain tensor views of the flat parameter
         params = [_attr_by_path(self, n) for n in self._param_names]
-        y = _BlockFn.apply(self, B, T, Ta, causal, kv_len, _xa_state, _as16_2d(x, dt), xa2, *params)
+        y = _BlockFn.apply(self, B, T, Ta, causal, kv_len, _xa_state, None, _as16_2d(x, dt), xa2, *params)
         return y.view(B, T, d)
 
     def _forward_cached(self, x, xa, mask, kv_cache):
@@ -814,14 +904,18 @@ class _LayerNormFn(torch.autograd.Function):
 # decoder
 # =====================================================================================================
 class _EmbedFn(torch.autograd.Function):
-    """(token_embedding(ids) + positional_embedding[offset:offset+S]).to(dtype)  (model.py:728-732)."""
+    """(token_embedding(ids) + positional_embedding[offset:offset+S]).to(dtype)  (model.py:728-732); with a PackedBatch
+    `pk` only its N rows, (N, d)."""
 
     @staticmethod
-    def forward(ctx, ids, emb, pos, offset, padding_idx, dec=None, dtype=torch.bfloat16):
-        out = K.embed_fwd(ids.contiguous(), _f32(emb), _f32(pos), offset, **_f16_kw(dtype))
+    def forward(ctx, ids, emb, pos, offset, padding_idx, dec=None, dtype=torch.bfloat16, pk=None):
+        if pk is not None:
+            out = K.embed_fwd_packed(ids.contiguous(), _f32(emb), _f32(pos), pk, dtype)
+        else:
+            out = K.embed_fwd(ids.contiguous(), _f32(emb), _f32(pos), offset, **_f16_kw(dtype))
         ctx.save_for_backward(ids)
         ctx.meta = (emb.shape, pos.shape, offset, padding_idx)
-        ctx.dec = dec
+        ctx.dec, ctx.pk = dec, pk
         return out
 
     @staticmethod
@@ -832,9 +926,12 @@ class _EmbedFn(torch.autograd.Function):
         grads, names = _GradDest(ctx.dec, dx.device), ("token_embedding.weight", "positional_embedding")
         # in direct mode a scatter-add straight into the slab, where the tied logits wgrad has already accumulated
         demb, dpos = grads.vec(names[0], eshape), grads.vec(names[1], pshape)
-        K.embed_bwd(ids.contiguous(), dx.contiguous(), demb, dpos[offset:], pad)
+        if ctx.pk is not None:
+            K.embed_bwd_packed(ids.contiguous(), dx.contiguous(), demb, dpos, ctx.pk, pad)
+        else:
+            K.embed_bwd(ids.contiguous(), dx.contiguous(), demb, dpos[offset:], pad)
         grads.done()     # decoder gradients (incl. the tied embedding) are final
-        return (None, *grads.grads_for(names), None, None, None, None)
+        return (None, *grads.grads_for(names), None, None, None, None, None)
 
 
 def _logits_ld(V: int) -> int:
@@ -941,19 +1038,26 @@ class TextDecoder(nn.Module):
         return self._emb_shadow.get((w,), lambda: _cast16(w.detach().contiguous(), dtype), dtype)
 
     def hidden(self, x: Tensor, xa: Tensor, kv_cache: Optional[dict] = None, padding_mask: Optional[Tensor] = None,
-               dtype: Optional[torch.dtype] = None) -> Tensor:
-        """Everything up to and including the final LayerNorm: (B, S) ids -> (B*S, d) in `dtype` (default: compute_dtype())."""
+               dtype: Optional[torch.dtype] = None, packed: Optional[PackedBatch] = None) -> Tensor:
+        """Everything up to and including the final LayerNorm: (B, S) ids -> (B*S, d) in `dtype` (default: compute_dtype()),
+        or -> (N, d) for the rows of a PackedBatch."""
         dt = compute_dtype() if dtype is None else dtype
         if self._slabs is not None:
             self._slabs.ensure_synced(dt)
         offset = next(iter(kv_cache.values())).shape[1] if kv_cache else 0
         B, S = x.shape
         d = self.positional_embedding.shape[1]
+        # shared accumulator of the layers' gradients w.r.t. the encoder output (see _BlockFn.backward); one per forward pass
+        xa_state = {"buf": None, "left": len(self.blocks)} if (kv_cache is None and torch.is_grad_enabled() and xa.requires_grad) else None
+        if packed is not None:
+            h = _EmbedFn.apply(x, self.token_embedding.weight, self.positional_embedding, 0, self.token_embedding.padding_idx,
+                               self, dt, packed)
+            for block in self.blocks:
+                h = block(h, xa, _xa_state=xa_state, _packed=packed)
+            return _LayerNormFn.apply(h, self.ln.weight, self.ln.bias, self.ln.eps, self, "ln")
         h = _EmbedFn.apply(x, self.token_embedding.weight, self.positional_embedding, offset,
                            self.token_embedding.padding_idx, self, dt).view(B, S, d)
         mask = padding_mask if padding_mask is not None else self.mask[:S, :S]
-        # shared accumulator of the layers' gradients w.r.t. the encoder output (see _BlockFn.backward); one per forward pass
-        xa_state = {"buf": None, "left": len(self.blocks)} if (kv_cache is None and torch.is_grad_enabled() and xa.requires_grad) else None
         for block in self.blocks:
             h = block(h, xa, mask=mask, kv_cache=kv_cache, _xa_state=xa_state) if xa_state is not None else \
                 block(h, xa, mask=mask, kv_cache=kv_cache)
@@ -967,10 +1071,20 @@ class TextDecoder(nn.Module):
         logits = _LogitsFn.apply(h, self.token_embedding.weight, self.embedding16(dt), self)
         return logits.view(B, S, -1)
 
-    def loss(self, x: Tensor, xa: Tensor, targets: Tensor, padding_mask: Optional[Tensor] = None, ignore_index: int = PAD_ID_EN):
+    def loss(self, x: Tensor, xa: Tensor, targets: Tensor, padding_mask: Optional[Tensor] = None, ignore_index: int = PAD_ID_EN,
+             text_lens=None):
+        """Mean token cross-entropy.  With `text_lens` (host-side lengths, one per sample) the decoder runs on each
+        sample's first text_lens[b] rows only; targets at t >= text_lens[b] count as ignored.  That is the loss of the
+        dense call with the reference's padding mask for those lengths (train_timestamps.py:314-315)."""
         dt = compute_dtype()
-        h = self.hidden(x, xa, None, padding_mask, dt)
-        return _LossHeadFn.apply(h, self.token_embedding.weight, self.embedding16(dt), targets, ignore_index, self)
+        if text_lens is None:
+            h = self.hidden(x, xa, None, padding_mask, dt)
+            return _LossHeadFn.apply(h, self.token_embedding.weight, self.embedding16(dt), targets, ignore_index, self)
+        lens = packed_text_lens(text_lens, x, targets, padding_mask)
+        pk = PackedBatch(lens, x.shape[1], x.device)
+        h = self.hidden(x, xa, None, None, dt, packed=pk)
+        t = targets.reshape(-1).index_select(0, pk.rows)
+        return _LossHeadFn.apply(h, self.token_embedding.weight, self.embedding16(dt), t, ignore_index, self)
 
 
 # =====================================================================================================
@@ -1081,17 +1195,28 @@ class OLMoASRBase(nn.Module):
         return self.decoder(tokens, audio_features, padding_mask=padding_mask)
 
     def forward(self, mel: Tensor, tokens: Tensor, padding_mask: Tensor = None, verbose: bool = False, *,
-                targets: Optional[Tensor] = None, ignore_index: int = PAD_ID_EN) -> Tensor:
+                targets: Optional[Tensor] = None, ignore_index: int = PAD_ID_EN, text_lens=None) -> Tensor:
         """Reference signature (model.py:856-887) -> fp32 logits.  With the keyword-only `targets` the call returns
-        the token cross-entropy instead (fused head); going through forward() keeps DDP / FSDP wrappers in the loop."""
+        the token cross-entropy instead (fused head); going through forward() keeps DDP / FSDP wrappers in the loop.
+        `text_lens` (with `targets`, instead of `padding_mask`): see `loss`."""
+        if text_lens is not None:
+            packed_text_lens(text_lens, tokens, targets, padding_mask)    # reject a bad call before the encoder runs
         if targets is not None:
-            return self.decoder.loss(tokens, self.encoder(mel), targets, padding_mask, ignore_index)
+            return self.decoder.loss(tokens, self.encoder(mel), targets, padding_mask, ignore_index, text_lens)
         return self.decoder(tokens, self.encoder(mel), padding_mask=padding_mask)
 
-    def loss(self, mel: Tensor, tokens: Tensor, targets: Tensor, padding_mask: Tensor = None, ignore_index: int = PAD_ID_EN):
+    def loss(self, mel: Tensor, tokens: Tensor, targets: Tensor, padding_mask: Tensor = None, ignore_index: int = PAD_ID_EN,
+             text_lens=None):
         """Fused equivalent of `F.cross_entropy(model(mel, tokens, padding_mask).view(-1, V), targets.view(-1),
-        ignore_index=51864)` (train_timestamps.py:1440-1448) that never materialises fp32 logits."""
-        return self.decoder.loss(tokens, self.encoder(mel), targets, padding_mask, ignore_index)
+        ignore_index=51864)` (train_timestamps.py:1440-1448) that never materialises fp32 logits.
+
+        text_lens: host-side lengths (a CPU integer tensor or a sequence of ints, 1 <= text_lens[b] <= tokens.shape[1]),
+        e.g. the `len(text_input)` a loader computes per sample, in place of `padding_mask`.  The decoder then runs on
+        each transcript's own rows only, packed back to back, and returns the loss of the dense call with the reference's
+        padding mask for those lengths, targets at t >= text_lens[b] counting as ignored."""
+        if text_lens is not None:
+            packed_text_lens(text_lens, tokens, targets, padding_mask)
+        return self.decoder.loss(tokens, self.encoder(mel), targets, padding_mask, ignore_index, text_lens)
 
     @property
     def device(self):

@@ -24,6 +24,12 @@
 // into it with atomics (whose order, and so rounding, changes from run to run), a second kernel owns each 128-query tile,
 // recomputes S and dP for it and accumulates dQ = sum_j dS_j K_j over the key tiles in order:
 //     S = Q K^T   dP = dO V^T   (wgmma m64n128k16)   dS = P o (dP - D)   dQ += dS K   (dS as register A, K MN-major)
+//
+// Packed (varlen) batches use the row offsets of attention_fwd_sm90.cu (LSE / delta (1, H, N)).  A 64-query step of the
+// dK / dV loop may then read the NEXT sample's rows, whose dO is not zero the way a padded row's is: every P^T / dS^T
+// column is tested against the sample's own query count, and dQ / dK / dV stores against its own lengths.  With packed
+// keys (self-attention) the dK / dV grid runs over the same (sample, 128-row tile) list as the dQ grid; with dense keys
+// (cross-attention) it keeps its (key tile, head, sample) grid.
 #include "common.cuh"
 #include "ptx_sm90.cuh"
 
@@ -53,6 +59,9 @@ struct BwdParams {
   void* dv;
   int64_t lddq, lddk, lddv;
   const int32_t* kv_len;
+  const int32_t* q_off;    // (B+1,) packed query row offsets, nullable
+  const int32_t* kv_off;   // (B+1,) packed key row offsets, nullable
+  const int32_t* tiles;    // (sample, 128-row tile) int32 pairs of the packed grids (4-byte aligned)
   int B, H, Tq, Tkv;
   int causal;
   float scale, scale_log2;
@@ -71,12 +80,19 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 
   const uint32_t sK = ptx::smem_u32(smem_raw), sV = sK + KV_BYTES;
   const uint32_t sQ0 = sV + KV_BYTES;                        // stage s: Q at sQ0 + s*16K, dO right after Q
-  const int kv_tile = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int h = blockIdx.y;
+  int kv_tile = blockIdx.x, b = blockIdx.z;
+  if (p.kv_off) { b = p.tiles[2 * blockIdx.x]; kv_tile = p.tiles[2 * blockIdx.x + 1]; }
   const int kv0 = kv_tile * BKV;
-  int kv_valid = p.Tkv;
+  const int q_row0 = p.q_off ? p.q_off[b] : b * p.Tq;
+  const int tq = p.q_off ? p.q_off[b + 1] - q_row0 : p.Tq;     // the sample's query rows; later rows are foreign or padding
+  const int kv_row0 = p.kv_off ? p.kv_off[b] : b * p.Tkv;
+  const int tkv = p.kv_off ? p.kv_off[b + 1] - kv_row0 : p.Tkv;
+  int kv_valid = tkv;
   if (p.kv_len) kv_valid = min(kv_valid, max(1, p.kv_len[b]));
+  const int64_t lse0 = p.q_off ? static_cast<int64_t>(h) * p.Tq + q_row0 : (static_cast<int64_t>(b) * p.H + h) * p.Tq;
 
-  const int n_q_tiles = (p.Tq + BQ - 1) / BQ;
+  const int n_q_tiles = (tq + BQ - 1) / BQ;
   const int i_begin = p.causal ? kv0 / BQ : 0;                 // earlier queries cannot see these keys
   const int n_iter = (kv0 < kv_valid) ? n_q_tiles - i_begin : 0;   // fully masked key tile: zero gradients
 
@@ -99,13 +115,13 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     const uint32_t dst = sQ0 + st * 2 * QT_BYTES;
     const int q0 = (i_begin + it) * BQ;
     ptx::mbar_arrive_expect_tx(full, 2 * QT_BYTES);
-    ptx::tma_load_2d(dst, &tmQ, full, h * HD, b * p.Tq + q0);
-    ptx::tma_load_2d(dst + QT_BYTES, &tmdO, full, h * HD, b * p.Tq + q0);
+    ptx::tma_load_2d(dst, &tmQ, full, h * HD, q_row0 + q0);
+    ptx::tma_load_2d(dst + QT_BYTES, &tmdO, full, h * HD, q_row0 + q0);
   };
   if (threadIdx.x == 0 && n_iter > 0) {
     ptx::mbar_arrive_expect_tx(ptx::smem_u32(&bar_kv), 2 * KV_BYTES);
-    ptx::tma_load_2d(sK, &tmK, ptx::smem_u32(&bar_kv), h * HD, b * p.Tkv + kv0);
-    ptx::tma_load_2d(sV, &tmV, ptx::smem_u32(&bar_kv), h * HD, b * p.Tkv + kv0);
+    ptx::tma_load_2d(sK, &tmK, ptx::smem_u32(&bar_kv), h * HD, kv_row0 + kv0);
+    ptx::tma_load_2d(sV, &tmV, ptx::smem_u32(&bar_kv), h * HD, kv_row0 + kv0);
     for (int it = 0; it < min(STAGES, n_iter); ++it) load_q(it);
   }
 
@@ -146,7 +162,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     auto grads = [&](int it) {
       const int q0 = (i_begin + it) * BQ;
       // every (key, query) pair of this thread visible: no per-element test (the common case away from the edges)
-      const bool all_vis = q0 + BQ <= p.Tq && key_abs[1] < kv_valid && (!p.causal || key_abs[1] <= q0);
+      const bool all_vis = q0 + BQ <= tq && key_abs[1] < kv_valid && (!p.causal || key_abs[1] <= q0);
       auto run = [&](auto masked) {
         // lse / delta of this thread's 16 query columns
         float lse_c[16], dlt_c[16];
@@ -155,9 +171,9 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int qn = q0 + 8 * i + qc + e;
-            const int64_t at = (static_cast<int64_t>(b) * p.H + h) * p.Tq + qn;
-            lse_c[2 * i + e] = (!masked || qn < p.Tq) ? __ldg(p.lse + at) : 0.f;
-            dlt_c[2 * i + e] = (!masked || qn < p.Tq) ? __ldg(p.delta + at) : 0.f;
+            const int64_t at = lse0 + qn;
+            lse_c[2 * i + e] = (!masked || qn < tq) ? __ldg(p.lse + at) : 0.f;
+            dlt_c[2 * i + e] = (!masked || qn < tq) ? __ldg(p.delta + at) : 0.f;
           }
         }
 #pragma unroll
@@ -168,7 +184,7 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
             for (int e = 0; e < 2; ++e) {
               const int qn = q0 + 8 * i + qc + e;
               const int key = key_abs[hh];
-              const bool vis = !masked || (qn < p.Tq && key < kv_valid && (!p.causal || key <= qn));
+              const bool vis = !masked || (qn < tq && key < kv_valid && (!p.causal || key <= qn));
               const int x = 4 * i + 2 * hh + e;
               const float pe = vis ? fast_exp2(fmaf(s[x], c, -lse_c[2 * i + e])) : 0.f;
               dp[x] = pe * (dp[x] - dlt_c[2 * i + e]);
@@ -232,13 +248,13 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     retire_dkdv(n_iter - 1);
   }
 
-  // ---- dK (scaled), dV: key rows past Tkv are not written
+  // ---- dK (scaled), dV: key rows past the sample's keys are not written
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int key = kv0 + key_loc + 8 * hh;
-    if (key < p.Tkv) {
-      T* dvp = static_cast<T*>(p.dv) + (static_cast<int64_t>(b) * p.Tkv + key) * p.lddv + h * HD + qc;
-      T* dkp = static_cast<T*>(p.dk) + (static_cast<int64_t>(b) * p.Tkv + key) * p.lddk + h * HD + qc;
+    if (key < tkv) {
+      T* dvp = static_cast<T*>(p.dv) + (static_cast<int64_t>(kv_row0) + key) * p.lddv + h * HD + qc;
+      T* dkp = static_cast<T*>(p.dk) + (static_cast<int64_t>(kv_row0) + key) * p.lddk + h * HD + qc;
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         *reinterpret_cast<uint32_t*>(dvp + 8 * i) = Act16<T>::pack2(dv[4 * i + 2 * hh], dv[4 * i + 2 * hh + 1]);
@@ -268,9 +284,14 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
 
   const uint32_t sQ = ptx::smem_u32(smem_raw), sdO = sQ + DQ_TILE;
   const uint32_t sKV = sdO + DQ_TILE;   // stage s: K at sKV + s*32K, V right after K
-  const int qblk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int h = blockIdx.y;
+  int qblk = blockIdx.x, b = blockIdx.z;
+  if (p.q_off) { b = p.tiles[2 * blockIdx.x]; qblk = p.tiles[2 * blockIdx.x + 1]; }
   const int q_base = qblk * DQ_BQ;
-  int kv_valid = p.Tkv;
+  const int q_row0 = p.q_off ? p.q_off[b] : b * p.Tq;
+  const int tq = p.q_off ? p.q_off[b + 1] - q_row0 : p.Tq;
+  const int kv_row0 = p.kv_off ? p.kv_off[b] : b * p.Tkv;
+  int kv_valid = p.kv_off ? p.kv_off[b + 1] - kv_row0 : p.Tkv;
   if (p.kv_len) kv_valid = min(kv_valid, max(1, p.kv_len[b]));
   const int kv_end = p.causal ? min(kv_valid, q_base + DQ_BQ) : kv_valid;
   const int n_kv = (kv_end + DQ_BKV - 1) / DQ_BKV;   // >= 1
@@ -293,13 +314,13 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
     const uint32_t full = ptx::smem_u32(&bar_full[st]);
     const uint32_t dst = sKV + st * 2 * DQ_TILE;
     ptx::mbar_arrive_expect_tx(full, 2 * DQ_TILE);
-    ptx::tma_load_2d(dst, &tmK, full, h * HD, b * p.Tkv + j * DQ_BKV);
-    ptx::tma_load_2d(dst + DQ_TILE, &tmV, full, h * HD, b * p.Tkv + j * DQ_BKV);
+    ptx::tma_load_2d(dst, &tmK, full, h * HD, kv_row0 + j * DQ_BKV);
+    ptx::tma_load_2d(dst + DQ_TILE, &tmV, full, h * HD, kv_row0 + j * DQ_BKV);
   };
   if (threadIdx.x == 0) {
     ptx::mbar_arrive_expect_tx(ptx::smem_u32(&bar_q), 2 * DQ_TILE);
-    ptx::tma_load_2d(sQ, &tmQ, ptx::smem_u32(&bar_q), h * HD, b * p.Tq + q_base);
-    ptx::tma_load_2d(sdO, &tmdO, ptx::smem_u32(&bar_q), h * HD, b * p.Tq + q_base);
+    ptx::tma_load_2d(sQ, &tmQ, ptx::smem_u32(&bar_q), h * HD, q_row0 + q_base);
+    ptx::tma_load_2d(sdO, &tmdO, ptx::smem_u32(&bar_q), h * HD, q_row0 + q_base);
     for (int j = 0; j < min(STAGES, n_kv); ++j) load_kv(j);
   }
 
@@ -313,11 +334,12 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
   const uint64_t do_desc = ptx::desc_sw128(sdO + wg * 8192, 16, 1024);
   float lse_r[2], dlt_r[2];
   bool q_ok[2];
+  const int64_t lse0 = p.q_off ? static_cast<int64_t>(h) * p.Tq + q_row0 : (static_cast<int64_t>(b) * p.H + h) * p.Tq;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int qi = q_base + r_loc + 8 * hh;
-    q_ok[hh] = qi < p.Tq;
-    const int64_t at = (static_cast<int64_t>(b) * p.H + h) * p.Tq + qi;
+    q_ok[hh] = qi < tq;
+    const int64_t at = lse0 + qi;
     lse_r[hh] = q_ok[hh] ? __ldg(p.lse + at) : 0.f;
     dlt_r[hh] = q_ok[hh] ? __ldg(p.delta + at) : 0.f;
   }
@@ -414,7 +436,7 @@ attention_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     if (!q_ok[hh]) continue;
-    T* dst = static_cast<T*>(p.dq) + (static_cast<int64_t>(b) * p.Tq + q_base + r_loc + 8 * hh) * p.lddq + h * HD + kc;
+    T* dst = static_cast<T*>(p.dq) + (static_cast<int64_t>(q_row0) + q_base + r_loc + 8 * hh) * p.lddq + h * HD + kc;
 #pragma unroll
     for (int i = 0; i < 8; ++i)
       *reinterpret_cast<uint32_t*>(dst + 8 * i) = Act16<T>::pack2(dq[4 * i + 2 * hh] * p.scale, dq[4 * i + 2 * hh + 1] * p.scale);
@@ -452,11 +474,14 @@ __global__ void attention_delta_kernel(const T* __restrict__ o, const T* __restr
   }
 }
 
+// Shapes as attention_fwd (attention_fwd_sm90.cu), packed batches included.
 template <typename T>
 int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* o,
                   int64_t ldo, const void* dout, int64_t lddo, const float* lse, float* delta, void* dq, int64_t lddq,
                   void* dk, int64_t lddk, void* dv, int64_t lddv, int64_t B, int64_t H, int64_t Tq, int64_t Tkv,
-                  int64_t head_dim, int causal, const int32_t* kv_len, float scale, void* stream) {
+                  int64_t head_dim, int causal, const int32_t* kv_len, float scale, void* stream,
+                  const int32_t* q_off = nullptr, const int32_t* kv_off = nullptr, const int32_t* tiles = nullptr,
+                  int64_t n_tiles = 0) {
   OASR_REQUIRE(head_dim == HD, "attention_bwd: head_dim %ld unsupported", (long)head_dim);
   OASR_REQUIRE(B > 0 && H > 0 && Tq > 0 && Tkv > 0, "attention_bwd: empty problem");
   OASR_REQUIRE(((ldq | ldk | ldv | ldo | lddo | lddq | lddk | lddv) & 7) == 0, "attention_bwd: strides must be multiples of 8");
@@ -467,24 +492,30 @@ int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const 
   OASR_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15) == 0, "attention_bwd: O must be 16-byte aligned");
   OASR_REQUIRE(!causal || Tq == Tkv, "attention_bwd: causal needs Tq == Tkv");
   OASR_REQUIRE(B <= 65535 && H <= 65535, "attention_bwd: B and H must fit the grid");
+  OASR_REQUIRE(!q_off || (tiles && n_tiles > 0 && n_tiles <= 0x7fffffff), "attention_bwd: a packed batch needs its tile list");
+  OASR_REQUIRE(!kv_off || q_off, "attention_bwd: packed keys need packed queries");
+  OASR_REQUIRE(!causal || !q_off || kv_off == q_off, "attention_bwd: packed causal attention reads keys packed like the queries");
   cudaStream_t st = (cudaStream_t)stream;
+  const uint64_t q_rows = q_off ? Tq : B * Tq, kv_rows = kv_off ? Tkv : B * Tkv;
   CUtensorMap tmQ, tmK, tmV, tmdO, tmQ128, tmdO128;
   constexpr bool f16 = Act16<T>::is_fp16;
   int rc;
-  if ((rc = make_tmap_2d(&tmQ, q, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)ldq * 2, HD, BQ, true, f16))) return rc;
-  if ((rc = make_tmap_2d(&tmK, k, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldk * 2, HD, BKV, true, f16))) return rc;
-  if ((rc = make_tmap_2d(&tmV, v, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldv * 2, HD, BKV, true, f16))) return rc;
-  if ((rc = make_tmap_2d(&tmdO, dout, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)lddo * 2, HD, BQ, true, f16))) return rc;
-  if ((rc = make_tmap_2d(&tmQ128, q, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)ldq * 2, HD, DQ_BQ, true, f16))) return rc;
-  if ((rc = make_tmap_2d(&tmdO128, dout, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)lddo * 2, HD, DQ_BQ, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmQ, q, 2, (uint64_t)(H * HD), q_rows, (uint64_t)ldq * 2, HD, BQ, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmK, k, 2, (uint64_t)(H * HD), kv_rows, (uint64_t)ldk * 2, HD, BKV, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmV, v, 2, (uint64_t)(H * HD), kv_rows, (uint64_t)ldv * 2, HD, BKV, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmdO, dout, 2, (uint64_t)(H * HD), q_rows, (uint64_t)lddo * 2, HD, BQ, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmQ128, q, 2, (uint64_t)(H * HD), q_rows, (uint64_t)ldq * 2, HD, DQ_BQ, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmdO128, dout, 2, (uint64_t)(H * HD), q_rows, (uint64_t)lddo * 2, HD, DQ_BQ, true, f16))) return rc;
 
-  const int64_t n_rows = B * Tq * H;
+  // delta over every query row; a packed batch is one "sample" of N rows, which gives its (1, H, N) layout
+  const int64_t n_rows = (int64_t)q_rows * H;
   attention_delta_kernel<T><<<(unsigned)ceil_div(n_rows * 8, 256), 256, 0, st>>>((const T*)o, (const T*)dout, delta, ldo, lddo,
-                                                                              (int)B, (int)H, (int)Tq);
+                                                                              q_off ? 1 : (int)B, (int)H, (int)Tq);
   OASR_LAUNCH_CHECK();
 
   BwdParams p;
   p.lse = lse; p.delta = delta; p.kv_len = kv_len;
+  p.q_off = q_off; p.kv_off = kv_off; p.tiles = q_off ? tiles : nullptr;
   p.dq = dq; p.dk = dk; p.dv = dv;
   p.lddq = lddq; p.lddk = lddk; p.lddv = lddv;
   p.B = (int)B; p.H = (int)H; p.Tq = (int)Tq; p.Tkv = (int)Tkv; p.causal = causal;
@@ -495,10 +526,13 @@ int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const 
     OASR_CUDA_OK(cudaFuncSetAttribute(attention_bwd_dq_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, DQ_SMEM));
     attr_set = true;
   }
-  const dim3 grid((unsigned)ceil_div(Tkv, BKV), (unsigned)H, (unsigned)B);
+  // packed keys share the query tiles' list (BKV == DQ_BQ == 128 rows); dense keys: every key tile of every sample
+  static_assert(BKV == DQ_BQ, "packed self-attention runs dK / dV and dQ over one tile list");
+  const dim3 grid = kv_off ? dim3((unsigned)n_tiles, (unsigned)H, 1u) : dim3((unsigned)ceil_div(Tkv, BKV), (unsigned)H, (unsigned)B);
   attention_bwd_kernel<T><<<grid, BWD_THREADS, BWD_SMEM, st>>>(tmQ, tmK, tmV, tmdO, p);
   OASR_LAUNCH_CHECK();
-  const dim3 grid_dq((unsigned)ceil_div(Tq, DQ_BQ), (unsigned)H, (unsigned)B);
+  const dim3 grid_dq = q_off ? dim3((unsigned)n_tiles, (unsigned)H, 1u)
+                             : dim3((unsigned)ceil_div(Tq, DQ_BQ), (unsigned)H, (unsigned)B);
   attention_bwd_dq_kernel<T><<<grid_dq, BWD_THREADS, DQ_SMEM, st>>>(tmQ128, tmK, tmV, tmdO128, p);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
@@ -525,4 +559,17 @@ extern "C" int oasr_attention_bwd16(const void* q, int64_t ldq, const void* k, i
                                     int64_t head_dim, int causal, const int32_t* kv_len, float scale, int dtype, void* stream) {
   return OASR_BY_DTYPE16(dtype, attention_bwd, q, ldq, k, ldk, v, ldv, o, ldo, dout, lddo, lse, delta, dq, lddq, dk, lddk, dv,
                          lddv, B, H, Tq, Tkv, head_dim, causal, kv_len, scale, stream);
+}
+
+extern "C" int oasr_attention_bwd_varlen16(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                           int64_t ldv, const void* o, int64_t ldo, const void* dout, int64_t lddo,
+                                           const float* lse, float* delta, void* dq, int64_t lddq, void* dk, int64_t lddk,
+                                           void* dv, int64_t lddv, int64_t B, int64_t H, int64_t N, int64_t Tkv,
+                                           int64_t head_dim, const int32_t* cu_seqlens, const int32_t* kv_cu_seqlens,
+                                           const int32_t* tiles, int64_t n_tiles, float scale, int dtype, void* stream) {
+  OASR_REQUIRE(cu_seqlens, "attention_bwd_varlen: cu_seqlens is required");
+  const int causal = kv_cu_seqlens != nullptr;
+  return OASR_BY_DTYPE16(dtype, attention_bwd, q, ldq, k, ldk, v, ldv, o, ldo, dout, lddo, lse, delta, dq, lddq, dk, lddk, dv,
+                         lddv, B, H, N, causal ? N : Tkv, head_dim, causal, nullptr, scale, stream, cu_seqlens, kv_cu_seqlens,
+                         tiles, n_tiles);
 }

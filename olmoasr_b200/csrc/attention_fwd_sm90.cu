@@ -18,6 +18,12 @@
 // software-pipelined one tile deep: S_{j+1} and O += P_j V_j are issued together and the exponentials of tile j + 1 run
 // (in place, in fp32) while P_j V_j is still on the tensor cores; P_{j+1} is packed to 16 bits once P_j V_j retires.  The arithmetic (tile sizes, k16 order, masks, exp2) is that of the
 // unpipelined loop, so the results are bit-for-bit the same.  The output leaves straight from the O fragment.
+//
+// Packed (varlen) batches: with q_off set, sample b's query rows are rows [q_off[b], q_off[b+1]) of Q / O, Tq is their
+// total N, LSE is (1, H, N), and the grid runs one CTA per entry of `tiles` (sample, 128-row tile) instead of
+// (tile, head, sample).  kv_off set: K / V are packed the same way (causal self-attention, the sample's own keys); unset:
+// sample b's keys are dense rows [b Tkv, b Tkv + Tkv).  A tile's TMA box may reach into the next sample's rows; those are
+// masked (keys) or never stored (queries), so every O / LSE store is guarded by the sample's own length.
 #include "common.cuh"
 #include "ptx_sm90.cuh"
 
@@ -43,6 +49,9 @@ struct AttnParams {
   int B, H, Tq, Tkv;
   int causal;
   float scale_log2;  // scale * log2(e)
+  const int32_t* q_off;   // (B+1,) packed query row offsets, nullable (dense: sample b at rows b Tq)
+  const int32_t* kv_off;  // (B+1,) packed key row offsets, nullable (dense: sample b at rows b Tkv)
+  const int32_t* tiles;   // (sample, query tile) int32 pairs, one per CTA when q_off is set (4-byte aligned)
 };
 
 __device__ __forceinline__ float quad_max(float v) {
@@ -54,7 +63,8 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-template <typename T>
+// PACKED: the packed-batch form.  A compile-time switch, so that the dense instantiation is the dense kernel as it was.
+template <typename T, bool PACKED>
 __global__ void __launch_bounds__(THREADS, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
@@ -67,9 +77,14 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 
   const uint32_t sQ = ptx::smem_u32(smem_raw);
   const uint32_t sKV = sQ + TILE_BYTES;   // stage s: K at sKV + s*32K, V right after K
-  const int qblk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int qblk = PACKED ? p.tiles[2 * blockIdx.x + 1] : blockIdx.x, h = blockIdx.y;
+  const int b = PACKED ? p.tiles[2 * blockIdx.x] : blockIdx.z;
   const int q_base = qblk * BQ;
-  int kv_valid = p.Tkv;
+  const int q_row0 = PACKED ? p.q_off[b] : b * p.Tq;                   // first Q / O row of the sample
+  const int tq = PACKED ? p.q_off[b + 1] - q_row0 : p.Tq;              // its query rows
+  const bool kv_packed = PACKED && p.kv_off;
+  const int kv_row0 = kv_packed ? p.kv_off[b] : b * p.Tkv;
+  int kv_valid = kv_packed ? p.kv_off[b + 1] - kv_row0 : p.Tkv;
   if (p.kv_len) kv_valid = min(kv_valid, max(1, p.kv_len[b]));
   const int kv_end = p.causal ? min(kv_valid, q_base + BQ) : kv_valid;
   const int n_kv = (kv_end + BKV - 1) / BKV;   // >= 1: every sample has at least one visible key
@@ -89,15 +104,16 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     // ===================== TMA producer =====================
     if (threadIdx.x == 0) {
       ptx::mbar_arrive_expect_tx(ptx::smem_u32(&bar_q), TILE_BYTES);
-      ptx::tma_load_2d(sQ, &tmQ, ptx::smem_u32(&bar_q), h * HD, b * p.Tq + q_base);
+      ptx::tma_load_2d(sQ, &tmQ, ptx::smem_u32(&bar_q), h * HD, PACKED ? q_row0 + q_base : b * p.Tq + q_base);
       for (int j = 0; j < n_kv; ++j) {
         const int st = j % STAGES;
         ptx::mbar_wait(ptx::smem_u32(&bar_empty[st]), ((j / STAGES) & 1) ^ 1);
         const uint32_t full = ptx::smem_u32(&bar_full[st]);
         const uint32_t dst = sKV + st * 2 * TILE_BYTES;
         ptx::mbar_arrive_expect_tx(full, 2 * TILE_BYTES);
-        ptx::tma_load_2d(dst, &tmK, full, h * HD, b * p.Tkv + j * BKV);
-        ptx::tma_load_2d(dst + TILE_BYTES, &tmV, full, h * HD, b * p.Tkv + j * BKV);
+        const int row = kv_packed ? kv_row0 + j * BKV : b * p.Tkv + j * BKV;   // dense: the expression as written before
+        ptx::tma_load_2d(dst, &tmK, full, h * HD, row);
+        ptx::tma_load_2d(dst + TILE_BYTES, &tmV, full, h * HD, row);
       }
     }
     return;
@@ -217,50 +233,65 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   issue_pv(n_kv - 1);
   retire_pv(n_kv - 1);
 
-  // ---- output: O / l -> T, rows past Tq are not written; lse in the log2 domain
+  // ---- output: O / l -> T, rows past the sample's length are not written; lse in the log2 domain
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const float lsum = quad_sum(l[hh]);
     const float inv = 1.f / lsum;
     const int qi = q_base + r_loc + 8 * hh;
-    if (qi < p.Tq) {
-      T* dst = static_cast<T*>(p.o) + (static_cast<int64_t>(b) * p.Tq + qi) * p.ldo + h * HD + 2 * (lane & 3);
+    if (qi < tq) {
+      const int64_t row = PACKED ? static_cast<int64_t>(q_row0) + qi : static_cast<int64_t>(b) * p.Tq + qi;
+      T* dst = static_cast<T*>(p.o) + row * p.ldo + h * HD + 2 * (lane & 3);
 #pragma unroll
       for (int i = 0; i < 8; ++i)
         *reinterpret_cast<uint32_t*>(dst + 8 * i) = Act16<T>::pack2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
-      if (p.lse && (lane & 3) == 0) p.lse[(static_cast<int64_t>(b) * p.H + h) * p.Tq + qi] = m[hh] * c + log2f(lsum);
+      if (p.lse && (lane & 3) == 0)
+        p.lse[(PACKED ? static_cast<int64_t>(h) * p.Tq + q_row0 : (static_cast<int64_t>(b) * p.H + h) * p.Tq) + qi] =
+            m[hh] * c + log2f(lsum);
     }
   }
 }
 
+// Dense: B samples of Tq query and Tkv key rows.  Packed (q_off set): Tq is the total N of packed query rows, kv_off set
+// makes Tkv the total of packed key rows, unset keeps B dense samples of Tkv keys; one CTA per (tiles entry, head).
 template <typename T>
 int attention_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o, int64_t ldo,
                   float* lse, int64_t B, int64_t H, int64_t Tq, int64_t Tkv, int64_t head_dim, int causal,
-                  const int32_t* kv_len, float scale, void* stream) {
+                  const int32_t* kv_len, float scale, void* stream, const int32_t* q_off = nullptr,
+                  const int32_t* kv_off = nullptr, const int32_t* tiles = nullptr, int64_t n_tiles = 0) {
   OASR_REQUIRE(head_dim == HD, "attention: head_dim %ld unsupported (every OLMoASR variant uses 64)", (long)head_dim);
   OASR_REQUIRE(B > 0 && H > 0 && Tq > 0 && Tkv > 0, "attention: empty problem");
   OASR_REQUIRE((ldq & 7) == 0 && (ldk & 7) == 0 && (ldv & 7) == 0 && (ldo & 7) == 0, "attention: strides must be multiples of 8");
   OASR_REQUIRE((reinterpret_cast<uintptr_t>(o) & 3) == 0, "attention: output must be 4-byte aligned");
   OASR_REQUIRE(!causal || Tq == Tkv, "attention: causal needs Tq == Tkv");
   OASR_REQUIRE(B <= 65535 && H <= 65535, "attention: B and H must fit the grid");
+  OASR_REQUIRE(!q_off || (tiles && n_tiles > 0 && n_tiles <= 0x7fffffff), "attention: a packed batch needs its tile list");
+  OASR_REQUIRE(!kv_off || q_off, "attention: packed keys need packed queries");
+  OASR_REQUIRE(!causal || !q_off || kv_off == q_off, "attention: packed causal attention reads keys packed like the queries");
+  const uint64_t q_rows = q_off ? Tq : B * Tq, kv_rows = kv_off ? Tkv : B * Tkv;
   CUtensorMap tmQ, tmK, tmV;
   constexpr bool f16 = Act16<T>::is_fp16;
   int rc;
-  if ((rc = make_tmap_2d(&tmQ, q, 2, (uint64_t)(H * HD), (uint64_t)(B * Tq), (uint64_t)ldq * 2, HD, BQ, true, f16))) return rc;
-  if ((rc = make_tmap_2d(&tmK, k, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldk * 2, HD, BKV, true, f16))) return rc;
-  if ((rc = make_tmap_2d(&tmV, v, 2, (uint64_t)(H * HD), (uint64_t)(B * Tkv), (uint64_t)ldv * 2, HD, BKV, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmQ, q, 2, (uint64_t)(H * HD), q_rows, (uint64_t)ldq * 2, HD, BQ, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmK, k, 2, (uint64_t)(H * HD), kv_rows, (uint64_t)ldk * 2, HD, BKV, true, f16))) return rc;
+  if ((rc = make_tmap_2d(&tmV, v, 2, (uint64_t)(H * HD), kv_rows, (uint64_t)ldv * 2, HD, BKV, true, f16))) return rc;
   AttnParams p;
   p.o = o; p.ldo = ldo;
   p.lse = lse; p.kv_len = kv_len;
+  p.q_off = q_off; p.kv_off = kv_off; p.tiles = q_off ? tiles : nullptr;
   p.B = (int)B; p.H = (int)H; p.Tq = (int)Tq; p.Tkv = (int)Tkv; p.causal = causal;
   p.scale_log2 = scale * 1.4426950408889634f;
   static bool attr_set = false;
   if (!attr_set) {
-    OASR_CUDA_OK(cudaFuncSetAttribute(attention_fwd_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+    OASR_CUDA_OK(cudaFuncSetAttribute(attention_fwd_kernel<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+    OASR_CUDA_OK(cudaFuncSetAttribute(attention_fwd_kernel<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
     attr_set = true;
   }
-  const dim3 grid((unsigned)ceil_div(Tq, BQ), (unsigned)H, (unsigned)B);
-  attention_fwd_kernel<T><<<grid, THREADS, ATT_SMEM, (cudaStream_t)stream>>>(tmQ, tmK, tmV, p);
+  if (q_off)
+    attention_fwd_kernel<T, true><<<dim3((unsigned)n_tiles, (unsigned)H, 1u), THREADS, ATT_SMEM, (cudaStream_t)stream>>>(tmQ, tmK, tmV, p);
+  else
+    attention_fwd_kernel<T, false><<<dim3((unsigned)ceil_div(Tq, BQ), (unsigned)H, (unsigned)B), THREADS, ATT_SMEM,
+                                     (cudaStream_t)stream>>>(tmQ, tmK, tmV, p);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
 }
@@ -281,4 +312,15 @@ extern "C" int oasr_attention_fwd16(const void* q, int64_t ldq, const void* k, i
                                     int64_t head_dim, int causal, const int32_t* kv_len, float scale, int dtype, void* stream) {
   return OASR_BY_DTYPE16(dtype, attention_fwd, q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, Tq, Tkv, head_dim, causal, kv_len,
                          scale, stream);
+}
+
+extern "C" int oasr_attention_fwd_varlen16(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                           int64_t ldv, void* o, int64_t ldo, float* lse, int64_t B, int64_t H, int64_t N,
+                                           int64_t Tkv, int64_t head_dim, const int32_t* cu_seqlens,
+                                           const int32_t* kv_cu_seqlens, const int32_t* tiles, int64_t n_tiles, float scale,
+                                           int dtype, void* stream) {
+  OASR_REQUIRE(cu_seqlens, "attention_varlen: cu_seqlens is required");
+  const int causal = kv_cu_seqlens != nullptr;
+  return OASR_BY_DTYPE16(dtype, attention_fwd, q, ldq, k, ldk, v, ldv, o, ldo, lse, B, H, N, causal ? N : Tkv, head_dim, causal,
+                         nullptr, scale, stream, cu_seqlens, kv_cu_seqlens, tiles, n_tiles);
 }

@@ -95,15 +95,17 @@ mask_to_kvlen_kernel(const float* __restrict__ mask, int32_t* __restrict__ kv_le
 
 // ------------------------------------------------------------------ embedding
 // x = (token_embedding(ids) + positional_embedding[offset : offset+S]).to(T)   (model.py:728-732)
+// Packed batches (src_rows set): output row r is dense row src_rows[r] = b*S + t of ids.
 template <typename T>
 __global__ void embed_fwd_kernel(const int64_t* __restrict__ ids, const float* __restrict__ emb,
                                  const float* __restrict__ pos, T* __restrict__ out, int64_t rows, int S,
-                                 int d, int pos_offset, int64_t n_rows_emb) {
+                                 int d, int pos_offset, int64_t n_rows_emb, const int32_t* __restrict__ src_rows = nullptr) {
   const int64_t row = blockIdx.x;
   if (row >= rows) return;
-  int64_t id = ids[row];
+  const int64_t src = src_rows ? src_rows[row] : row;
+  int64_t id = ids[src];
   if (id < 0 || id >= n_rows_emb) id = 0;  // guarded like a clamped gather; callers validate ids
-  const int s = static_cast<int>(row % S) + pos_offset;
+  const int s = static_cast<int>(src % S) + pos_offset;
   const float4* e = reinterpret_cast<const float4*>(emb + id * d);
   const float4* p = reinterpret_cast<const float4*>(pos + static_cast<int64_t>(s) * d);
   uint2* o = reinterpret_cast<uint2*>(out + row * d);
@@ -119,34 +121,48 @@ __global__ void embed_fwd_kernel(const int64_t* __restrict__ ids, const float* _
 // One block per row, sums taken in row order so that the result does not depend on scheduling: the block of a row
 // with b == 0 writes dP[s] (sum over the batch), the block of the FIRST row carrying an id writes dE[id] (sum over
 // every row with that id, gathered 128 rows at a time).
+// Packed batches (src_rows / cu set): dx holds the N = rows packed rows, row r being dense row src_rows[r] of ids and
+// sample b owning rows [cu[b], cu[b+1]); the grid covers max(rows, S) blocks.  The sums run over the same rows in the same
+// order as the dense kernel's minus the padded rows.
 constexpr int EMB_COLS = 10;   // columns per thread: 128 threads cover d <= 1280 (every OLMoASR width)
 template <typename T>
 __global__ void __launch_bounds__(128)
 embed_bwd_kernel(const int64_t* __restrict__ ids, const T* __restrict__ dx,
                  float* __restrict__ demb, float* __restrict__ dpos, int64_t rows, int S, int d,
-                 int64_t padding_idx, int64_t n_rows_emb) {
+                 int64_t padding_idx, int64_t n_rows_emb, const int32_t* __restrict__ src_rows = nullptr,
+                 const int32_t* __restrict__ cu = nullptr, int n_seq = 0) {
   __shared__ int64_t s_rows[128];
   __shared__ int s_cnt[4];
   const int64_t row = blockIdx.x;
-  if (row >= rows) return;
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
   if (row < S) {
-    const int64_t batch = rows / S;
-    for (int c = t; c < d; c += blockDim.x) {
-      float v = 0.f;
-      for (int64_t b = 0; b < batch; ++b) v += Act16<T>::to_f(dx[(b * S + row) * d + c]);
-      dpos[row * d + c] += v;
+    if (cu) {
+      for (int c = t; c < d; c += blockDim.x) {
+        float v = 0.f;
+        for (int b = 0; b < n_seq; ++b)
+          if (cu[b] + row < cu[b + 1]) v += Act16<T>::to_f(dx[(cu[b] + row) * d + c]);
+        dpos[row * d + c] += v;
+      }
+    } else {
+      const int64_t batch = rows / S;
+      for (int c = t; c < d; c += blockDim.x) {
+        float v = 0.f;
+        for (int64_t b = 0; b < batch; ++b) v += Act16<T>::to_f(dx[(b * S + row) * d + c]);
+        dpos[row * d + c] += v;
+      }
     }
   }
-  const int64_t id = ids[row];
+  if (row >= rows) return;
+  auto id_of = [&](int64_t r) { return ids[src_rows ? src_rows[r] : r]; };
+  const int64_t id = id_of(row);
   if (id == padding_idx || id < 0 || id >= n_rows_emb) return;
   for (int64_t base = 0; base < row; base += blockDim.x)   // an earlier row with this id owns the sum
-    if (__syncthreads_or(base + t < row && ids[base + t] == id)) return;
+    if (__syncthreads_or(base + t < row && id_of(base + t) == id)) return;
   float acc[EMB_COLS];
 #pragma unroll
   for (int j = 0; j < EMB_COLS; ++j) acc[j] = 0.f;
   for (int64_t base = row; base < rows; base += blockDim.x) {
-    const bool hit = base + t < rows && ids[base + t] == id;
+    const bool hit = base + t < rows && id_of(base + t) == id;
     const unsigned bal = __ballot_sync(0xffffffffu, hit);
     if (lane == 0) s_cnt[warp] = __popc(bal);
     __syncthreads();
@@ -375,6 +391,28 @@ static int embed_bwd(const int64_t* ids, const void* dx, float* demb, float* dpo
   return OASR_OK;
 }
 
+template <typename T>
+static int embed_fwd_packed(const int64_t* ids, const float* emb, const float* pos, void* out, const int32_t* src_rows,
+                            int64_t N, int64_t S, int64_t d, int64_t n_rows_emb, void* stream) {
+  OASR_REQUIRE(src_rows && N > 0 && S > 0 && (d & 3) == 0, "embed_fwd_packed: bad shape");
+  embed_fwd_kernel<T><<<(unsigned)N, 128, 0, (cudaStream_t)stream>>>(ids, emb, pos, (T*)out, N, (int)S, (int)d, 0, n_rows_emb,
+                                                                    src_rows);
+  OASR_LAUNCH_CHECK();
+  return OASR_OK;
+}
+
+template <typename T>
+static int embed_bwd_packed(const int64_t* ids, const void* dx, float* demb, float* dpos, const int32_t* src_rows,
+                            const int32_t* cu, int64_t n_seq, int64_t N, int64_t S, int64_t d, int64_t padding_idx,
+                            int64_t n_rows_emb, void* stream) {
+  OASR_REQUIRE(src_rows && cu && n_seq > 0 && N > 0 && S > 0 && d <= 128 * EMB_COLS, "embed_bwd_packed: bad shape");
+  embed_bwd_kernel<T><<<(unsigned)(N > S ? N : S), 128, 0, (cudaStream_t)stream>>>(ids, (const T*)dx, demb, dpos, N, (int)S,
+                                                                                 (int)d, padding_idx, n_rows_emb, src_rows, cu,
+                                                                                 (int)n_seq);
+  OASR_LAUNCH_CHECK();
+  return OASR_OK;
+}
+
 template <typename E>
 static int im2col_conv1(const float* mel, void* A, int64_t batch, int64_t C, int64_t T, int64_t kpad, void* stream) {
   OASR_REQUIRE(kpad >= 3 * C && (kpad & 7) == 0, "im2col_conv1: kpad must be >= 3C and a multiple of 8");
@@ -489,4 +527,16 @@ extern "C" int oasr_gelu_bwd16(const void* dy, const void* pre, void* out, int64
 }
 extern "C" int oasr_colsum16(const void* dy, float* db, int64_t M, int64_t N, int64_t ld, int dtype, void* stream) {
   return OASR_BY_DTYPE16(dtype, colsum, dy, db, M, N, ld, stream);
+}
+
+extern "C" int oasr_embed_fwd_packed16(const int64_t* ids, const float* emb, const float* pos, void* out,
+                                       const int32_t* src_rows, int64_t N, int64_t S, int64_t d, int64_t n_rows_emb, int dtype,
+                                       void* stream) {
+  return OASR_BY_DTYPE16(dtype, embed_fwd_packed, ids, emb, pos, out, src_rows, N, S, d, n_rows_emb, stream);
+}
+extern "C" int oasr_embed_bwd_packed16(const int64_t* ids, const void* dx, float* demb, float* dpos, const int32_t* src_rows,
+                                       const int32_t* cu_seqlens, int64_t B, int64_t N, int64_t S, int64_t d,
+                                       int64_t padding_idx, int64_t n_rows_emb, int dtype, void* stream) {
+  return OASR_BY_DTYPE16(dtype, embed_bwd_packed, ids, dx, demb, dpos, src_rows, cu_seqlens, B, N, S, d, padding_idx,
+                         n_rows_emb, stream);
 }

@@ -159,6 +159,59 @@ def attention_bwd(q, k, v, o, dout, lse, B, H, Tq, Tkv, causal=False, kv_len=Non
     return dq, dk, dv
 
 
+def _packed_rows(pk, Tkv):
+    """Rows of K / V for a packed attention call: pk.N packed rows (self-attention, Tkv None) or B * Tkv dense rows."""
+    return pk.N if Tkv is None else pk.B * Tkv
+
+
+def attention_fwd_varlen(q, k, v, pk, H, Tkv=None, scale=None, want_lse=True, out=None):
+    """Attention over a packed batch (`pk`, olmoasr_b200._core.PackedBatch): q (N, >=H*64) holds sample b's rows at
+    [pk.cu[b], pk.cu[b+1]).  Tkv None: causal self-attention, k / v packed like q, sample b sees its own keys.  Tkv given:
+    cross-attention over dense k / v (B*Tkv rows, sample b at row b*Tkv).  Returns (out (N, H*64), lse (H, N) f32)."""
+    dt = q.dtype
+    _req(dt in ACT16, "attention_varlen: q must be bf16 or fp16")
+    for t, n in ((q, "q"), (k, "k"), (v, "v")):
+        _bf16_2d(t, n, dt)
+    kv_rows = _packed_rows(pk, Tkv)
+    _req(q.shape[0] == pk.N and k.shape[0] == kv_rows and v.shape[0] == kv_rows, "attention_varlen: row counts")
+    _req(q.shape[1] == H * 64 and k.shape[1] == H * 64 and v.shape[1] == H * 64, "attention_varlen: width must be H*64")
+    if scale is None:
+        scale = 64 ** -0.5
+    if out is None:
+        out = torch.empty((pk.N, H * 64), device=q.device, dtype=dt)
+    lse = torch.empty((H, pk.N), device=q.device, dtype=torch.float32) if want_lse else None
+    call("oasr_attention_fwd_varlen16", ptr(q), q.stride(0), ptr(k), k.stride(0), ptr(v), v.stride(0), ptr(out), out.stride(0),
+         ptr(lse), pk.B, H, pk.N, 0 if Tkv is None else Tkv, 64, ptr(pk.cu), ptr(pk.cu) if Tkv is None else None,
+         ptr(pk.tiles), pk.n_tiles, float(scale), _DTYPE_CODE[dt], stream())
+    return out, lse
+
+
+def attention_bwd_varlen(q, k, v, o, dout, lse, pk, H, Tkv=None, scale=None, dq=None, dk=None, dv=None):
+    """Backward of `attention_fwd_varlen` (same forms); lse is its (H, N) output."""
+    dt = q.dtype
+    _req(dt in ACT16, "attention_bwd_varlen: q must be bf16 or fp16")
+    for t, n in ((q, "q"), (k, "k"), (v, "v"), (o, "o"), (dout, "dout")):
+        _bf16_2d(t, n, dt)
+    kv_rows = _packed_rows(pk, Tkv)
+    _req(q.shape[0] == pk.N and o.shape[0] == pk.N and dout.shape[0] == pk.N and k.shape[0] == kv_rows and
+         v.shape[0] == kv_rows, "attention_bwd_varlen: row counts")
+    if scale is None:
+        scale = 64 ** -0.5
+    dev = q.device
+    if dq is None:
+        dq = torch.empty((pk.N, H * 64), device=dev, dtype=dt)
+    if dk is None:
+        dk = torch.empty((kv_rows, H * 64), device=dev, dtype=dt)
+    if dv is None:
+        dv = torch.empty((kv_rows, H * 64), device=dev, dtype=dt)
+    delta = torch.empty((H, pk.N), device=dev, dtype=torch.float32)
+    call("oasr_attention_bwd_varlen16", ptr(q), q.stride(0), ptr(k), k.stride(0), ptr(v), v.stride(0), ptr(o), o.stride(0),
+         ptr(dout), dout.stride(0), ptr(lse), ptr(delta), ptr(dq), dq.stride(0), ptr(dk), dk.stride(0), ptr(dv), dv.stride(0),
+         pk.B, H, pk.N, 0 if Tkv is None else Tkv, 64, ptr(pk.cu), ptr(pk.cu) if Tkv is None else None,
+         ptr(pk.tiles), pk.n_tiles, float(scale), _DTYPE_CODE[dt], stream())
+    return dq, dk, dv
+
+
 def ce_fwd(logits, targets, V, ignore_index):
     """logits (rows, ld) bf16 / fp16; returns (lse (rows,), lsc (4,)): lsc = [loss sum, target count, bad-target count, -];
     `ce_finalize(lsc)` turns it into the mean loss."""
@@ -205,6 +258,24 @@ def embed_fwd(ids, emb, pos, pos_offset=0, dtype=torch.bfloat16):
 def embed_bwd(ids, dx, demb, dpos, padding_idx):
     B, S = ids.shape
     _call16("oasr_embed_bwd", dx.dtype, ptr(ids), ptr(dx), ptr(demb), ptr(dpos), B, S, dx.shape[1], padding_idx, demb.shape[0], stream())
+
+
+def embed_fwd_packed(ids, emb, pos, pk, dtype=torch.bfloat16):
+    """`embed_fwd` of the packed rows of `pk` only: (N, d) in `dtype`, row r = dense row pk.rows[r] of ids (B, S)."""
+    _req(ids.dtype == torch.int64 and ids.dim() == 2 and ids.is_contiguous(), "embed: ids int64 (B,S)")
+    _req(tuple(ids.shape) == (pk.B, pk.S), "embed_packed: ids shape must match the packed batch")
+    d = emb.shape[1]
+    out = torch.empty((pk.N, d), device=emb.device, dtype=dtype)
+    call("oasr_embed_fwd_packed16", ptr(ids), ptr(emb), ptr(pos), ptr(out), ptr(pk.rows), pk.N, pk.S, d, emb.shape[0],
+         _DTYPE_CODE[dtype], stream())
+    return out
+
+
+def embed_bwd_packed(ids, dx, demb, dpos, pk, padding_idx):
+    """`embed_bwd` from the packed gradient dx (N, d): the same sums in the same order, padded rows left out."""
+    _req(dx.shape[0] == pk.N and dx.is_contiguous(), "embed_bwd_packed: dx (N, d) contiguous")
+    call("oasr_embed_bwd_packed16", ptr(ids), ptr(dx), ptr(demb), ptr(dpos), ptr(pk.rows), ptr(pk.cu), pk.B, pk.N, pk.S,
+         dx.shape[1], padding_idx, demb.shape[0], _DTYPE_CODE[dx.dtype], stream())
 
 
 def cast_bf16(src, dst=None):
