@@ -353,6 +353,22 @@ OASR_API int oasr_convert(const void* src, int src_dtype, void* dst, int dst_dty
 OASR_API int oasr_gemm16(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, int b_layout, void* C,
                          int64_t ldc, void* C2, const float* bias, const void* aux, int64_t ldaux, int64_t M, int64_t N,
                          int64_t K, int epilogue, int split_k, int block_n, int dtype, void* stream);
+/* Low-rank adapters (LoRA).  oasr_gemm_lowrank16: oasr_gemm16 with a low-rank tail in the same fp32 accumulator,
+ *   D[M,N] = epilogue( sum_k A[m,k] B[n,k] + sum_j A2[m,j] B2[n,j] )
+ * A and A2 (M, K2) K-major, B2 stored like B ((N, K2) for b_layout K-major, (K2, N) for MN-major), K2 a multiple of 8
+ * up to 192.  Forward (B K-major): OASR_EPI_BF16, _GELU, _RESIDUAL; dgrad (B MN-major): OASR_EPI_BF16, _RESIDUAL,
+ * _GELU_BWD; no split-K.  A Linear y = x W^T + b + s (x A^T) B^T runs as A2 = T(s x A^T), B2 = B, and its dgrad
+ * dx = dy W + s (dy B) A as A2 = T(s dy B), B2 = A.
+ * oasr_cast_scaled16: dst[r * ld_dst + c] = T(scale * src[r * cols + c]) for an fp32 (rows, cols) src.
+ * oasr_lora_merge_f32: out = W + scale * B A for fp32 W / out (N, K), B (N, r), A (r, K); out may be W; deterministic. */
+OASR_API int oasr_gemm_lowrank16(const void* A, int64_t lda, const void* B, int64_t ldb, int b_layout, const void* A2,
+                                 int64_t lda2, const void* B2, int64_t ldb2, void* C, int64_t ldc, void* C2,
+                                 const float* bias, const void* aux, int64_t ldaux, int64_t M, int64_t N, int64_t K,
+                                 int64_t K2, int epilogue, int block_n, int dtype, void* stream);
+OASR_API int oasr_cast_scaled16(const float* src, int64_t rows, int64_t cols, float scale, void* dst, int64_t ld_dst,
+                                int dtype, void* stream);
+OASR_API int oasr_lora_merge_f32(const float* W, const float* B, const float* A, float scale, float* out, int64_t N,
+                                 int64_t K, int64_t r, void* stream);
 OASR_API int oasr_layernorm_fwd16(const void* x, const float* weight, const float* bias, void* y, float* mean,
                                   float* rstd, int64_t rows, int64_t d, float eps, int dtype, void* stream);
 OASR_API int oasr_layernorm_bwd16(const void* dy, const void* x, const float* weight, const float* mean,

@@ -132,6 +132,73 @@ def linear_wgrad(dy: Tensor, x: Tensor, n_valid: Optional[int] = None, side=None
     return side.run(launch) if side is not None else launch()
 
 
+class _LoraOps:
+    """16-bit operands of the low-rank adapters of one projection site: a Linear, or the fused members of `_FUSED`
+    (member i owns output rows [i*d, (i+1)*d)).  The adapters of the members that have one are stacked along the rank,
+    R = sum of their ranks (member m's slice of the rank is cols[m] = (offset, r)):
+        a  (R, in) = [A_m]          as (R, in) = [s_m A_m]
+        bz (N, R)  = B_m in (rows of m, cols[m]), zero elsewhere; bzs the same with s_m B_m
+    so that u = x as^T is s (x A^T) for every member and y += u bz^T adds each member's term to its own rows only."""
+
+    def __init__(self, linears, dtype):
+        d = linears[0].out_features
+        self.cols = {}
+        R = 0
+        for i, lin in enumerate(linears):
+            if lin.has_lora:
+                self.cols[i] = (R, lin.lora_A.shape[0])
+                R += lin.lora_A.shape[0]
+        self.R = R
+        dev = linears[0].weight.device
+        n_in = linears[0].in_features
+        self.a = torch.empty((R, n_in), device=dev, dtype=dtype)
+        self.a_s = torch.empty((R, n_in), device=dev, dtype=dtype)
+        self.bz = torch.zeros((len(linears) * d, R), device=dev, dtype=dtype)
+        self.bz_s = torch.zeros((len(linears) * d, R), device=dev, dtype=dtype)
+        for i, (off, r) in self.cols.items():
+            lin = linears[i]
+            A, B = lin.lora_A.detach().contiguous(), lin.lora_B.detach().contiguous()
+            K.cast_scaled16(A, 1.0, self.a[off:off + r])
+            K.cast_scaled16(A, lin.lora_scale, self.a_s[off:off + r])
+            K.cast_scaled16(B, 1.0, self.bz[i * d:(i + 1) * d, off:off + r])
+            K.cast_scaled16(B, lin.lora_scale, self.bz_s[i * d:(i + 1) * d, off:off + r])
+
+    @staticmethod
+    def of(linears, cache: "_ShadowCache", dtype):
+        """The site's operands (rebuilt when an adapter changed), or None when no member has an adapter."""
+        ps = [p for lin in linears if lin.has_lora for p in (lin.lora_A, lin.lora_B)]
+        if not ps:
+            return None
+        return cache.get(ps, lambda: _LoraOps(linears, dtype), dtype)
+
+
+def lora_fwd(x: Tensor, w: Tensor, bias: Optional[Tensor], ops: Optional[_LoraOps], *, epi=K.EPI_BF16, aux=None, out=None,
+             u: Optional[Tensor] = None):
+    """(epi(x W^T + b + u bz^T), u) with u = x as^T (M, R) the adapters' low-rank activations (kept for the backward),
+    or (linear_fwd(...), None) without adapters.  `u` may be given preallocated (side-stream launches)."""
+    if ops is None:
+        return linear_fwd(x, w, bias, epi=epi, aux=aux, out=out), None
+    M, Kd = x.shape
+    N = w.shape[0]
+    u = linear_fwd(x, ops.a_s, None, out=u)
+    y = K.gemm_lowrank(x, w, u, ops.bz, M, N, Kd, ops.R, bias=bias, aux=aux, epi=epi, out=out, block_n=_pick_block_n(M, N))
+    return y, u
+
+
+def lora_v(dy: Tensor, ops: Optional[_LoraOps]) -> Optional[Tensor]:
+    """v = dy bz_s (M, R) = s (dy B) per member: the dgrad tail's A2 and the A-gradient's left operand."""
+    return None if ops is None else linear_dgrad(dy, ops.bz_s)
+
+
+def lora_dgrad(dy: Tensor, w: Tensor, ops: Optional[_LoraOps], v: Optional[Tensor], *, epi=K.EPI_BF16, aux=None, out=None):
+    """dx = epi(dy W + v a): the dgrad of a projection with adapters (plain `linear_dgrad` without)."""
+    if ops is None:
+        return linear_dgrad(dy, w, epi=epi, aux=aux, out=out)
+    M, N = dy.shape
+    Kd = w.shape[1]
+    return K.gemm_lowrank(dy, w, v, ops.a, M, Kd, N, ops.R, b_mn=True, epi=epi, aux=aux, out=out, block_n=_pick_block_n(M, Kd))
+
+
 # Projections of a block whose weight gradients one GEMM computes, stacked in this order (d rows each), and whose bias
 # gradients one column sum covers.  The key projections have no bias (model.py:259): their rows of the fused [bq; 0; bv]
 # bias are a gap of the slab that no gradient may ever be written to.
@@ -155,6 +222,16 @@ class _GradDest:
         self.pool = torch.zeros(pool_size, device=device, dtype=torch.float32) if (pool_size and not direct) else None
         self.used = 0
         self.grads: Dict[str, Tensor] = {}
+        # names of the owner's parameters that take a gradient: a frozen one gets no kernel launch at all
+        self.trainable = None if owner is None else {n for n, p in owner.named_parameters() if p.requires_grad}
+
+    def wants(self, key: str) -> bool:
+        """Whether parameter `key` (or, for a fused name of `_FUSED`, any of its members) takes a gradient."""
+        have = self.slab if self.slab is not None else self.trainable   # direct mode: the slab holds what trains
+        if have is None or key in have:
+            return True
+        name, kind = key.rsplit(".", 1)
+        return any(m + "." + kind in have for m in _FUSED.get(name, ()))
 
     def out(self, key: str) -> Optional[Tensor]:
         """The slab view a kernel accumulates `key`'s gradient into, or None: the kernel allocates the gradient."""
@@ -172,8 +249,11 @@ class _GradDest:
         self.used += (shape + 63) // 64 * 64
         return v
 
-    def vec(self, key: str, shape) -> Tensor:
-        """Zero-initialised accumulation target of `key`'s gradient (LayerNorm, embedding and bias vectors)."""
+    def vec(self, key: str, shape) -> Optional[Tensor]:
+        """Zero-initialised accumulation target of `key`'s gradient (LayerNorm, embedding and bias vectors); None when
+        `key` takes no gradient (kernels that accept a null target then skip that reduction)."""
+        if not self.wants(key):
+            return None
         return self.slab[key] if self.slab is not None else self.keep(key, self._zeros(shape))
 
     def _launch(self, fn):
@@ -185,31 +265,54 @@ class _GradDest:
     def bias(self, key: str, dy: Tensor):
         """Column sums of dy (M, n) bf16 into the bias gradient `key`."""
         db = self.vec(key, dy.shape[1])
-        self._launch(lambda: K.colsum_(dy, db, dy.shape[1]))
+        if db is not None:
+            self._launch(lambda: K.colsum_(dy, db, dy.shape[1]))
 
-    def linear(self, name: str, dy: Tensor, x: Tensor):
+    def linear(self, name: str, dy: Tensor, x: Tensor, lora: Optional[tuple] = None):
         """Weight and bias gradients of the Linear `name`, or of the projections `_FUSED[name]`, from the output
-        gradient dy and the input x."""
-        dw = self.weight(name + ".weight", dy, x)
+        gradient dy and the input x; with `lora` = (ops, u, v) also the gradients of the site's adapters.  Only the
+        parameters that take a gradient get one."""
         members = _FUSED.get(name)
+        if lora is not None:
+            self._lora(members or (name,), dy, x, *lora)
+        d = dy.shape[1] // len(members or (name,))
+        if members is not None and not all(self.wants(m + ".weight") for m in members):
+            for i, m in enumerate(members):     # a partly trainable fused weight: one GEMM per trainable member
+                if self.wants(m + ".weight"):
+                    self.weight(m + ".weight", dy[:, i * d:(i + 1) * d], x)
+        elif self.wants(name + ".weight"):
+            self.weight(name + ".weight", dy, x)
         if members is None:
-            return self.bias(name + ".bias", dy)
-        d = dw.shape[0] // len(members)
+            if self.wants(name + ".bias"):
+                self.bias(name + ".bias", dy)
+            return
         if self.slab is not None:      # one column sum per member that has a bias, so no gap of the slab is written
             for i, m in enumerate(members):
                 if m + ".bias" in self.slab:
                     self.bias(m + ".bias", dy[:, i * d:(i + 1) * d])
             return
-        self.bias(name + ".bias", dy)  # one column sum over the whole fused width; every member takes its rows
+        if self.wants(name + ".bias"):
+            self.bias(name + ".bias", dy)  # one column sum over the whole fused width; every member takes its rows
         for i, m in enumerate(members):
             for kind in (".weight", ".bias"):
-                self.grads[m + kind] = self.grads[name + kind][i * d:(i + 1) * d]
+                if name + kind in self.grads:
+                    self.grads[m + kind] = self.grads[name + kind][i * d:(i + 1) * d]
+
+    def _lora(self, members, dy: Tensor, x: Tensor, ops: _LoraOps, u: Tensor, v: Tensor):
+        """dA = v^T x and dB = dy^T u per member, on its slices of v / u (rank columns) and dy (output rows)."""
+        d = dy.shape[1] // len(members)
+        for i, (off, r) in ops.cols.items():
+            m = members[i]
+            if self.wants(m + ".lora_A"):
+                self.weight(m + ".lora_A", v[:, off:off + r], x)
+            if self.wants(m + ".lora_B"):
+                self.weight(m + ".lora_B", dy[:, i * d:(i + 1) * d], u[:, off:off + r])
 
     def grads_for(self, names: Iterable[str]) -> tuple:
         """What autograd receives for these parameters: all None in direct mode, where the slab already holds them."""
         if self.slab is not None:
             return tuple(None for _ in names)
-        return tuple(self.grads[n] for n in names)
+        return tuple(self.grads.get(n) for n in names)
 
     def done(self):
         """Direct mode: tell the owner's gradient synchronisation hook that its slab range is final."""
@@ -415,6 +518,12 @@ class Linear(nn.Linear):
         self._shadow = _ShadowCache()
 
     _slab_view: Optional[Tensor] = None   # set by OLMoASRBase.use_slabs(): a view into the shadow slab
+    lora_scale = 0.0                      # s = alpha / r of the adapter that olmoasr_b200.lora.add_lora registers
+
+    @property
+    def has_lora(self) -> bool:
+        """True when a low-rank adapter (lora_A (r, in), lora_B (out, r)) is registered on this Linear."""
+        return "lora_A" in self._parameters
 
     def weight_bf16(self) -> Tensor:
         return self.weight16(torch.bfloat16)
@@ -431,7 +540,8 @@ class Linear(nn.Linear):
     def forward(self, x: Tensor) -> Tensor:  # inference / hook path (no autograd through the kernels)
         shp = x.shape
         dt = compute_dtype()
-        y = linear_fwd(_as16_2d(x, dt), self.weight16(dt), None if self.bias is None else _f32(self.bias))
+        ops = _LoraOps.of((self,), self.__dict__.setdefault("_lora_shadow", _ShadowCache()), dt) if self.has_lora else None
+        y, _ = lora_fwd(_as16_2d(x, dt), self.weight16(dt), None if self.bias is None else _f32(self.bias), ops)
         return y.view(*shp[:-1], self.out_features)
 
 
@@ -609,33 +719,42 @@ class _BlockFn(torch.autograd.Function):
         H = blk.attn.n_head
         d = x.shape[1]
         sh = blk._shadows(x.dtype)
+        lo = blk._lora_ops(x.dtype)   # site -> _LoraOps of its adapters, or None
+        us = {}                       # site -> low-rank activations u, saved for the backward
         side = _Side(x.device)
         kvc = None
         if xa is not None:   # the cross-attention K/V projection only needs the encoder output: side stream, joined below
             kvc = torch.empty((xa.shape[0], 2 * d), device=x.device, dtype=x.dtype)
-            side.run(lambda: linear_fwd(xa, sh["wckv"], sh["bckv"], out=kvc))
+            ops = lo.get("cross_attn.kv")
+            u = None if ops is None else torch.empty((xa.shape[0], ops.R), device=x.device, dtype=x.dtype)
+            side.run(lambda: lora_fwd(xa, sh["wckv"], sh["bckv"], ops, out=kvc, u=u))
+            us["cross_attn.kv"] = u
         ln1, mean1, rstd1 = K.layernorm_fwd(x, sh["ln1w"], sh["ln1b"])
-        qkv = linear_fwd(ln1, sh["wqkv"], sh["bqkv"])
+        qkv, us["attn.qkv"] = lora_fwd(ln1, sh["wqkv"], sh["bqkv"], lo.get("attn.qkv"))
         ao, lse = _self_attn_fwd(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], B, H, T, causal, kv_len, pk)
-        x1 = linear_fwd(ao, sh["wo"], sh["bo"], epi=K.EPI_BF16_RESIDUAL, aux=x)
+        x1, us["attn.out"] = lora_fwd(ao, sh["wo"], sh["bo"], lo.get("attn.out"), epi=K.EPI_BF16_RESIDUAL, aux=x)
         saved = [x, mean1, rstd1, ln1, qkv, ao, lse, x1]
         if xa is not None:
             lnc, meanc, rstdc = K.layernorm_fwd(x1, sh["lncw"], sh["lncb"])
-            qc = linear_fwd(lnc, sh["wcq"], sh["bcq"])
+            qc, us["cross_attn.query"] = lora_fwd(lnc, sh["wcq"], sh["bcq"], lo.get("cross_attn.query"))
             side.join()
             co, lsec = _cross_attn_fwd(qc, kvc[:, :d], kvc[:, d:], B, H, T, Ta, pk)
-            x2 = linear_fwd(co, sh["wco"], sh["bco"], epi=K.EPI_BF16_RESIDUAL, aux=x1)
+            x2, us["cross_attn.out"] = lora_fwd(co, sh["wco"], sh["bco"], lo.get("cross_attn.out"), epi=K.EPI_BF16_RESIDUAL,
+                                                aux=x1)
             saved += [xa, meanc, rstdc, lnc, qc, kvc, co, lsec, x2]
         else:
             x2 = x1
         ln2, mean2, rstd2 = K.layernorm_fwd(x2, sh["ln2w"], sh["ln2b"])
-        h, g = linear_fwd(ln2, sh["w1"], sh["b1"], epi=K.EPI_BF16_GELU)
-        x3 = linear_fwd(g, sh["w2"], sh["b2"], epi=K.EPI_BF16_RESIDUAL, aux=x2)
+        (h, g), us["mlp.0"] = lora_fwd(ln2, sh["w1"], sh["b1"], lo.get("mlp.0"), epi=K.EPI_BF16_GELU)
+        x3, us["mlp.2"] = lora_fwd(g, sh["w2"], sh["b2"], lo.get("mlp.2"), epi=K.EPI_BF16_RESIDUAL, aux=x2)
         saved += [mean2, rstd2, ln2, h, g]
         if kv_len is not None:
             saved.append(kv_len)
+        sites = [k for k, u in us.items() if u is not None]
+        saved += [us[k] for k in sites]
         ctx.save_for_backward(*saved)
         ctx.blk, ctx.dims, ctx.sh, ctx.pk = blk, (B, T, Ta, H, d, causal, xa is not None, kv_len is not None), sh, pk
+        ctx.lora = lo, sites
         return x3
 
     @staticmethod
@@ -646,6 +765,9 @@ class _BlockFn(torch.autograd.Function):
             sh = blk._shadows(sv[0].dtype)   # FSDP frees and re-gathers the unsharded parameters between forward and backward
         B, T, Ta, H, d, causal, cross, has_len = ctx.dims
         pk = ctx.pk
+        lo, sites = ctx.lora
+        us = dict(zip(sites, sv[len(sv) - len(sites):]))
+        del sv[len(sv) - len(sites):]
         kv_len = sv.pop() if has_len else None
         x, mean1, rstd1, ln1, qkv, ao, lse, x1 = sv[:8]
         if cross:
@@ -658,18 +780,32 @@ class _BlockFn(torch.autograd.Function):
         side = _Side(x.device)
         # hand-over mode takes all bias / LayerNorm gradient vectors (<= 26 d) from one zero fill
         grads = _GradDest(blk, x.device, side, pool_size=32 * d + 4096)
+
+        # Operands allocated here on the main stream and read by side-stream launches (the adapters' v) must outlive
+        # side.join(): dropped earlier, the allocator could hand their memory to a main-stream tensor while the side
+        # stream still reads it.
+        live = []
+
+        def site(name, dy, x_in):
+            """The site's weight / bias / adapter gradients; returns (ops, v) for its dgrad."""
+            ops = lo.get(name)
+            v = lora_v(dy, ops)
+            live.append(v)
+            grads.linear(name, dy, x_in, None if ops is None else (ops, us[name], v))
+            return ops, v
+
         # ---- MLP: x3 = x2 + fc2(gelu(fc1(ln(x2))))
-        grads.linear("mlp.2", dx3, g)
-        dh = linear_dgrad(dx3, sh["w2"], epi=K.EPI_BF16_GELU_BWD, aux=h)
-        grads.linear("mlp.0", dh, ln2)
-        dln2 = linear_dgrad(dh, sh["w1"])
+        ops, v = site("mlp.2", dx3, g)
+        dh = lora_dgrad(dx3, sh["w2"], ops, v, epi=K.EPI_BF16_GELU_BWD, aux=h)
+        ops, v = site("mlp.0", dh, ln2)
+        dln2 = lora_dgrad(dh, sh["w1"], ops, v)
         dx2 = K.layernorm_bwd(dln2, x2, sh["ln2w"], mean2, rstd2, grads.vec("mlp_ln.weight", d), grads.vec("mlp_ln.bias", d),
                               dresidual=dx3)
         dxa = None
         if cross:
             # ---- cross attention: x2 = x1 + out(attn(q(ln(x1)), kv(xa)))
-            grads.linear("cross_attn.out", dx2, co)
-            dco = linear_dgrad(dx2, sh["wco"])
+            ops, v = site("cross_attn.out", dx2, co)
+            dco = lora_dgrad(dx2, sh["wco"], ops, v)
             dqc = torch.empty_like(qc)
             dkvc = torch.empty_like(kvc)
             if pk is not None:
@@ -677,35 +813,38 @@ class _BlockFn(torch.autograd.Function):
                                        dv=dkvc[:, d:])
             else:
                 K.attention_bwd(qc, kvc[:, :d], kvc[:, d:], co, dco, lsec, B, H, T, Ta, dq=dqc, dk=dkvc[:, :d], dv=dkvc[:, d:])
-            grads.linear("cross_attn.query", dqc, lnc)
-            grads.linear("cross_attn.kv", dkvc, xa)         # [dWk; dWv] in one GEMM
+            ops_q, v_q = site("cross_attn.query", dqc, lnc)
+            ops, v = site("cross_attn.kv", dkvc, xa)         # [dWk; dWv] in one GEMM
             # d(loss)/d(xa): every decoder layer contributes one (B*1500, d) term.  Instead of 24 separate tensors that
             # autograd adds pairwise (23 elementwise kernels over 98 MB each at medium), the layers accumulate into ONE buffer
             # through the GEMM's residual epilogue (bf16(buf + bf16(acc)), the rounding autograd's bf16 adds would apply);
             # the layer whose backward runs last hands the sum to autograd.
+            # No dxa at all when the encoder output takes no gradient (a frozen encoder).
             st = ctx.xa_state
-            if st is None:
+            if not ctx.needs_input_grad[9]:
+                pass
+            elif st is None:
                 dxa = torch.empty_like(xa)
-                side.run(lambda: linear_dgrad(dkvc, sh["wckv"], out=dxa))
+                side.run(lambda: lora_dgrad(dkvc, sh["wckv"], ops, v, out=dxa))
             else:
                 first = st["buf"] is None
                 if first:
                     st["buf"] = torch.empty_like(xa)
                 buf = st["buf"]
                 if first:
-                    side.run(lambda: linear_dgrad(dkvc, sh["wckv"], out=buf))
+                    side.run(lambda: lora_dgrad(dkvc, sh["wckv"], ops, v, out=buf))
                 else:
-                    side.run(lambda: linear_dgrad(dkvc, sh["wckv"], epi=K.EPI_BF16_RESIDUAL, aux=buf, out=buf))
+                    side.run(lambda: lora_dgrad(dkvc, sh["wckv"], ops, v, epi=K.EPI_BF16_RESIDUAL, aux=buf, out=buf))
                 st["left"] -= 1
                 dxa = buf if st["left"] == 0 else None
-            dlnc = linear_dgrad(dqc, sh["wcq"])
+            dlnc = lora_dgrad(dqc, sh["wcq"], ops_q, v_q)
             dx1 = K.layernorm_bwd(dlnc, x1, sh["lncw"], meanc, rstdc, grads.vec("cross_attn_ln.weight", d),
                                   grads.vec("cross_attn_ln.bias", d), dresidual=dx2)
         else:
             dx1 = dx2
         # ---- self attention: x1 = x + out(attn(qkv(ln(x))))
-        grads.linear("attn.out", dx1, ao)
-        dao = linear_dgrad(dx1, sh["wo"])
+        ops, v = site("attn.out", dx1, ao)
+        dao = lora_dgrad(dx1, sh["wo"], ops, v)
         dqkv = torch.empty_like(qkv)
         if pk is not None:
             K.attention_bwd_varlen(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ao, dao, lse, pk, H,
@@ -713,12 +852,17 @@ class _BlockFn(torch.autograd.Function):
         else:
             K.attention_bwd(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ao, dao, lse, B, H, T, T, causal=causal, kv_len=kv_len,
                             dq=dqkv[:, :d], dk=dqkv[:, d:2 * d], dv=dqkv[:, 2 * d:])
-        grads.linear("attn.qkv", dqkv, ln1)                 # [dWq; dWk; dWv] in one GEMM
-        dln1 = linear_dgrad(dqkv, sh["wqkv"])
-        dx = K.layernorm_bwd(dln1, x, sh["ln1w"], mean1, rstd1, grads.vec("attn_ln.weight", d), grads.vec("attn_ln.bias", d),
-                             dresidual=dx1)
+        ops, v = site("attn.qkv", dqkv, ln1)                 # [dWq; dWk; dWv] in one GEMM
+        dx = None
+        dw_ln1, db_ln1 = grads.vec("attn_ln.weight", d), grads.vec("attn_ln.bias", d)
+        if ctx.needs_input_grad[8] or dw_ln1 is not None or db_ln1 is not None:   # else nothing below the qkv site trains
+            dln1 = lora_dgrad(dqkv, sh["wqkv"], ops, v)
+            dx = K.layernorm_bwd(dln1, x, sh["ln1w"], mean1, rstd1, dw_ln1, db_ln1, dresidual=dx1)
         side.join()
+        del live
         grads.done()
+        if not ctx.needs_input_grad[8]:
+            dx = None
         return (None, None, None, None, None, None, None, None, dx, dxa, *grads.grads_for(blk._param_names))
 
 
@@ -742,6 +886,8 @@ class ResidualAttentionBlock(nn.Module):
         self._slab_sh16: Optional[Dict[str, Tensor]] = None
         self._direct: Optional[Dict[str, Tensor]] = None
         self._bwd_done_cb = None
+        self._lora_on = False                             # set by olmoasr_b200.lora.add_lora / merge_lora
+        self._lora_cache: Dict[str, _ShadowCache] = {}   # site -> cached adapter operands
 
     def _build_shadows(self, dtype: torch.dtype = torch.bfloat16) -> Dict[str, Tensor]:
         """Every operand the fused block kernels read that derives from a parameter: 16-bit weights of type `dtype` (fused
@@ -771,7 +917,28 @@ class ResidualAttentionBlock(nn.Module):
         if not _is_master(self.attn.query.weight):
             with torch.no_grad():
                 return self._build_shadows(dtype)   # FSDP mixed precision: parameters are transient views, never cached
-        return self._shadow.get([p for _, p in self.named_parameters()], lambda: self._build_shadows(dtype), dtype)
+        base = [p for n, p in self.named_parameters() if ".lora_" not in n]   # adapter updates leave the base shadows alone
+        return self._shadow.get(base, lambda: self._build_shadows(dtype), dtype)
+
+    def _lora_sites(self):
+        """Projection site of the fused block -> its Linears (in `_FUSED` member order)."""
+        a, c = self.attn, self.cross_attn
+        sites = {"attn.qkv": (a.query, a.key, a.value), "attn.out": (a.out,)}
+        if c is not None:
+            sites.update({"cross_attn.query": (c.query,), "cross_attn.kv": (c.key, c.value), "cross_attn.out": (c.out,)})
+        sites.update({"mlp.0": (self.mlp[0],), "mlp.2": (self.mlp[2],)})
+        return sites
+
+    def _lora_ops(self, dtype: torch.dtype) -> Dict[str, _LoraOps]:
+        """Site -> `_LoraOps` for every site with an adapter (empty without adapters)."""
+        if not self._lora_on:
+            return {}
+        out = {}
+        for name, lins in self._lora_sites().items():
+            ops = _LoraOps.of(lins, self._lora_cache.setdefault(name, _ShadowCache()), dtype)
+            if ops is not None:
+                out[name] = ops
+        return out
 
     def forward(self, x: Tensor, xa: Optional[Tensor] = None, mask: Optional[Tensor] = None,
                 kv_cache: Optional[dict] = None, verbose: bool = False, _xa_state: Optional[dict] = None,
@@ -839,12 +1006,15 @@ class _StemFn(torch.autograd.Function):
         B, C, T, T2, d = ctx.dims
         grads = _GradDest(enc, dx0.device)
         dpre2 = K.gelu_bwd(dx0.contiguous(), pre2)
-        grads.keep("conv2.weight", K.unpermute_conv_wgrad(linear_wgrad(dpre2, A2), d, d, out=grads.out("conv2.weight")))
+        if grads.wants("conv2.weight"):
+            grads.keep("conv2.weight", K.unpermute_conv_wgrad(linear_wgrad(dpre2, A2), d, d, out=grads.out("conv2.weight")))
         grads.bias("conv2.bias", dpre2)
-        dA2 = linear_dgrad(dpre2, enc.conv2.weight16(pre2.dtype))
-        dpre1 = K.col2im_conv2_gelu_bwd(dA2, pre1, B, T, T2, d)
-        grads.keep("conv1.weight", K.unpermute_conv_wgrad(linear_wgrad(dpre1, A1), d, C, out=grads.out("conv1.weight")))
-        grads.bias("conv1.bias", dpre1)
+        if grads.wants("conv1.weight") or grads.wants("conv1.bias"):
+            dA2 = linear_dgrad(dpre2, enc.conv2.weight16(pre2.dtype))
+            dpre1 = K.col2im_conv2_gelu_bwd(dA2, pre1, B, T, T2, d)
+            if grads.wants("conv1.weight"):
+                grads.keep("conv1.weight", K.unpermute_conv_wgrad(linear_wgrad(dpre1, A1), d, C, out=grads.out("conv1.weight")))
+            grads.bias("conv1.bias", dpre1)
         grads.done()     # last gradients of the whole backward pass
         return (None, None, *grads.grads_for(("conv1.weight", "conv1.bias", "conv2.weight", "conv2.bias")), None)
 
@@ -926,8 +1096,13 @@ class _EmbedFn(torch.autograd.Function):
         grads, names = _GradDest(ctx.dec, dx.device), ("token_embedding.weight", "positional_embedding")
         # in direct mode a scatter-add straight into the slab, where the tied logits wgrad has already accumulated
         demb, dpos = grads.vec(names[0], eshape), grads.vec(names[1], pshape)
-        if ctx.pk is not None:
+        if demb is None and dpos is None:
+            grads.done()
+            return (None, None, None, None, None, None, None, None)
+        if ctx.pk is not None:        # a null target (frozen) skips its sums
             K.embed_bwd_packed(ids.contiguous(), dx.contiguous(), demb, dpos, ctx.pk, pad)
+        elif dpos is None:
+            K.embed_bwd(ids.contiguous(), dx.contiguous(), demb, None, pad)
         else:
             K.embed_bwd(ids.contiguous(), dx.contiguous(), demb, dpos[offset:], pad)
         grads.done()     # decoder gradients (incl. the tied embedding) are final
@@ -960,7 +1135,8 @@ class _LogitsFn(torch.autograd.Function):
         buf[:, :V].copy_(dlogits)  # `.float()` backward: the gradient enters the matmul in the logits' 16-bit type
         dx = K.gemm(buf[:, :V], emb_bf16, M, d, V, b_mn=True, block_n=_pick_block_n(M, d))
         grads = _GradDest(ctx.dec)
-        grads.weight("token_embedding.weight", buf, x, n_valid=V)
+        if grads.wants("token_embedding.weight"):
+            grads.weight("token_embedding.weight", buf, x, n_valid=V)
         return (dx, *grads.grads_for(("token_embedding.weight",)), None, None)
 
 
@@ -995,7 +1171,8 @@ class _LossHeadFn(torch.autograd.Function):
         K.ce_bwd_(buf, t, lse, lsc, dloss.reshape(1).float().contiguous(), V, ignore_index)
         dx = K.gemm(buf[:, :V], emb_bf16, M, d, V, b_mn=True, block_n=_pick_block_n(M, d))
         grads = _GradDest(ctx.dec)
-        grads.weight("token_embedding.weight", buf, x, n_valid=V)
+        if grads.wants("token_embedding.weight"):
+            grads.weight("token_embedding.weight", buf, x, n_valid=V)
         return (dx, *grads.grads_for(("token_embedding.weight",)), None, None, None, None)
 
 
@@ -1122,12 +1299,17 @@ class OLMoASRBase(nn.Module):
         if d_enc % 64 or self.dims.n_text_state % 64:
             raise ValueError("use_slabs: model widths must be multiples of 64")
 
+        def lora(*lins):   # adapters sit with their site, so a block's parameters stay one run of the layout
+            return [p for lin in lins if lin.has_lora for p in (lin.lora_A, lin.lora_B)]
+
         def mha_items(a: "MultiHeadAttention"):
             d = a.query.weight.shape[0]
-            return [a.out.weight, a.out.bias, a.query.weight, a.key.weight, a.value.weight, a.query.bias, d, a.value.bias]
+            return ([a.out.weight, a.out.bias] + lora(a.out) + [a.query.weight, a.key.weight, a.value.weight, a.query.bias,
+                    d, a.value.bias] + lora(a.query, a.key, a.value))
 
         def block_items(b: "ResidualAttentionBlock"):
-            it = [b.mlp_ln.weight, b.mlp_ln.bias, b.mlp[2].weight, b.mlp[2].bias, b.mlp[0].weight, b.mlp[0].bias]
+            it = [b.mlp_ln.weight, b.mlp_ln.bias, b.mlp[2].weight, b.mlp[2].bias] + lora(b.mlp[2])
+            it += [b.mlp[0].weight, b.mlp[0].bias] + lora(b.mlp[0])
             if b.cross_attn is not None:
                 it += [b.cross_attn_ln.weight, b.cross_attn_ln.bias] + mha_items(b.cross_attn)
             it += [b.attn_ln.weight, b.attn_ln.bias] + mha_items(b.attn)
@@ -1141,36 +1323,56 @@ class OLMoASRBase(nn.Module):
         for b in reversed(list(enc.blocks)):
             layout += block_items(b)
         layout += [enc.conv2.weight, enc.conv2.bias, enc.conv1.weight, enc.conv1.bias]
-        sl = ParamSlabs(self, layout)
+        # Only what trains is laid out.  The zero gap of a [bq; 0; bv] bias stays when both biases train.
+        keep = []
+        for i, it in enumerate(layout):
+            if isinstance(it, int):
+                if layout[i - 1].requires_grad and layout[i + 1].requires_grad:
+                    keep.append(it)
+            elif it.requires_grad:
+                keep.append(it)
+        if not any(not isinstance(it, int) for it in keep):
+            raise ValueError("use_slabs: the model has no trainable parameter")
+        sl = ParamSlabs(self, keep)
         sl.direct_grads = direct_grads
 
         def install_mha(a: "MultiHeadAttention"):
             d = a.query.weight.shape[0]
-            assert sl.adjacent(a.query.weight, a.key.weight, a.value.weight)
-            assert sl.offset[id(a.value.bias)] == sl.offset[id(a.query.bias)] + 2 * d
-            a._slab_fused = (sl.span("S", a.query.weight, 3 * d * d).view(3 * d, d), sl.span("P", a.query.bias, 3 * d))
+            group = (a.query.weight, a.key.weight, a.value.weight, a.query.bias, a.value.bias)
+            if all(p.requires_grad for p in group):   # the fused [Wq;Wk;Wv] / [bq;0;bv] operands ARE slab ranges
+                assert sl.adjacent(a.query.weight, a.key.weight, a.value.weight)
+                assert sl.offset[id(a.value.bias)] == sl.offset[id(a.query.bias)] + 2 * d
+                a._slab_fused = (sl.span("S", a.query.weight, 3 * d * d).view(3 * d, d), sl.span("P", a.query.bias, 3 * d))
+            # else the fused shadow is built from the members' masters (slab views for those that train) and cached
+            # on their versions, which the fused optimizer bumps
             for lin in (a.query, a.key, a.value, a.out):
-                lin._slab_view = sl.shadow(lin.weight)
+                if lin.weight.requires_grad:
+                    lin._slab_view = sl.shadow(lin.weight)
 
         def grad_views(mod: nn.Module) -> Dict[str, Tensor]:   # the gradients its own backward writes, by name
-            return {n: sl.grad(p) for n, p in mod.named_parameters() if not n.startswith("blocks.")}
+            return {n: sl.grad(p) for n, p in mod.named_parameters() if not n.startswith("blocks.") and p.requires_grad}
 
         for b in list(enc.blocks) + list(dec.blocks):
             install_mha(b.attn)
             if b.cross_attn is not None:
                 install_mha(b.cross_attn)
             for lin in (b.mlp[0], b.mlp[2]):
-                lin._slab_view = sl.shadow(lin.weight)
+                if lin.weight.requires_grad:
+                    lin._slab_view = sl.shadow(lin.weight)
             direct = grad_views(b)
             for name, members in _FUSED.items():     # a fused weight gradient is the slab span of its adjacent members
-                if members[0] + ".weight" in direct:
+                if all(m + ".weight" in direct for m in members):
                     w = _attr_by_path(b, members[0]).weight
                     direct[name + ".weight"] = sl.span("G", w, len(members) * w.numel()).view(len(members) * w.shape[0], -1)
-            sh = b._build_shadows()      # slab views throughout: 16-bit weights from S, fp32 vectors from P
-            b._slabs, b._slab_sh, b._slab_sh16, b._direct = sl, sh, None, direct
+            # A block whose base parameters all train reads slab views throughout (16-bit weights from S, fp32 vectors
+            # from P).  Otherwise its frozen weights keep their cached shadows, and its operand dictionary is cached on
+            # the parameters' versions like outside slab mode (_shadows).
+            full = all(p.requires_grad for n, p in b.named_parameters() if ".lora_" not in n)
+            b._slabs, b._slab_sh, b._slab_sh16, b._direct = sl, (b._build_shadows() if full else None), None, direct
         enc._slabs, dec._slabs = sl, sl
         enc._direct, dec._direct = grad_views(enc), grad_views(dec)
-        dec._emb_slab_view = sl.shadow(dec.token_embedding.weight)
+        if dec.token_embedding.weight.requires_grad:
+            dec._emb_slab_view = sl.shadow(dec.token_embedding.weight)
         self._slabs = sl
         if sl.device.type == "cuda":
             sl.sync_shadows()
@@ -1186,7 +1388,9 @@ class OLMoASRBase(nn.Module):
         units.append(([enc.ln_post.weight, enc.ln_post.bias], None))
         units += [(list(b.parameters()), b) for b in reversed(list(enc.blocks))]
         units.append(([enc.conv2.weight, enc.conv2.bias, enc.conv1.weight, enc.conv1.bias], enc))
-        return units
+        # the trainable parameters only (what the slabs hold); a unit with none left drops out
+        units = [([p for p in ps if p.requires_grad], mod) for ps, mod in units]
+        return [(ps, mod) for ps, mod in units if ps]
 
     def embed_audio(self, mel: Tensor):
         return self.encoder(mel)

@@ -134,6 +134,11 @@ _SIGNATURES = {
     # 16-bit activation dtype (OASR_DTYPE_BF16 / OASR_DTYPE_F16) before the stream
     "oasr_gemm16": [c_void_p, c_i64, c_int, c_void_p, c_i64, c_int, c_void_p, c_i64, c_void_p, c_void_p,
                     c_void_p, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_int, c_void_p],
+    # low-rank adapters: tail GEMM, scaled 16-bit cast into a strided destination, merged fp32 weight
+    "oasr_gemm_lowrank16": [c_void_p, c_i64, c_void_p, c_i64, c_int, c_void_p, c_i64, c_void_p, c_i64, c_void_p, c_i64,
+                            c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_void_p],
+    "oasr_cast_scaled16": [c_void_p, c_i64, c_i64, c_float, c_void_p, c_i64, c_int, c_void_p],
+    "oasr_lora_merge_f32": [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_i64, c_i64, c_i64, c_void_p],
     "oasr_layernorm_fwd16": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_float, c_int, c_void_p],
     "oasr_layernorm_bwd16": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                              c_i64, c_i64, c_int, c_void_p],

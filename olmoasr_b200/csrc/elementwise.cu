@@ -135,7 +135,7 @@ embed_bwd_kernel(const int64_t* __restrict__ ids, const T* __restrict__ dx,
   __shared__ int s_cnt[4];
   const int64_t row = blockIdx.x;
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
-  if (row < S) {
+  if (row < S && dpos) {   // a null dpos / demb (a frozen parameter) skips its sums
     if (cu) {
       for (int c = t; c < d; c += blockDim.x) {
         float v = 0.f;
@@ -152,7 +152,7 @@ embed_bwd_kernel(const int64_t* __restrict__ ids, const T* __restrict__ dx,
       }
     }
   }
-  if (row >= rows) return;
+  if (row >= rows || !demb) return;
   auto id_of = [&](int64_t r) { return ids[src_rows ? src_rows[r] : r]; };
   const int64_t id = id_of(row);
   if (id == padding_idx || id < 0 || id >= n_rows_emb) return;

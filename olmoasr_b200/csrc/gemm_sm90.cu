@@ -115,11 +115,14 @@ __device__ __forceinline__ void box_to_global(const uint8_t* box, void* dst, int
   }
 }
 
-template <typename T, int BN, int A_MN, int B_MN, int EPI>
-__global__ void __launch_bounds__(THREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2,
-                  const __grid_constant__ CUtensorMap tmAux, const GemmParams p) {
+// The kernel body.  LR (a compile-time switch; the plain kernels pass false and null tail maps) adds the low-rank tail
+// A2 B2^T: after a tile's k-blocks the operand producer streams kb_tail more k-blocks from tmA2 (A2 (M, K2) K-major) and
+// tmB2 (B2 with B's major) into the same ring, and the consumers accumulate them into the same registers, so every
+// epilogue applies to acc = A B^T + A2 B2^T unchanged.  TMA zero-fills the k columns past K2.
+template <typename T, int BN, int A_MN, int B_MN, int EPI, bool LR>
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
+                                          const CUtensorMap& tmC2, const CUtensorMap& tmAux, const CUtensorMap* tmA2,
+                                          const CUtensorMap* tmB2, const GemmParams& p, int kb_tail) {
   using C = Cfg<BN, EPI>;
   constexpr int STAGES = C::STAGES;
   constexpr int NACC = BN / 2;   // accumulator registers per thread (64 x BN fp32 over 128 threads)
@@ -147,6 +150,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (EPI == OASR_EPI_BF16_GELU) ptx::tma_prefetch_desc(&tmC2);
     }
     if (reads_aux(EPI) && p.tma_aux) ptx::tma_prefetch_desc(&tmAux);
+    if (LR) {
+      ptx::tma_prefetch_desc(tmA2);
+      ptx::tma_prefetch_desc(tmB2);
+    }
     for (int s = 0; s < STAGES; ++s) {
       ptx::mbar_init(ptx::smem_u32(&bar_full[s]), 1);
       ptx::mbar_init(ptx::smem_u32(&bar_empty[s]), 2);   // one arrival per consumer warpgroup
@@ -168,23 +175,28 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         decode_tile(tile, p, m_blk, n_blk, split);
         const int kb0 = split * p.kblocks_per_split;
         const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
-        for (int kb = kb0; kb < kb1; ++kb) {
+        for (int kb = kb0; kb < kb1 + (LR ? kb_tail : 0); ++kb) {
           ptx::mbar_wait(ptx::smem_u32(&bar_empty[stage]), phase ^ 1);
           const uint32_t sa = smem_base + stage * C::STAGE_BYTES;
           const uint32_t sb = sa + A_STAGE_BYTES;
           const uint32_t full = ptx::smem_u32(&bar_full[stage]);
           ptx::mbar_arrive_expect_tx(full, C::STAGE_BYTES);
+          // a tail k-block reads A2 / B2 at k0 = (kb - kb1) * BK instead of A / B at kb * BK, nothing else
+          const bool tail = LR && kb >= kb1;
+          const CUtensorMap* ma = tail ? tmA2 : &tmA;
+          const CUtensorMap* mb = tail ? tmB2 : &tmB;
+          const int k0 = (tail ? kb - kb1 : kb) * BK;
           if (A_MN) {
 #pragma unroll
-            for (int i = 0; i < BM / 64; ++i) ptx::tma_load_2d(sa + i * (BK * 128), &tmA, full, m_blk * BM + i * 64, kb * BK);
+            for (int i = 0; i < BM / 64; ++i) ptx::tma_load_2d(sa + i * (BK * 128), ma, full, m_blk * BM + i * 64, k0);
           } else {
-            ptx::tma_load_2d(sa, &tmA, full, kb * BK, m_blk * BM);
+            ptx::tma_load_2d(sa, ma, full, k0, m_blk * BM);
           }
           if (B_MN) {
 #pragma unroll
-            for (int i = 0; i < BN / 64; ++i) ptx::tma_load_2d(sb + i * (BK * 128), &tmB, full, n_blk * BN + i * 64, kb * BK);
+            for (int i = 0; i < BN / 64; ++i) ptx::tma_load_2d(sb + i * (BK * 128), mb, full, n_blk * BN + i * 64, k0);
           } else {
-            ptx::tma_load_2d(sb, &tmB, full, kb * BK, n_blk * BN);
+            ptx::tma_load_2d(sb, mb, full, k0, n_blk * BN);
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
@@ -251,7 +263,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int kb0 = split * p.kblocks_per_split;
     const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
     int prev = -1;
-    for (int kb = kb0; kb < kb1; ++kb) {
+    for (int kb = kb0; kb < kb1 + (LR ? kb_tail : 0); ++kb) {
       ptx::mbar_wait(ptx::smem_u32(&bar_full[stage]), phase);
       const uint64_t ad = ptx::desc_add(a_desc0, stage * C::STAGE_BYTES);
       const uint64_t bd = ptx::desc_add(b_desc0, stage * C::STAGE_BYTES);
@@ -389,6 +401,24 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (EPI16 && t == 0) ptx::bulk_wait_group<0>();   // the stores read shared memory until they complete
 }
 
+template <typename T, int BN, int A_MN, int B_MN, int EPI>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2,
+                  const __grid_constant__ CUtensorMap tmAux, const GemmParams p) {
+  gemm_body<T, BN, A_MN, B_MN, EPI, false>(tmA, tmB, tmC, tmC2, tmAux, nullptr, nullptr, p, 0);
+}
+
+// D = epi(A B^T + A2 B2^T), A and A2 K-major, B2 with B's major
+template <typename T, int BN, int B_MN, int EPI>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_lowrank_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2,
+                    const __grid_constant__ CUtensorMap tmAux, const __grid_constant__ CUtensorMap tmA2,
+                    const __grid_constant__ CUtensorMap tmB2, const GemmParams p, const int kb_tail) {
+  gemm_body<T, BN, 0, B_MN, EPI, true>(tmA, tmB, tmC, tmC2, tmAux, &tmA2, &tmB2, p, kb_tail);
+}
+
 // split-K: out[m, n] += sum_s ws[s][m][n], splits in order (fp32 atomics would round differently from run to run)
 __global__ void splitk_reduce_kernel(const float* __restrict__ ws, int splits, int M, int N, float* __restrict__ out, int64_t ldc) {
   const int64_t mn = static_cast<int64_t>(M) * N;
@@ -399,9 +429,9 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ ws, int splits, i
   }
 }
 
-// operand maps (A, B) and the 16-bit epilogues' maps (C, C2, aux; zero when unused)
+// operand maps (A, B), the 16-bit epilogues' maps (C, C2, aux) and the low-rank tail's (A2, B2); zero when unused
 struct Maps {
-  CUtensorMap a, b, c, c2, aux;
+  CUtensorMap a, b, c, c2, aux, a2, b2;
 };
 
 template <typename T, int BN, int A_MN, int B_MN, int EPI>
@@ -417,6 +447,42 @@ int launch(const Maps& m, const GemmParams& p, cudaStream_t st) {
   kern<<<grid, THREADS, C::SMEM_BYTES, st>>>(m.a, m.b, m.c, m.c2, m.aux, p);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
+}
+
+template <typename T, int BN, int B_MN, int EPI>
+int launch_lowrank(const Maps& m, const GemmParams& p, int kb_tail, cudaStream_t st) {
+  using C = Cfg<BN, EPI>;
+  auto kern = gemm_lowrank_kernel<T, BN, B_MN, EPI>;
+  static bool attr_set = false;  // per instantiation
+  if (!attr_set) {
+    OASR_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    attr_set = true;
+  }
+  const int grid = p.num_tiles < gemm_sm_budget() ? p.num_tiles : gemm_sm_budget();
+  kern<<<grid, THREADS, C::SMEM_BYTES, st>>>(m.a, m.b, m.c, m.c2, m.aux, m.a2, m.b2, p, kb_tail);
+  OASR_LAUNCH_CHECK();
+  return OASR_OK;
+}
+
+// The pairs a Linear with a low-rank adapter needs, for every tile width: forward (B K-major) BF16, BF16_GELU and
+// BF16_RESIDUAL; dgrad (B MN-major) BF16, BF16_RESIDUAL and BF16_GELU_BWD.
+template <typename T, int BN>
+int dispatch_lowrank(int b_mn, int epi, const Maps& m, const GemmParams& p, int kb_tail, cudaStream_t st) {
+  if (!b_mn) {
+    switch (epi) {
+      case OASR_EPI_BF16: return launch_lowrank<T, BN, 0, OASR_EPI_BF16>(m, p, kb_tail, st);
+      case OASR_EPI_BF16_GELU: return launch_lowrank<T, BN, 0, OASR_EPI_BF16_GELU>(m, p, kb_tail, st);
+      case OASR_EPI_BF16_RESIDUAL: return launch_lowrank<T, BN, 0, OASR_EPI_BF16_RESIDUAL>(m, p, kb_tail, st);
+    }
+  } else {
+    switch (epi) {
+      case OASR_EPI_BF16: return launch_lowrank<T, BN, 1, OASR_EPI_BF16>(m, p, kb_tail, st);
+      case OASR_EPI_BF16_RESIDUAL: return launch_lowrank<T, BN, 1, OASR_EPI_BF16_RESIDUAL>(m, p, kb_tail, st);
+      case OASR_EPI_BF16_GELU_BWD: return launch_lowrank<T, BN, 1, OASR_EPI_BF16_GELU_BWD>(m, p, kb_tail, st);
+    }
+  }
+  set_last_error("gemm_lowrank: no kernel for b_layout=%d epilogue=%d", b_mn, epi);
+  return OASR_ERR_UNSUPPORTED;
 }
 
 // The (operand majors, epilogue) pairs the library calls; each is compiled for every tile width:
@@ -459,7 +525,8 @@ bool tma_addressable(const void* base, int64_t ld) {
 template <typename T>
 int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, int b_layout, void* Cout, int64_t ldc,
          void* C2, const float* bias, const void* aux, int64_t ldaux, int64_t M, int64_t N, int64_t K, int epilogue,
-         int split_k, int block_n, void* stream) {
+         int split_k, int block_n, void* stream, const void* A2 = nullptr, int64_t lda2 = 0, const void* B2 = nullptr,
+         int64_t ldb2 = 0, int64_t K2 = 0) {
   OASR_REQUIRE(M > 0 && N > 0 && K > 0, "gemm: empty problem M=%ld N=%ld K=%ld", (long)M, (long)N, (long)K);
   OASR_REQUIRE(A && B && Cout, "gemm: null operand");
   OASR_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0,
@@ -475,6 +542,14 @@ int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, i
   OASR_REQUIRE(split_k == 1 || epilogue == OASR_EPI_F32_ATOMIC_ADD, "gemm: split_k needs the accumulating fp32 epilogue");
   // C += acc: a bias would be added once per split (each split's partial runs the F32 epilogue)
   OASR_REQUIRE(bias == nullptr || epilogue != OASR_EPI_F32_ATOMIC_ADD, "gemm: the accumulating fp32 epilogue takes no bias");
+  if (A2 != nullptr) {   // low-rank tail: the 16-bit epilogues of a Linear's forward or dgrad, one split
+    OASR_REQUIRE(B2 != nullptr && K2 > 0 && K2 <= 192 && (K2 & 7) == 0,
+                 "gemm_lowrank: K2=%ld must be a multiple of 8 in [8, 192] with both tail operands given", (long)K2);
+    OASR_REQUIRE(a_layout == OASR_K_MAJOR, "gemm_lowrank: A must be K-major");
+    OASR_REQUIRE(!is_f32_epi(epilogue) && split_k == 1, "gemm_lowrank: 16-bit epilogues only, without split-K");
+    OASR_REQUIRE((reinterpret_cast<uintptr_t>(A2) & 15) == 0 && (reinterpret_cast<uintptr_t>(B2) & 15) == 0 &&
+                 (lda2 & 7) == 0 && (ldb2 & 7) == 0, "gemm_lowrank: A2/B2 must be 16-byte aligned with lda2/ldb2 multiples of 8");
+  }
   if (block_n == 0) block_n = (N > 128) ? 256 : (N > 64 ? 128 : 64);
   OASR_REQUIRE(block_n == 64 || block_n == 128 || block_n == 256, "gemm: block_n must be 64/128/256");
 
@@ -505,6 +580,14 @@ int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, i
   else
     rc = make_tmap_2d(&m.b, B, 2, (uint64_t)N, (uint64_t)K, (uint64_t)ldb * 2, 64, BK, true, f16);
   if (rc) return rc;
+  if (A2 != nullptr) {
+    if ((rc = make_tmap_2d(&m.a2, A2, 2, (uint64_t)K2, (uint64_t)M, (uint64_t)lda2 * 2, BK, BM, true, f16))) return rc;
+    if (b_layout == OASR_K_MAJOR)
+      rc = make_tmap_2d(&m.b2, B2, 2, (uint64_t)K2, (uint64_t)N, (uint64_t)ldb2 * 2, BK, block_n, true, f16);
+    else
+      rc = make_tmap_2d(&m.b2, B2, 2, (uint64_t)N, (uint64_t)K2, (uint64_t)ldb2 * 2, 64, BK, true, f16);
+    if (rc) return rc;
+  }
 
   // 16-bit epilogues: outputs and aux move by TMA in 64 x 64 boxes where TMA can address them (clipped at M and N by
   // the maps; an output box past N with N % 8 != 0 is stored by plain copies, see the consumer), by plain bounded
@@ -528,6 +611,12 @@ int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, i
     ws = static_cast<float*>(scratch_alloc(sizeof(float) * p.splits * M * N, st));
     if (!ws) return OASR_ERR_CUDA;
     p.C = ws; p.ldc = N; epilogue = OASR_EPI_F32; p.split_stride = M * N;
+  }
+  if (A2 != nullptr) {
+    const int kb_tail = (int)ceil_div(K2, BK);
+    return block_n == 256 ? dispatch_lowrank<T, 256>(b_layout, epilogue, m, p, kb_tail, st)
+         : block_n == 128 ? dispatch_lowrank<T, 128>(b_layout, epilogue, m, p, kb_tail, st)
+                          : dispatch_lowrank<T, 64>(b_layout, epilogue, m, p, kb_tail, st);
   }
   rc = block_n == 256 ? dispatch<T, 256>(a_layout, b_layout, epilogue, m, p, st)
      : block_n == 128 ? dispatch<T, 128>(a_layout, b_layout, epilogue, m, p, st)
@@ -563,4 +652,13 @@ extern "C" int oasr_gemm16(const void* A, int64_t lda, int a_layout, const void*
                            int64_t K, int epilogue, int split_k, int block_n, int dtype, void* stream) {
   return OASR_BY_DTYPE16(dtype, gemm, A, lda, a_layout, B, ldb, b_layout, Cout, ldc, C2, bias, aux, ldaux, M, N, K, epilogue,
                          split_k, block_n, stream);
+}
+
+extern "C" int oasr_gemm_lowrank16(const void* A, int64_t lda, const void* B, int64_t ldb, int b_layout, const void* A2,
+                                   int64_t lda2, const void* B2, int64_t ldb2, void* Cout, int64_t ldc, void* C2,
+                                   const float* bias, const void* aux, int64_t ldaux, int64_t M, int64_t N, int64_t K,
+                                   int64_t K2, int epilogue, int block_n, int dtype, void* stream) {
+  OASR_REQUIRE(A2 != nullptr, "gemm_lowrank: null tail operand A2");
+  return OASR_BY_DTYPE16(dtype, gemm, A, lda, OASR_K_MAJOR, B, ldb, b_layout, Cout, ldc, C2, bias, aux, ldaux, M, N, K,
+                         epilogue, 1, block_n, stream, A2, lda2, B2, ldb2, K2);
 }

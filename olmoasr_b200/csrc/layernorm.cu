@@ -260,8 +260,9 @@ int layernorm_bwd(const void* dy, const void* x, const float* weight, const floa
   }
 #undef OASR_LN_BWD
   OASR_LAUNCH_CHECK();
-  int rc = add_partials(part, (int)blocks, d, dweight, st);
-  if (rc == OASR_OK) rc = add_partials(part + blocks * d, (int)blocks, d, dbias, st);
+  // a null dweight / dbias (a frozen affine) skips its reduction
+  int rc = dweight ? add_partials(part, (int)blocks, d, dweight, st) : OASR_OK;
+  if (rc == OASR_OK && dbias) rc = add_partials(part + blocks * d, (int)blocks, d, dbias, st);
   scratch_free(part, st);
   return rc;
 }

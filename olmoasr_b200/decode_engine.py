@@ -34,7 +34,7 @@ import math
 from typing import Dict, Optional, Sequence, Tuple
 
 import torch
-from torch import Tensor
+from torch import Tensor, nn
 
 from . import _lib
 from ._lib import (DTYPE_BF16, DTYPE_F16, DTYPE_F32, DecAttnArgs, DecBeamArgs, DecLinearArgs, DecSampleArgs, DecSampleRulesArgs,
@@ -151,10 +151,13 @@ class DecodeEngine:
         sig = tuple((p.data_ptr(), p._version) for p in self._params())
         if sig == self._w_sig:
             return
+        from .lora import effective_weight
         dec, d, T = self.model.decoder, self.d, self.dtype
 
-        def cast(*ps):
-            out = torch.empty((sum(p.shape[0] for p in ps), ps[0].shape[1]), device=self.dev, dtype=T)
+        def cast(*ps, dtype=T):
+            # a Linear with an adapter contributes its effective weight W + s B A
+            ps = [effective_weight(p) if isinstance(p, nn.Module) else p for p in ps]
+            out = torch.empty((sum(p.shape[0] for p in ps), ps[0].shape[1]), device=self.dev, dtype=dtype)
             r = 0
             for p in ps:
                 _convert(p.detach().contiguous(), out[r:r + p.shape[0]])
@@ -166,13 +169,15 @@ class DecodeEngine:
             a, c = blk.attn, blk.cross_attn
             zeros = torch.zeros(d, device=self.dev)
             layers.append(dict(
-                wqkv=cast(a.query.weight, a.key.weight, a.value.weight),
+                wqkv=cast(a.query, a.key, a.value),
                 bqkv=torch.cat([a.query.bias.detach().float(), zeros, a.value.bias.detach().float()]).contiguous(),
-                wo=cast(a.out.weight), bo=a.out.bias.detach().float().contiguous(),
-                wcq=cast(c.query.weight), bcq=c.query.bias.detach().float().contiguous(),
-                wco=cast(c.out.weight), bco=c.out.bias.detach().float().contiguous(),
-                w1=cast(blk.mlp[0].weight), b1=blk.mlp[0].bias.detach().float().contiguous(),
-                w2=cast(blk.mlp[2].weight), b2=blk.mlp[2].bias.detach().float().contiguous(),
+                wo=cast(a.out), bo=a.out.bias.detach().float().contiguous(),
+                wcq=cast(c.query), bcq=c.query.bias.detach().float().contiguous(),
+                wco=cast(c.out), bco=c.out.bias.detach().float().contiguous(),
+                w1=cast(blk.mlp[0]), b1=blk.mlp[0].bias.detach().float().contiguous(),
+                w2=cast(blk.mlp[2]), b2=blk.mlp[2].bias.detach().float().contiguous(),
+                # the bf16 cross K / V weight prepare() runs on the encoder output, when an adapter changes it
+                wckv=cast(c.key, c.value, dtype=torch.bfloat16) if (c.key.has_lora or c.value.has_lora) else None,
                 ln1=(blk.attn_ln.weight.detach(), blk.attn_ln.bias.detach(), blk.attn_ln.eps),
                 lnc=(blk.cross_attn_ln.weight.detach(), blk.cross_attn_ln.bias.detach(), blk.cross_attn_ln.eps),
                 ln2=(blk.mlp_ln.weight.detach(), blk.mlp_ln.bias.detach(), blk.mlp_ln.eps)))
@@ -331,6 +336,8 @@ class DecodeEngine:
         rows = n * self.n_audio_ctx
         for l, blk in enumerate(self.model.decoder.blocks):
             wkv, bkv = blk.cross_attn.fused_kv()
+            if self._w["layers"][l]["wckv"] is not None:
+                wkv = self._w["layers"][l]["wckv"]
             if self.dtype == torch.bfloat16:
                 linear_fwd(xa, wkv, bkv, out=self.cross_kv[l][:rows])
             else:

@@ -86,6 +86,57 @@ def gemm(a, b, M, N, K, *, a_mn=False, b_mn=False, out=None, out2=None, bias=Non
     return out
 
 
+def gemm_lowrank(a, b, a2, b2, M, N, K, K2, *, b_mn=False, out=None, out2=None, bias=None, aux=None, epi=EPI_BF16,
+                 block_n=0):
+    """D[M,N] = epi(A B^T + A2 B2^T): `gemm` (A K-major) with a low-rank tail in the same accumulator.  a2 (M, K2) is
+    K-major, b2 is (N, K2), or (K2, N) when b_mn; K2 a multiple of 8 up to 192; 16-bit epilogues only."""
+    dt = a.dtype
+    _req(dt in ACT16 and b.dtype == dt and a2.dtype == dt and b2.dtype == dt, "gemm_lowrank: operands of one 16-bit type")
+    _req(all(t.is_cuda and t.dim() == 2 and t.stride(1) == 1 for t in (a, b, a2, b2)), "gemm_lowrank: 2-D CUDA, unit inner stride")
+    _req(tuple(a.shape) == (M, K) and tuple(b.shape) == ((K, N) if b_mn else (N, K)), "gemm_lowrank: A / B shapes")
+    _req(tuple(a2.shape) == (M, K2) and tuple(b2.shape) == ((K2, N) if b_mn else (N, K2)), "gemm_lowrank: A2 / B2 shapes")
+    _req(epi in ((EPI_BF16, EPI_BF16_RESIDUAL, EPI_BF16_GELU_BWD) if b_mn else (EPI_BF16, EPI_BF16_GELU, EPI_BF16_RESIDUAL)),
+         f"gemm_lowrank: no kernel for b_mn={b_mn} epilogue {epi}")
+    if out is None:
+        out = torch.empty((M, N), device=a.device, dtype=dt)
+    _req(out.dtype == dt and out.dim() == 2 and out.shape[0] == M and out.shape[1] >= N and out.stride(1) == 1, "gemm_lowrank: out")
+    if epi == EPI_BF16_GELU and out2 is None:
+        out2 = torch.empty_like(out)
+    if aux is not None:
+        _req(aux.dtype == dt and aux.stride(1) == 1 and aux.shape[0] == M, "gemm_lowrank: aux")
+    if bias is not None:
+        _req(bias.dtype == torch.float32 and bias.numel() >= N and bias.is_contiguous(), "gemm_lowrank: bias must be f32")
+    call("oasr_gemm_lowrank16", ptr(a), a.stride(0), ptr(b), b.stride(0), int(b_mn), ptr(a2), a2.stride(0), ptr(b2),
+         b2.stride(0), ptr(out), out.stride(0), ptr(out2), ptr(bias), ptr(aux), aux.stride(0) if aux is not None else 0,
+         M, N, K, K2, epi, block_n, _DTYPE_CODE[dt], stream())
+    if epi == EPI_BF16_GELU:
+        return out, out2
+    return out
+
+
+def cast_scaled16(src, scale, dst):
+    """dst = dst.dtype(scale * src) for an fp32 (rows, cols) src; dst a 2-D 16-bit view with unit inner stride."""
+    _req(src.dtype == torch.float32 and src.is_contiguous() and src.dim() == 2, "cast_scaled16: contiguous 2-D f32 src")
+    _req(dst.dtype in ACT16 and dst.shape == src.shape and dst.stride(1) == 1, "cast_scaled16: 2-D 16-bit dst of src's shape")
+    call("oasr_cast_scaled16", ptr(src), src.shape[0], src.shape[1], float(scale), ptr(dst), dst.stride(0), _DTYPE_CODE[dst.dtype],
+         stream())
+    return dst
+
+
+def lora_merge(w, b, a, scale, out=None):
+    """out = w + scale * b @ a in fp32 (w, out (N, K); b (N, r); a (r, K)); out may be w."""
+    for t, n in ((w, "w"), (b, "b"), (a, "a")):
+        _req(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 2, f"lora_merge: {n} contiguous 2-D f32")
+    N, Kd = w.shape
+    r = a.shape[0]
+    _req(tuple(b.shape) == (N, r) and tuple(a.shape) == (r, Kd), "lora_merge: shapes")
+    if out is None:
+        out = torch.empty_like(w)
+    _req(out.is_contiguous() and out.shape == w.shape and out.dtype == torch.float32, "lora_merge: out")
+    call("oasr_lora_merge_f32", ptr(w), ptr(b), ptr(a), float(scale), ptr(out), N, Kd, r, stream())
+    return out
+
+
 # ----------------------------------------------------------------------------------------------------
 def _bf16_2d(t, name, dtype=torch.bfloat16):
     _req(t.is_cuda and t.dtype == dtype and t.dim() == 2 and t.stride(1) == 1,
@@ -257,7 +308,9 @@ def embed_fwd(ids, emb, pos, pos_offset=0, dtype=torch.bfloat16):
 
 def embed_bwd(ids, dx, demb, dpos, padding_idx):
     B, S = ids.shape
-    _call16("oasr_embed_bwd", dx.dtype, ptr(ids), ptr(dx), ptr(demb), ptr(dpos), B, S, dx.shape[1], padding_idx, demb.shape[0], stream())
+    """demb / dpos may be None (a frozen parameter): that sum is skipped."""
+    _call16("oasr_embed_bwd", dx.dtype, ptr(ids), ptr(dx), ptr(demb), ptr(dpos), B, S, dx.shape[1], padding_idx,
+            0 if demb is None else demb.shape[0], stream())
 
 
 def embed_fwd_packed(ids, emb, pos, pk, dtype=torch.bfloat16):
@@ -275,7 +328,7 @@ def embed_bwd_packed(ids, dx, demb, dpos, pk, padding_idx):
     """`embed_bwd` from the packed gradient dx (N, d): the same sums in the same order, padded rows left out."""
     _req(dx.shape[0] == pk.N and dx.is_contiguous(), "embed_bwd_packed: dx (N, d) contiguous")
     call("oasr_embed_bwd_packed16", ptr(ids), ptr(dx), ptr(demb), ptr(dpos), ptr(pk.rows), ptr(pk.cu), pk.B, pk.N, pk.S,
-         dx.shape[1], padding_idx, demb.shape[0], _DTYPE_CODE[dx.dtype], stream())
+         dx.shape[1], padding_idx, 0 if demb is None else demb.shape[0], _DTYPE_CODE[dx.dtype], stream())
 
 
 def cast_bf16(src, dst=None):
