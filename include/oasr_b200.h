@@ -369,6 +369,29 @@ OASR_API int oasr_cast_scaled16(const float* src, int64_t rows, int64_t cols, fl
                                 int dtype, void* stream);
 OASR_API int oasr_lora_merge_f32(const float* W, const float* B, const float* A, float scale, float* out, int64_t N,
                                  int64_t K, int64_t r, void* stream);
+/* FP8 training GEMMs (per-row dynamic scaling).  Formats: */
+#define OASR_FP8_E4M3 0   /* max 448   */
+#define OASR_FP8_E5M2 1   /* max 57344 */
+/* oasr_gemm_fp8: D[M,N] = epilogue( (a_scale[m] * b_scale[n]) * sum_k A[m,k] B[n,k] ) with bf16 C / C2 / aux and the
+ *   epilogues of oasr_gemm_bf16, the scaling applied to the fp32 accumulator as (acc * a_scale[m]) * b_scale[n] before
+ *   the bias.  A (M, K) and B (N, K) are K-major fp8 (one byte per element) with 16-byte aligned bases, lda / ldb and K
+ *   multiples of 16; a_scale (M,) and b_scale (N,) fp32.  Format pairs (a_fmt x b_fmt): e4m3 x e4m3 with OASR_EPI_BF16,
+ *   _GELU or _RESIDUAL (a Linear's forward, B = W), and e5m2 x e4m3 with OASR_EPI_BF16, _RESIDUAL or _GELU_BWD (its
+ *   dgrad, A = dy, B = W^T); anything else is OASR_ERR_INVALID / OASR_ERR_UNSUPPORTED.  The fp8 products of each
+ *   128-deep k-block are summed in a separate accumulator and added to the fp32 one with IEEE adds.  block_n: 64, 128,
+ *   or 0 (pick).  No split-K.
+ * oasr_quantize_fp8_rows: per-row dynamic quantisation of a 16-bit (rows, cols) matrix x (type `dtype`, row stride ldx):
+ *   amax = max |x[r, :]|, inv = fmax / amax, q[r, c] = fp8(x[r, c] * inv) (round to nearest even, saturating to
+ *   +-fmax), scale[r] = amax / fmax, in fp32 with IEEE division; a zero row gives inv = scale = 1.  With transpose = 1
+ *   the rows of x^T are quantised instead: q is (cols, rows) with row stride ldq and scale has cols entries.  cols (rows
+ *   for transpose) a multiple of 8, x 16-byte aligned with ldx a multiple of 8, q 8-byte aligned with ldq a multiple
+ *   of 8. */
+OASR_API int oasr_gemm_fp8(const void* A, int64_t lda, int a_fmt, const float* a_scale, const void* B, int64_t ldb,
+                           int b_fmt, const float* b_scale, void* C, int64_t ldc, void* C2, const float* bias,
+                           const void* aux, int64_t ldaux, int64_t M, int64_t N, int64_t K, int epilogue, int block_n,
+                           void* stream);
+OASR_API int oasr_quantize_fp8_rows(const void* x, int64_t ldx, int64_t rows, int64_t cols, int dtype, int fmt,
+                                    int transpose, void* q, int64_t ldq, float* scale, void* stream);
 OASR_API int oasr_layernorm_fwd16(const void* x, const float* weight, const float* bias, void* y, float* mean,
                                   float* rstd, int64_t rows, int64_t d, float eps, int dtype, void* stream);
 OASR_API int oasr_layernorm_bwd16(const void* dy, const void* x, const float* weight, const float* mean,

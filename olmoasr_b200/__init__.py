@@ -7,11 +7,11 @@ from typing import Optional, Union
 
 import torch
 
-from . import inf_model, model
+from . import fp8, inf_model, model
 from .audio import load_audio, log_mel_spectrogram, pad_or_trim
 from .config.model_dims import VARIANT_TO_DIMS, ModelDimensions
 
-__all__ = ["load_model", "model", "inf_model", "load_audio", "log_mel_spectrogram", "pad_or_trim", "ModelDimensions",
+__all__ = ["load_model", "model", "inf_model", "fp8", "load_audio", "log_mel_spectrogram", "pad_or_trim", "ModelDimensions",
            "VARIANT_TO_DIMS"]
 
 

@@ -73,13 +73,39 @@ def compute_dtype() -> torch.dtype:
 @contextlib.contextmanager
 def bf16_compute():
     """Run the model in bf16 whatever the autocast state: decode() and transcribe() keep their bf16 encoder and hook
-    path when they are called inside an fp16 autocast region."""
+    path when they are called inside an fp16 autocast region or inside `fp8_autocast()`."""
     global _bf16_pinned
     _bf16_pinned += 1
     try:
         yield
     finally:
         _bf16_pinned -= 1
+
+
+_fp8_on = False   # set inside fp8_autocast(enabled=True)
+
+
+@contextlib.contextmanager
+def fp8_autocast(enabled: bool = True):
+    """Run the forward and dgrad GEMMs of every block projection in FP8 (olmoasr_b200/fp8.py), or, with enabled=False,
+    in bf16 inside an outer FP8 region.  Nests like torch.autocast: the state of the enclosing region comes back on exit."""
+    global _fp8_on
+    prev, _fp8_on = _fp8_on, bool(enabled)
+    try:
+        yield
+    finally:
+        _fp8_on = prev
+
+
+def fp8_enabled() -> bool:
+    """Whether a fused block's forward starting now runs its projections in FP8 (never inside `bf16_compute()`)."""
+    return _fp8_on and _bf16_pinned == 0
+
+
+def fp8_checkpoint_context_fn():
+    """`context_fn` for torch.utils.checkpoint(..., use_reentrant=False): the recompute runs in the FP8 state of the
+    forward, wherever the backward runs (torch restores autocast's state for a recompute, but not this one)."""
+    return contextlib.nullcontext(), fp8_autocast(fp8_enabled())
 
 
 def _f16_kw(dtype: torch.dtype) -> dict:
@@ -106,6 +132,40 @@ def linear_dgrad(dy: Tensor, w_bf16: Tensor, *, epi=K.EPI_BF16, aux=None, out=No
     M, N = dy.shape
     Kd = w_bf16.shape[1]
     return K.gemm(dy, w_bf16, M, Kd, N, b_mn=True, epi=epi, aux=aux, out=out, block_n=_pick_block_n(M, Kd))
+
+
+def _pick_block_n_fp8(M: int, N: int) -> int:
+    """Tile width (128 or 64) of the FP8 GEMM, by `_pick_block_n`'s cost: its temporary accumulator (promotion every
+    128 k) doubles the accumulator registers, which leaves no room for 256-wide tiles."""
+    sms = _sm_count()
+    tiles_m = math.ceil(M / 128)
+    return min((128, 64), key=lambda bn: math.ceil(tiles_m * math.ceil(N / bn) / sms) * (128 + bn))
+
+
+def linear_fwd_fp8(x8, w8, bias: Optional[Tensor], *, epi=K.EPI_BF16, aux=None, out=None):
+    """y = epi(x W^T + b) in FP8: x8 = (q, s) the e4m3 rows of x (M, K), w8 = (q, s) the e4m3 rows of W (N, K)."""
+    (xq, xs), (wq, ws) = x8, w8
+    M, Kd = xq.shape
+    N = wq.shape[0]
+    return K.gemm_fp8(xq, xs, wq, ws, M, N, Kd, bias=bias, aux=aux, epi=epi, out=out, block_n=_pick_block_n_fp8(M, N))
+
+
+def linear_dgrad_fp8(dy8, wt8, *, epi=K.EPI_BF16, aux=None, out=None):
+    """dx = epi(dy W) in FP8: dy8 = (q, s) the e5m2 rows of dy (M, N), wt8 = (q, s) the e4m3 rows of W^T (K, N)."""
+    (dq, ds), (wq, ws) = dy8, wt8
+    M, N = dq.shape
+    Kd = wq.shape[0]
+    return K.gemm_fp8(dq, ds, wq, ws, M, Kd, N, epi=epi, aux=aux, out=out, block_n=_pick_block_n_fp8(M, Kd))
+
+
+def fp8_inputs(xa: Optional[Tensor]) -> dict:
+    """The per-forward FP8 operands shared by the layers of a stack: the e4m3 rows of the encoder output, which feeds
+    every decoder layer's cross K/V projection (None for the encoder)."""
+    return {"xa": None if xa is None else K.quantize_fp8_rows(_as16_2d(xa, torch.bfloat16), K.FP8_E4M3)}
+
+
+# weight operands of a block's projections: forward (W, e4m3 rows) and dgrad (W^T, e4m3 rows = per input feature)
+_FP8_WEIGHTS = ("wqkv", "wo", "wcq", "wckv", "wco", "w1", "w2")
 
 
 def linear_wgrad(dy: Tensor, x: Tensor, n_valid: Optional[int] = None, side=None, out: Optional[Tensor] = None):
@@ -711,42 +771,64 @@ class _BlockFn(torch.autograd.Function):
     size and dense length, the self-attention is causal over each sample's own rows and kv_len is None).
 
     inputs: x, xa (or None), kv_len (or None), then the block's parameters in `ResidualAttentionBlock._param_list`
-    order.  Saves every GEMM input it needs for wgrad; recomputes nothing."""
+    order.  Saves every GEMM input it needs for wgrad; recomputes nothing.
+
+    f8: None, or (inside `fp8_autocast()`) `fp8_inputs(xa)`: every projection's forward then runs as an e4m3 x e4m3 GEMM
+    over per-row quantised operands, and the backward (wherever it runs) its dgrad as e5m2 x e4m3; the wgrads keep
+    reading the saved bf16 activations."""
 
     @staticmethod
-    def forward(ctx, blk, B, T, Ta, causal, kv_len, xa_state, pk, x, xa, *params):
+    def forward(ctx, blk, B, T, Ta, causal, kv_len, xa_state, pk, f8, x, xa, *params):
         ctx.xa_state = xa_state
         H = blk.attn.n_head
         d = x.shape[1]
         sh = blk._shadows(x.dtype)
         lo = blk._lora_ops(x.dtype)   # site -> _LoraOps of its adapters, or None
+        w8 = None
+        if f8 is not None:
+            if x.dtype != torch.bfloat16:
+                raise ValueError("fp8_autocast() computes in bf16: it cannot be combined with torch.autocast(\"cuda\", "
+                                 "torch.float16)")
+            if blk._lora_on:
+                raise ValueError("fp8_autocast() does not support LoRA adapters: train them in bf16, or merge_lora() first")
+            w8 = blk._fp8_weights(sh)
         us = {}                       # site -> low-rank activations u, saved for the backward
+
+        def proj(w, b, site, x_in, x8=None, **kw):
+            """(y, u) of one projection site: bf16 (with its adapters), or FP8 over the e4m3 rows of x_in."""
+            if w8 is None:
+                return lora_fwd(x_in, sh[w], sh[b], lo.get(site), **kw)
+            if x8 is None:
+                x8 = K.quantize_fp8_rows(x_in, K.FP8_E4M3)
+            kw.pop("u", None)    # (no adapters under FP8)
+            return linear_fwd_fp8(x8, w8[w][0], sh[b], **kw), None
+
         side = _Side(x.device)
         kvc = None
         if xa is not None:   # the cross-attention K/V projection only needs the encoder output: side stream, joined below
             kvc = torch.empty((xa.shape[0], 2 * d), device=x.device, dtype=x.dtype)
             ops = lo.get("cross_attn.kv")
             u = None if ops is None else torch.empty((xa.shape[0], ops.R), device=x.device, dtype=x.dtype)
-            side.run(lambda: lora_fwd(xa, sh["wckv"], sh["bckv"], ops, out=kvc, u=u))
+            xa8 = None if f8 is None else f8["xa"]   # quantised on the main stream before the first layer
+            side.run(lambda: proj("wckv", "bckv", "cross_attn.kv", xa, xa8, out=kvc, u=u))
             us["cross_attn.kv"] = u
         ln1, mean1, rstd1 = K.layernorm_fwd(x, sh["ln1w"], sh["ln1b"])
-        qkv, us["attn.qkv"] = lora_fwd(ln1, sh["wqkv"], sh["bqkv"], lo.get("attn.qkv"))
+        qkv, us["attn.qkv"] = proj("wqkv", "bqkv", "attn.qkv", ln1)
         ao, lse = _self_attn_fwd(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], B, H, T, causal, kv_len, pk)
-        x1, us["attn.out"] = lora_fwd(ao, sh["wo"], sh["bo"], lo.get("attn.out"), epi=K.EPI_BF16_RESIDUAL, aux=x)
+        x1, us["attn.out"] = proj("wo", "bo", "attn.out", ao, epi=K.EPI_BF16_RESIDUAL, aux=x)
         saved = [x, mean1, rstd1, ln1, qkv, ao, lse, x1]
         if xa is not None:
             lnc, meanc, rstdc = K.layernorm_fwd(x1, sh["lncw"], sh["lncb"])
-            qc, us["cross_attn.query"] = lora_fwd(lnc, sh["wcq"], sh["bcq"], lo.get("cross_attn.query"))
+            qc, us["cross_attn.query"] = proj("wcq", "bcq", "cross_attn.query", lnc)
             side.join()
             co, lsec = _cross_attn_fwd(qc, kvc[:, :d], kvc[:, d:], B, H, T, Ta, pk)
-            x2, us["cross_attn.out"] = lora_fwd(co, sh["wco"], sh["bco"], lo.get("cross_attn.out"), epi=K.EPI_BF16_RESIDUAL,
-                                                aux=x1)
+            x2, us["cross_attn.out"] = proj("wco", "bco", "cross_attn.out", co, epi=K.EPI_BF16_RESIDUAL, aux=x1)
             saved += [xa, meanc, rstdc, lnc, qc, kvc, co, lsec, x2]
         else:
             x2 = x1
         ln2, mean2, rstd2 = K.layernorm_fwd(x2, sh["ln2w"], sh["ln2b"])
-        (h, g), us["mlp.0"] = lora_fwd(ln2, sh["w1"], sh["b1"], lo.get("mlp.0"), epi=K.EPI_BF16_GELU)
-        x3, us["mlp.2"] = lora_fwd(g, sh["w2"], sh["b2"], lo.get("mlp.2"), epi=K.EPI_BF16_RESIDUAL, aux=x2)
+        (h, g), us["mlp.0"] = proj("w1", "b1", "mlp.0", ln2, epi=K.EPI_BF16_GELU)
+        x3, us["mlp.2"] = proj("w2", "b2", "mlp.2", g, epi=K.EPI_BF16_RESIDUAL, aux=x2)
         saved += [mean2, rstd2, ln2, h, g]
         if kv_len is not None:
             saved.append(kv_len)
@@ -755,14 +837,21 @@ class _BlockFn(torch.autograd.Function):
         ctx.save_for_backward(*saved)
         ctx.blk, ctx.dims, ctx.sh, ctx.pk = blk, (B, T, Ta, H, d, causal, xa is not None, kv_len is not None), sh, pk
         ctx.lora = lo, sites
+        # the FP8 weight copies, for the dgrads; FSDP's unsharded views are gone by the backward, which rebuilds them
+        # from the re-gathered parameters, so only the mode is kept then
+        ctx.fp8 = w8 is not None
+        ctx.w8 = w8 if _is_master(blk.attn.query.weight) else None
         return x3
 
     @staticmethod
     def backward(ctx, dx3):
         blk, sh = ctx.blk, ctx.sh
         sv = list(ctx.saved_tensors)
+        w8 = ctx.w8     # the FP8 weight copies when the forward ran under fp8_autocast()
         if not _is_master(blk.attn.query.weight):
             sh = blk._shadows(sv[0].dtype)   # FSDP frees and re-gathers the unsharded parameters between forward and backward
+            if ctx.fp8:
+                w8 = blk._fp8_weights(sh)
         B, T, Ta, H, d, causal, cross, has_len = ctx.dims
         pk = ctx.pk
         lo, sites = ctx.lora
@@ -794,18 +883,24 @@ class _BlockFn(torch.autograd.Function):
             grads.linear(name, dy, x_in, None if ops is None else (ops, us[name], v))
             return ops, v
 
+        def dgrad(w, dy, ops, v, dy8=None, **kw):
+            """dx of the projection with weight sh[w]: bf16 (with its adapters), or FP8 over the e5m2 rows of dy."""
+            if w8 is None:
+                return lora_dgrad(dy, sh[w], ops, v, **kw)
+            return linear_dgrad_fp8(K.quantize_fp8_rows(dy, K.FP8_E5M2) if dy8 is None else dy8, w8[w][1], **kw)
+
         # ---- MLP: x3 = x2 + fc2(gelu(fc1(ln(x2))))
         ops, v = site("mlp.2", dx3, g)
-        dh = lora_dgrad(dx3, sh["w2"], ops, v, epi=K.EPI_BF16_GELU_BWD, aux=h)
+        dh = dgrad("w2", dx3, ops, v, epi=K.EPI_BF16_GELU_BWD, aux=h)
         ops, v = site("mlp.0", dh, ln2)
-        dln2 = lora_dgrad(dh, sh["w1"], ops, v)
+        dln2 = dgrad("w1", dh, ops, v)
         dx2 = K.layernorm_bwd(dln2, x2, sh["ln2w"], mean2, rstd2, grads.vec("mlp_ln.weight", d), grads.vec("mlp_ln.bias", d),
                               dresidual=dx3)
         dxa = None
         if cross:
             # ---- cross attention: x2 = x1 + out(attn(q(ln(x1)), kv(xa)))
             ops, v = site("cross_attn.out", dx2, co)
-            dco = lora_dgrad(dx2, sh["wco"], ops, v)
+            dco = dgrad("wco", dx2, ops, v)
             dqc = torch.empty_like(qc)
             dkvc = torch.empty_like(kvc)
             if pk is not None:
@@ -821,30 +916,33 @@ class _BlockFn(torch.autograd.Function):
             # the layer whose backward runs last hands the sum to autograd.
             # No dxa at all when the encoder output takes no gradient (a frozen encoder).
             st = ctx.xa_state
-            if not ctx.needs_input_grad[9]:
+            # FP8: dkvc is quantised here, on the main stream, and kept alive until the side stream is joined
+            dk8 = None if (w8 is None or not ctx.needs_input_grad[10]) else K.quantize_fp8_rows(dkvc, K.FP8_E5M2)
+            live.append(dk8)
+            if not ctx.needs_input_grad[10]:
                 pass
             elif st is None:
                 dxa = torch.empty_like(xa)
-                side.run(lambda: lora_dgrad(dkvc, sh["wckv"], ops, v, out=dxa))
+                side.run(lambda: dgrad("wckv", dkvc, ops, v, dk8, out=dxa))
             else:
                 first = st["buf"] is None
                 if first:
                     st["buf"] = torch.empty_like(xa)
                 buf = st["buf"]
                 if first:
-                    side.run(lambda: lora_dgrad(dkvc, sh["wckv"], ops, v, out=buf))
+                    side.run(lambda: dgrad("wckv", dkvc, ops, v, dk8, out=buf))
                 else:
-                    side.run(lambda: lora_dgrad(dkvc, sh["wckv"], ops, v, epi=K.EPI_BF16_RESIDUAL, aux=buf, out=buf))
+                    side.run(lambda: dgrad("wckv", dkvc, ops, v, dk8, epi=K.EPI_BF16_RESIDUAL, aux=buf, out=buf))
                 st["left"] -= 1
                 dxa = buf if st["left"] == 0 else None
-            dlnc = lora_dgrad(dqc, sh["wcq"], ops_q, v_q)
+            dlnc = dgrad("wcq", dqc, ops_q, v_q)
             dx1 = K.layernorm_bwd(dlnc, x1, sh["lncw"], meanc, rstdc, grads.vec("cross_attn_ln.weight", d),
                                   grads.vec("cross_attn_ln.bias", d), dresidual=dx2)
         else:
             dx1 = dx2
         # ---- self attention: x1 = x + out(attn(qkv(ln(x))))
         ops, v = site("attn.out", dx1, ao)
-        dao = lora_dgrad(dx1, sh["wo"], ops, v)
+        dao = dgrad("wo", dx1, ops, v)
         dqkv = torch.empty_like(qkv)
         if pk is not None:
             K.attention_bwd_varlen(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], ao, dao, lse, pk, H,
@@ -855,15 +953,15 @@ class _BlockFn(torch.autograd.Function):
         ops, v = site("attn.qkv", dqkv, ln1)                 # [dWq; dWk; dWv] in one GEMM
         dx = None
         dw_ln1, db_ln1 = grads.vec("attn_ln.weight", d), grads.vec("attn_ln.bias", d)
-        if ctx.needs_input_grad[8] or dw_ln1 is not None or db_ln1 is not None:   # else nothing below the qkv site trains
-            dln1 = lora_dgrad(dqkv, sh["wqkv"], ops, v)
+        if ctx.needs_input_grad[9] or dw_ln1 is not None or db_ln1 is not None:   # else nothing below the qkv site trains
+            dln1 = dgrad("wqkv", dqkv, ops, v)
             dx = K.layernorm_bwd(dln1, x, sh["ln1w"], mean1, rstd1, dw_ln1, db_ln1, dresidual=dx1)
         side.join()
         del live
         grads.done()
-        if not ctx.needs_input_grad[8]:
+        if not ctx.needs_input_grad[9]:
             dx = None
-        return (None, None, None, None, None, None, None, None, dx, dxa, *grads.grads_for(blk._param_names))
+        return (None, None, None, None, None, None, None, None, None, dx, dxa, *grads.grads_for(blk._param_names))
 
 
 class ResidualAttentionBlock(nn.Module):
@@ -888,6 +986,7 @@ class ResidualAttentionBlock(nn.Module):
         self._bwd_done_cb = None
         self._lora_on = False                             # set by olmoasr_b200.lora.add_lora / merge_lora
         self._lora_cache: Dict[str, _ShadowCache] = {}   # site -> cached adapter operands
+        self._fp8_cache = _ShadowCache()                  # FP8 weight copies (fp8_autocast())
 
     def _build_shadows(self, dtype: torch.dtype = torch.bfloat16) -> Dict[str, Tensor]:
         """Every operand the fused block kernels read that derives from a parameter: 16-bit weights of type `dtype` (fused
@@ -920,6 +1019,21 @@ class ResidualAttentionBlock(nn.Module):
         base = [p for n, p in self.named_parameters() if ".lora_" not in n]   # adapter updates leave the base shadows alone
         return self._shadow.get(base, lambda: self._build_shadows(dtype), dtype)
 
+    def _build_fp8_weights(self, sh: Dict[str, Tensor]) -> Dict[str, tuple]:
+        """Weight key of `_FP8_WEIGHTS` -> ((W8, s), (W^T8, s)): the e4m3 rows of the 16-bit operand W (N, K), for the
+        forward, and of W^T (K, N), i.e. one scale per input feature, for the dgrad."""
+        return {k: (K.quantize_fp8_rows(sh[k], K.FP8_E4M3), K.quantize_fp8_rows(sh[k], K.FP8_E4M3, transpose=True))
+                for k in _FP8_WEIGHTS if k in sh}
+
+    def _fp8_weights(self, sh: Dict[str, Tensor]) -> Dict[str, tuple]:
+        """The FP8 weight copies of the 16-bit operands `sh`: rebuilt when a parameter changed (once per optimizer
+        step), or on every call under FSDP, whose unsharded views are transient like the 16-bit operands."""
+        if not _is_master(self.attn.query.weight):
+            with torch.no_grad():
+                return self._build_fp8_weights(sh)
+        base = [p for n, p in self.named_parameters() if ".lora_" not in n]
+        return self._fp8_cache.get(base, lambda: self._build_fp8_weights(sh), torch.float8_e4m3fn)
+
     def _lora_sites(self):
         """Projection site of the fused block -> its Linears (in `_FUSED` member order)."""
         a, c = self.attn, self.cross_attn
@@ -942,13 +1056,15 @@ class ResidualAttentionBlock(nn.Module):
 
     def forward(self, x: Tensor, xa: Optional[Tensor] = None, mask: Optional[Tensor] = None,
                 kv_cache: Optional[dict] = None, verbose: bool = False, _xa_state: Optional[dict] = None,
-                _packed: Optional[PackedBatch] = None):
+                _packed: Optional[PackedBatch] = None, _fp8: Optional[dict] = None):
         if kv_cache is not None:
             return self._forward_cached(x, xa, mask, kv_cache)
+        # inside fp8_autocast(): the FP8 operands the layers share, unless the decoder quantised them for all layers
+        f8 = (_fp8 if _fp8 is not None else fp8_inputs(xa)) if fp8_enabled() else None
         if _packed is not None:      # x: the (N, d) rows of a packed decoder batch (TextDecoder.hidden)
             params = [_attr_by_path(self, n) for n in self._param_names]
             xa2 = _as16_2d(xa, x.dtype)
-            return _BlockFn.apply(self, _packed.B, _packed.S, xa.shape[1], True, None, _xa_state, _packed, x, xa2, *params)
+            return _BlockFn.apply(self, _packed.B, _packed.S, xa.shape[1], True, None, _xa_state, _packed, f8, x, xa2, *params)
         B, T, d = x.shape
         causal, kv_len = False, None
         if mask is not None:
@@ -960,7 +1076,7 @@ class ResidualAttentionBlock(nn.Module):
         xa2 = _as16_2d(xa, dt) if xa is not None else None
         # attribute walk, not get_parameter(): under FSDP the attributes are plain tensor views of the flat parameter
         params = [_attr_by_path(self, n) for n in self._param_names]
-        y = _BlockFn.apply(self, B, T, Ta, causal, kv_len, _xa_state, None, _as16_2d(x, dt), xa2, *params)
+        y = _BlockFn.apply(self, B, T, Ta, causal, kv_len, _xa_state, None, f8, _as16_2d(x, dt), xa2, *params)
         return y.view(B, T, d)
 
     def _forward_cached(self, x, xa, mask, kv_cache):
@@ -1226,18 +1342,22 @@ class TextDecoder(nn.Module):
         d = self.positional_embedding.shape[1]
         # shared accumulator of the layers' gradients w.r.t. the encoder output (see _BlockFn.backward); one per forward pass
         xa_state = {"buf": None, "left": len(self.blocks)} if (kv_cache is None and torch.is_grad_enabled() and xa.requires_grad) else None
+        # fp8_autocast(): the encoder output feeds every layer's cross K/V projection; quantise it once, here on the main
+        # stream, so that each layer's side-stream GEMM is ordered after it
+        kw = {} if xa_state is None else {"_xa_state": xa_state}
+        if kv_cache is None and fp8_enabled() and dt == torch.bfloat16:
+            kw["_fp8"] = fp8_inputs(xa)
         if packed is not None:
             h = _EmbedFn.apply(x, self.token_embedding.weight, self.positional_embedding, 0, self.token_embedding.padding_idx,
                                self, dt, packed)
             for block in self.blocks:
-                h = block(h, xa, _xa_state=xa_state, _packed=packed)
+                h = block(h, xa, _packed=packed, **kw)
             return _LayerNormFn.apply(h, self.ln.weight, self.ln.bias, self.ln.eps, self, "ln")
         h = _EmbedFn.apply(x, self.token_embedding.weight, self.positional_embedding, offset,
                            self.token_embedding.padding_idx, self, dt).view(B, S, d)
         mask = padding_mask if padding_mask is not None else self.mask[:S, :S]
         for block in self.blocks:
-            h = block(h, xa, mask=mask, kv_cache=kv_cache, _xa_state=xa_state) if xa_state is not None else \
-                block(h, xa, mask=mask, kv_cache=kv_cache)
+            h = block(h, xa, mask=mask, kv_cache=kv_cache, **kw)
         return _LayerNormFn.apply(h.reshape(B * S, d), self.ln.weight, self.ln.bias, self.ln.eps, self, "ln")
 
     def forward(self, x: Tensor, xa: Tensor, kv_cache: Optional[dict] = None, padding_mask: Optional[Tensor] = None,

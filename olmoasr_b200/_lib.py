@@ -139,6 +139,10 @@ _SIGNATURES = {
                             c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_void_p],
     "oasr_cast_scaled16": [c_void_p, c_i64, c_i64, c_float, c_void_p, c_i64, c_int, c_void_p],
     "oasr_lora_merge_f32": [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_i64, c_i64, c_i64, c_void_p],
+    # FP8 training GEMMs: per-row scaled fp8 GEMM, per-row quantiser (rows of x or of x^T)
+    "oasr_gemm_fp8": [c_void_p, c_i64, c_int, c_void_p, c_void_p, c_i64, c_int, c_void_p, c_void_p, c_i64, c_void_p, c_void_p,
+                      c_void_p, c_i64, c_i64, c_i64, c_i64, c_int, c_int, c_void_p],
+    "oasr_quantize_fp8_rows": [c_void_p, c_i64, c_i64, c_i64, c_int, c_int, c_int, c_void_p, c_i64, c_void_p, c_void_p],
     "oasr_layernorm_fwd16": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_float, c_int, c_void_p],
     "oasr_layernorm_bwd16": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                              c_i64, c_i64, c_int, c_void_p],

@@ -51,6 +51,7 @@ static EncodeTiledFn get_encode() {
 }
 
 static CUtensorMapDataType dtype_of(int elt_bytes, bool fp16) {
+  if (elt_bytes == 1) return CU_TENSOR_MAP_DATA_TYPE_UINT8;   // fp8 operands (TMA copies bytes; wgmma reads the format)
   if (elt_bytes == 2) return fp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   return CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
 }

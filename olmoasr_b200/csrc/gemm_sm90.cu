@@ -27,6 +27,14 @@ namespace oasr {
 namespace {
 
 constexpr int BM = 128;
+// FP8 accumulation: the library promotes every k-block (see gemm_body).  An A/B build with -DOASR_FP8_NO_PROMOTE
+// (python -m olmoasr_b200.build --variant ... -DOASR_FP8_NO_PROMOTE) chains all k-blocks in the MMA accumulator instead,
+// which is how far tools/fp8_accumulation_error.py measures the unpromoted sum from fp64; it is not a shipped form.
+#ifdef OASR_FP8_NO_PROMOTE
+constexpr bool FP8_PROMOTE = false;
+#else
+constexpr bool FP8_PROMOTE = true;
+#endif
 constexpr int BK = 64;               // 64 bf16 = 128 B = swizzle span
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
 constexpr int THREADS = 384;
@@ -53,12 +61,14 @@ struct GemmParams {
   int64_t split_stride;   // split-K: split s stores its fp32 partial at C + s * split_stride (0: one split)
   // 16-bit epilogues: C (and C2) / aux move by TMA (16-byte aligned base and row stride), else by plain bounded copies
   int tma_out, tma_aux;
+  const float* sa;   // FP8 kernels: the per-row scales of A (M) and of B (N), applied to acc before the epilogue
+  const float* sb;
 };
 
 constexpr bool is_f32_epi(int epi) { return epi == OASR_EPI_F32 || epi == OASR_EPI_F32_ATOMIC_ADD; }
 constexpr bool reads_aux(int epi) { return epi == OASR_EPI_BF16_RESIDUAL || epi == OASR_EPI_BF16_GELU_BWD; }
 
-template <int BN, int EPI>
+template <int BN, int EPI, bool SCALED = false>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
@@ -66,9 +76,10 @@ struct Cfg {
   // own aux and stored from there); BF16 and GELU cycle two output boxes per consumer warpgroup.  Then BN fp32 of bias.
   static constexpr int EPI_BYTES = is_f32_epi(EPI) ? 0 : (reads_aux(EPI) ? BM * BN * 2 : 2 * 2 * BOX_BYTES);
   static constexpr int BIAS_BYTES = is_f32_epi(EPI) ? 0 : BN * 4;
-  static constexpr int BUDGET = 232448 - 1024 - EPI_BYTES - BIAS_BYTES;   // 227 KB per block, minus the barrier area
+  static constexpr int SCALE_BYTES = SCALED ? BN * 4 : 0;   // FP8: B's row scales of the tile, after the bias
+  static constexpr int BUDGET = 232448 - 1024 - EPI_BYTES - BIAS_BYTES - SCALE_BYTES;   // 227 KB per block, minus the barrier area
   static constexpr int STAGES = (BUDGET / STAGE_BYTES) > 8 ? 8 : (BUDGET / STAGE_BYTES);
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + BIAS_BYTES + 1024;   // 1024-aligned base, barriers last
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + BIAS_BYTES + SCALE_BYTES + 1024;   // 1024-aligned base, barriers last
   static_assert(STAGES >= 3, "gemm: shared-memory ring too shallow");
 };
 
@@ -119,11 +130,18 @@ __device__ __forceinline__ void box_to_global(const uint8_t* box, void* dst, int
 // A2 B2^T: after a tile's k-blocks the operand producer streams kb_tail more k-blocks from tmA2 (A2 (M, K2) K-major) and
 // tmB2 (B2 with B's major) into the same ring, and the consumers accumulate them into the same registers, so every
 // epilogue applies to acc = A B^T + A2 B2^T unchanged.  TMA zero-fills the k columns past K2.
-template <typename T, int BN, int A_MN, int B_MN, int EPI, bool LR>
+// F8 (a compile-time switch; 0 for the 16-bit kernels) makes A and B fp8, both K-major: 1 = e4m3 x e4m3 (forward),
+// 2 = e5m2 x e4m3 (dgrad).  A k-block is then 128 elements, the same 128-byte swizzle row, so the ring, the stage bytes
+// and the 32-byte descriptor k-step are those of the 16-bit kernels.  Hopper's fp8 MMA accumulates with reduced
+// precision, so each k-block's four k32 MMAs go into a temporary accumulator that the consumer adds into the fp32 one
+// with IEEE adds (promotion every 128 k).  Before the epilogue acc = (acc * sa[m]) * sb[n]; the output is T (bf16).
+template <typename T, int BN, int A_MN, int B_MN, int EPI, bool LR, int F8 = 0>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
                                           const CUtensorMap& tmC2, const CUtensorMap& tmAux, const CUtensorMap* tmA2,
                                           const CUtensorMap* tmB2, const GemmParams& p, int kb_tail) {
-  using C = Cfg<BN, EPI>;
+  using C = Cfg<BN, EPI, F8 != 0>;
+  static_assert(F8 == 0 || (!A_MN && !B_MN && !LR && !is_f32_epi(EPI) && BN <= 128), "gemm fp8: K-major, 16-bit epilogues, BN <= 128");
+  constexpr int BKE = F8 ? 2 * BK : BK;   // elements per k-block (128 bytes either way)
   constexpr int STAGES = C::STAGES;
   constexpr int NACC = BN / 2;   // accumulator registers per thread (64 x BN fp32 over 128 threads)
   constexpr bool EPI16 = !is_f32_epi(EPI);
@@ -131,7 +149,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* epi_buf = smem_raw + STAGES * C::STAGE_BYTES;
   float* bias_s = reinterpret_cast<float*>(epi_buf + C::EPI_BYTES);
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(epi_buf + C::EPI_BYTES + C::BIAS_BYTES);
+  float* sb_s = bias_s + BN;   // FP8 only (SCALE_BYTES)
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(epi_buf + C::EPI_BYTES + C::BIAS_BYTES + C::SCALE_BYTES);
   uint64_t* bar_empty = bar_full + STAGES;
   // 16-bit epilogues: the epilogue producer fills bias (and aux) for a tile -> epi_full; both consumer warpgroups are
   // done with them -> epi_empty
@@ -185,7 +204,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
           const bool tail = LR && kb >= kb1;
           const CUtensorMap* ma = tail ? tmA2 : &tmA;
           const CUtensorMap* mb = tail ? tmB2 : &tmB;
-          const int k0 = (tail ? kb - kb1 : kb) * BK;
+          const int k0 = (tail ? kb - kb1 : kb) * BKE;
           if (A_MN) {
 #pragma unroll
             for (int i = 0; i < BM / 64; ++i) ptx::tma_load_2d(sa + i * (BK * 128), ma, full, m_blk * BM + i * 64, k0);
@@ -213,6 +232,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
         ptx::mbar_wait(epi_empty, phase ^ 1);   // both consumer warpgroups are done with the previous tile's
         for (int j = lane; j < BN; j += 32)     // rounded to T like bias.to(x.dtype); 0 past N
           bias_s[j] = (p.bias != nullptr && n0 + j < p.N) ? Act16<T>::round(__ldg(p.bias + n0 + j)) : 0.f;
+        if constexpr (F8 != 0)
+          for (int j = lane; j < BN; j += 32) sb_s[j] = n0 + j < p.N ? __ldg(p.sb + n0 + j) : 0.f;
         if (reads_aux(EPI) && p.tma_aux) {
           if (lane == 0) {   // the boxes that hold rows < M and columns < N; TMA zero-fills past the edges
             const int halves = p.M - m0 > 64 ? 2 : 1;
@@ -262,35 +283,67 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
     decode_tile(tile, p, m_blk, n_blk, split);
     const int kb0 = split * p.kblocks_per_split;
     const int kb1 = min(kb0 + p.kblocks_per_split, p.kblocks_total);
-    int prev = -1;
-    for (int kb = kb0; kb < kb1 + (LR ? kb_tail : 0); ++kb) {
-      ptx::mbar_wait(ptx::smem_u32(&bar_full[stage]), phase);
-      const uint64_t ad = ptx::desc_add(a_desc0, stage * C::STAGE_BYTES);
-      const uint64_t bd = ptx::desc_add(b_desc0, stage * C::STAGE_BYTES);
-      ptx::wgmma_fence();
+    if constexpr (F8 != 0) {
+      // one k-block at a time: its MMAs into tmp, retired, the slot handed back, then tmp promoted into acc
+      float tmp[NACC];
+      for (int kb = kb0; kb < kb1; ++kb) {
+        ptx::mbar_wait(ptx::smem_u32(&bar_full[stage]), phase);
+        const uint64_t ad = ptx::desc_add(a_desc0, stage * C::STAGE_BYTES);
+        const uint64_t bd = ptx::desc_add(b_desc0, stage * C::STAGE_BYTES);
+        ptx::wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < BK / 16; ++k) {
-        const uint32_t accumulate = (kb > kb0 || k > 0) ? 1u : 0u;
-        const uint64_t da = ptx::desc_add(ad, k * a_kstep), db = ptx::desc_add(bd, k * b_kstep);
-        if constexpr (BN == 256) ptx::wgmma_m64n256k16_ss<A_MN, B_MN, T>(acc, da, db, accumulate);
-        else if constexpr (BN == 128) ptx::wgmma_m64n128k16_ss<A_MN, B_MN, T>(acc, da, db, accumulate);
-        else ptx::wgmma_m64n64k16_ss<A_MN, B_MN, T>(acc, da, db, accumulate);
+        for (int k = 0; k < BKE / 32; ++k) {
+          const uint64_t da = ptx::desc_add(ad, k * 32), db = ptx::desc_add(bd, k * 32);
+          float (&d)[NACC] = FP8_PROMOTE ? tmp : acc;
+          const uint32_t accumulate = (k > 0 || (!FP8_PROMOTE && kb > kb0)) ? 1u : 0u;
+          if constexpr (BN == 128) ptx::wgmma_m64n128k32_f8<F8>(d, da, db, accumulate);
+          else ptx::wgmma_m64n64k32_f8<F8>(d, da, db, accumulate);
+        }
+        ptx::wgmma_commit();
+        if (kb == kb0 && tile != static_cast<int>(blockIdx.x) && t == 0) {   // as in the 16-bit loop below
+          if (reads_aux(EPI) && p.tma_out) ptx::bulk_wait_group_read<0>();
+          ptx::mbar_arrive(epi_empty);
+        }
+        ptx::wgmma_wait<0>();
+        ptx::fence_regs(FP8_PROMOTE ? tmp : acc);
+        if (t == 0) ptx::mbar_arrive(ptx::smem_u32(&bar_empty[stage]));
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        if constexpr (FP8_PROMOTE) {
+#pragma unroll
+          for (int i = 0; i < NACC; ++i) acc[i] = kb == kb0 ? tmp[i] : __fadd_rn(acc[i], tmp[i]);
+        }
       }
-      ptx::wgmma_commit();
-      if (EPI16 && kb == kb0 && tile != static_cast<int>(blockIdx.x) && t == 0) {
-        // The previous tile's epilogue is over (its last box barrier came after every read of bias and aux); with the
-        // MMAs of this tile under way, hand its buffers back once the TMA engine has read the stores' sources.
-        if (reads_aux(EPI) && p.tma_out) ptx::bulk_wait_group_read<0>();
-        ptx::mbar_arrive(epi_empty);
+    } else {   // 16-bit: one k-block of MMAs kept in flight behind the next one
+      int prev = -1;
+      for (int kb = kb0; kb < kb1 + (LR ? kb_tail : 0); ++kb) {
+        ptx::mbar_wait(ptx::smem_u32(&bar_full[stage]), phase);
+        const uint64_t ad = ptx::desc_add(a_desc0, stage * C::STAGE_BYTES);
+        const uint64_t bd = ptx::desc_add(b_desc0, stage * C::STAGE_BYTES);
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint32_t accumulate = (kb > kb0 || k > 0) ? 1u : 0u;
+          const uint64_t da = ptx::desc_add(ad, k * a_kstep), db = ptx::desc_add(bd, k * b_kstep);
+          if constexpr (BN == 256) ptx::wgmma_m64n256k16_ss<A_MN, B_MN, T>(acc, da, db, accumulate);
+          else if constexpr (BN == 128) ptx::wgmma_m64n128k16_ss<A_MN, B_MN, T>(acc, da, db, accumulate);
+          else ptx::wgmma_m64n64k16_ss<A_MN, B_MN, T>(acc, da, db, accumulate);
+        }
+        ptx::wgmma_commit();
+        if (EPI16 && kb == kb0 && tile != static_cast<int>(blockIdx.x) && t == 0) {
+          // The previous tile's epilogue is over (its last box barrier came after every read of bias and aux); with the
+          // MMAs of this tile under way, hand its buffers back once the TMA engine has read the stores' sources.
+          if (reads_aux(EPI) && p.tma_out) ptx::bulk_wait_group_read<0>();
+          ptx::mbar_arrive(epi_empty);
+        }
+        ptx::wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot may be refilled
+        if (prev >= 0 && t == 0) ptx::mbar_arrive(ptx::smem_u32(&bar_empty[prev]));
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      ptx::wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot may be refilled
-      if (prev >= 0 && t == 0) ptx::mbar_arrive(ptx::smem_u32(&bar_empty[prev]));
-      prev = stage;
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      ptx::wgmma_wait<0>();
+      ptx::fence_regs(acc);
+      if (t == 0) ptx::mbar_arrive(ptx::smem_u32(&bar_empty[prev]));
     }
-    ptx::wgmma_wait<0>();
-    ptx::fence_regs(acc);
-    if (t == 0) ptx::mbar_arrive(ptx::smem_u32(&bar_empty[prev]));
 
     if constexpr (is_f32_epi(EPI)) {
       // ---- straight from the fragments: row 16*warp + lane/4 (+8), columns 8i + 2*(lane%4) (+1)
@@ -334,6 +387,14 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
       if (row0 < p.M) {
         const uint32_t word = (16 * warp + (lane >> 2)) * 128 + 4 * (lane & 3);
         const uint32_t bias_q = ptx::smem_u32(bias_s) + 8 * (lane & 3);
+        float sa[2] = {0.f, 0.f};   // FP8: A's scales of this thread's rows r and r + 8
+        if constexpr (F8 != 0) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = row0 + 16 * warp + (lane >> 2) + 8 * h;
+            sa[h] = row < p.M ? __ldg(p.sa + row) : 0.f;
+          }
+        }
 #pragma unroll
         for (int b = 0; b < BN / BOX; ++b) {
           const int col0 = n_blk * BN + BOX * b;
@@ -360,11 +421,18 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmA, const CUtensor
             for (int j = 0; j < BOX / 8; ++j) {
               const int i = (BOX / 8) * b + j;
               const float2 bb = ptx::ld_shared_f32x2(bias_q + 32 * i);
+              float2 sbv = make_float2(0.f, 0.f);
+              if constexpr (F8 != 0) sbv = ptx::ld_shared_f32x2(bias_q + BN * 4 + 32 * i);
               const uint32_t wa = box + word + ((j ^ (lane >> 2)) << 4);
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
                 using A = Act16<T>;
-                const uint32_t v = A::pack2(__fadd_rn(acc[4 * i + 2 * h], bb.x), __fadd_rn(acc[4 * i + 2 * h + 1], bb.y));
+                float a0 = acc[4 * i + 2 * h], a1 = acc[4 * i + 2 * h + 1];
+                if constexpr (F8 != 0) {
+                  a0 = __fmul_rn(__fmul_rn(a0, sa[h]), sbv.x);
+                  a1 = __fmul_rn(__fmul_rn(a1, sa[h]), sbv.y);
+                }
+                const uint32_t v = A::pack2(__fadd_rn(a0, bb.x), __fadd_rn(a1, bb.y));
                 uint32_t o = v;
                 if constexpr (EPI == OASR_EPI_BF16_GELU) {   // h = T(acc + b), g = T(gelu(h))
                   if (out) {
@@ -419,6 +487,15 @@ gemm_lowrank_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   gemm_body<T, BN, 0, B_MN, EPI, true>(tmA, tmB, tmC, tmC2, tmAux, &tmA2, &tmB2, p, kb_tail);
 }
 
+// D = epi((sa[m] sb[n]) sum_k A[m,k] B[n,k]), A (M, K) and B (N, K) fp8, K-major, bf16 output
+template <int BN, int F8, int EPI>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2,
+                const __grid_constant__ CUtensorMap tmAux, const GemmParams p) {
+  gemm_body<bf16, BN, 0, 0, EPI, false, F8>(tmA, tmB, tmC, tmC2, tmAux, nullptr, nullptr, p, 0);
+}
+
 // split-K: out[m, n] += sum_s ws[s][m][n], splits in order (fp32 atomics would round differently from run to run)
 __global__ void splitk_reduce_kernel(const float* __restrict__ ws, int splits, int M, int N, float* __restrict__ out, int64_t ldc) {
   const int64_t mn = static_cast<int64_t>(M) * N;
@@ -462,6 +539,42 @@ int launch_lowrank(const Maps& m, const GemmParams& p, int kb_tail, cudaStream_t
   kern<<<grid, THREADS, C::SMEM_BYTES, st>>>(m.a, m.b, m.c, m.c2, m.aux, m.a2, m.b2, p, kb_tail);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
+}
+
+template <int BN, int F8, int EPI>
+int launch_fp8(const Maps& m, const GemmParams& p, cudaStream_t st) {
+  using C = Cfg<BN, EPI, true>;
+  auto kern = gemm_fp8_kernel<BN, F8, EPI>;
+  static bool attr_set = false;  // per instantiation
+  if (!attr_set) {
+    OASR_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    attr_set = true;
+  }
+  const int grid = p.num_tiles < gemm_sm_budget() ? p.num_tiles : gemm_sm_budget();
+  kern<<<grid, THREADS, C::SMEM_BYTES, st>>>(m.a, m.b, m.c, m.c2, m.aux, p);
+  OASR_LAUNCH_CHECK();
+  return OASR_OK;
+}
+
+// The FP8 forms of a block projection: forward (e4m3 x e4m3) BF16, BF16_GELU and BF16_RESIDUAL; dgrad (e5m2 x e4m3)
+// BF16, BF16_RESIDUAL and BF16_GELU_BWD.
+template <int BN>
+int dispatch_fp8(int f8, int epi, const Maps& m, const GemmParams& p, cudaStream_t st) {
+  if (f8 == 1) {
+    switch (epi) {
+      case OASR_EPI_BF16: return launch_fp8<BN, 1, OASR_EPI_BF16>(m, p, st);
+      case OASR_EPI_BF16_GELU: return launch_fp8<BN, 1, OASR_EPI_BF16_GELU>(m, p, st);
+      case OASR_EPI_BF16_RESIDUAL: return launch_fp8<BN, 1, OASR_EPI_BF16_RESIDUAL>(m, p, st);
+    }
+  } else {
+    switch (epi) {
+      case OASR_EPI_BF16: return launch_fp8<BN, 2, OASR_EPI_BF16>(m, p, st);
+      case OASR_EPI_BF16_RESIDUAL: return launch_fp8<BN, 2, OASR_EPI_BF16_RESIDUAL>(m, p, st);
+      case OASR_EPI_BF16_GELU_BWD: return launch_fp8<BN, 2, OASR_EPI_BF16_GELU_BWD>(m, p, st);
+    }
+  }
+  set_last_error("gemm_fp8: no kernel for %s with epilogue %d", f8 == 1 ? "e4m3 x e4m3" : "e5m2 x e4m3", epi);
+  return OASR_ERR_UNSUPPORTED;
 }
 
 // The pairs a Linear with a low-rank adapter needs, for every tile width: forward (B K-major) BF16, BF16_GELU and
@@ -565,6 +678,7 @@ int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, i
   p.raster_m = (N > M) ? 1 : 0;
   p.num_tiles = p.tiles_m * p.tiles_n * p.splits;
   p.split_stride = 0;
+  p.sa = p.sb = nullptr;
 
   Maps m;
   memset(&m, 0, sizeof(m));
@@ -634,10 +748,68 @@ int gemm(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb, i
   return rc;
 }
 
+int gemm_fp8(const void* A, int64_t lda, int a_fmt, const float* a_scale, const void* B, int64_t ldb, int b_fmt,
+             const float* b_scale, void* Cout, int64_t ldc, void* C2, const float* bias, const void* aux, int64_t ldaux,
+             int64_t M, int64_t N, int64_t K, int epilogue, int block_n, void* stream) {
+  OASR_REQUIRE(M > 0 && N > 0 && K > 0, "gemm_fp8: empty problem M=%ld N=%ld K=%ld", (long)M, (long)N, (long)K);
+  OASR_REQUIRE(A && B && Cout && a_scale && b_scale, "gemm_fp8: null operand or scale");
+  OASR_REQUIRE(b_fmt == OASR_FP8_E4M3 && (a_fmt == OASR_FP8_E4M3 || a_fmt == OASR_FP8_E5M2),
+               "gemm_fp8: formats A=%d B=%d; supported are e4m3 x e4m3 and e5m2 x e4m3", a_fmt, b_fmt);
+  // TMA: 16-byte aligned bases and row strides, i.e. multiples of 16 one-byte elements
+  OASR_REQUIRE((K & 15) == 0, "gemm_fp8: K=%ld must be a multiple of 16", (long)K);
+  OASR_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0 && (lda & 15) == 0 &&
+               (ldb & 15) == 0, "gemm_fp8: A/B must be 16-byte aligned with lda/ldb multiples of 16");
+  OASR_REQUIRE(epilogue >= OASR_EPI_BF16 && epilogue <= OASR_EPI_BF16_GELU_BWD, "gemm_fp8: 16-bit epilogues only, got %d",
+               epilogue);
+  if (epilogue == OASR_EPI_BF16_GELU) OASR_REQUIRE(C2 != nullptr, "gemm_fp8: GELU epilogue needs C2");
+  if (reads_aux(epilogue)) OASR_REQUIRE(aux != nullptr, "gemm_fp8: epilogue %d needs aux", epilogue);
+  if (block_n == 0) block_n = N > 64 ? 128 : 64;
+  OASR_REQUIRE(block_n == 64 || block_n == 128, "gemm_fp8: block_n must be 64 or 128");
+
+  GemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.C = Cout; p.C2 = C2; p.bias = bias; p.aux = aux; p.ldc = ldc; p.ldaux = ldaux;
+  p.M = (int)M; p.N = (int)N; p.K = (int)K;
+  p.tiles_m = (int)ceil_div(M, BM);
+  p.tiles_n = (int)ceil_div(N, block_n);
+  p.kblocks_total = p.kblocks_per_split = (int)ceil_div(K, 2 * BK);
+  p.splits = 1;
+  p.raster_m = (N > M) ? 1 : 0;
+  p.num_tiles = p.tiles_m * p.tiles_n;
+  p.sa = a_scale; p.sb = b_scale;
+
+  Maps m;
+  memset(&m, 0, sizeof(m));
+  int rc;
+  if ((rc = make_tmap_2d(&m.a, A, 1, (uint64_t)K, (uint64_t)M, (uint64_t)lda, 2 * BK, BM, true))) return rc;
+  if ((rc = make_tmap_2d(&m.b, B, 1, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, 2 * BK, block_n, true))) return rc;
+  p.tma_out = tma_addressable(Cout, ldc) && (epilogue != OASR_EPI_BF16_GELU || tma_addressable(C2, ldc));
+  p.tma_aux = reads_aux(epilogue) && tma_addressable(aux, ldaux);
+  if (p.tma_out) {
+    if ((rc = make_tmap_2d(&m.c, Cout, 2, (uint64_t)N, (uint64_t)M, (uint64_t)ldc * 2, BOX, BOX, true))) return rc;
+    if (epilogue == OASR_EPI_BF16_GELU &&
+        (rc = make_tmap_2d(&m.c2, C2, 2, (uint64_t)N, (uint64_t)M, (uint64_t)ldc * 2, BOX, BOX, true)))
+      return rc;
+  }
+  if (p.tma_aux && (rc = make_tmap_2d(&m.aux, aux, 2, (uint64_t)N, (uint64_t)M, (uint64_t)ldaux * 2, BOX, BOX, true)))
+    return rc;
+  const int f8 = a_fmt == OASR_FP8_E4M3 ? 1 : 2;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return block_n == 128 ? dispatch_fp8<128>(f8, epilogue, m, p, st) : dispatch_fp8<64>(f8, epilogue, m, p, st);
+}
+
 }  // namespace
 }  // namespace oasr
 
 using namespace oasr;
+
+extern "C" int oasr_gemm_fp8(const void* A, int64_t lda, int a_fmt, const float* a_scale, const void* B, int64_t ldb,
+                             int b_fmt, const float* b_scale, void* Cout, int64_t ldc, void* C2, const float* bias,
+                             const void* aux, int64_t ldaux, int64_t M, int64_t N, int64_t K, int epilogue, int block_n,
+                             void* stream) {
+  return gemm_fp8(A, lda, a_fmt, a_scale, B, ldb, b_fmt, b_scale, Cout, ldc, C2, bias, aux, ldaux, M, N, K, epilogue,
+                  block_n, stream);
+}
 
 extern "C" int oasr_gemm_bf16(const void* A, int64_t lda, int a_layout, const void* B, int64_t ldb,
                               int b_layout, void* Cout, int64_t ldc, void* C2, const float* bias,

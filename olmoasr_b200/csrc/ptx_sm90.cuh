@@ -196,6 +196,29 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_
     OASR_WGMMA_RS64("bf16");
 }
 #undef OASR_WGMMA_RS64
+// FP8: D (+)= A * B over k = 32, both operands K-major from shared memory (wgmma has no transpose for 8-bit types).
+// F8 = 1: e4m3 x e4m3, F8 = 2: e5m2 (A) x e4m3 (B).  A 32-deep k-step is 32 bytes, like a 16-deep 16-bit one.
+#define OASR_WGMMA_F8(N, TA, TB, REGS, DOUT, P, A, B)                                                        \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" P ", 0;\n\t"                                    \
+               "wgmma.mma_async.sync.aligned.m64n" #N "k32.f32." TA "." TB " " REGS ", %" A ", %" B ", p, 1, 1;\n\t}" \
+               : DOUT : "l"(da), "l"(db), "r"(acc))
+template <int F8>
+__device__ __forceinline__ void wgmma_m64n64k32_f8(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
+  static_assert(F8 == 1 || F8 == 2, "wgmma fp8: F8 is 1 (e4m3.e4m3) or 2 (e5m2.e4m3)");
+  if constexpr (F8 == 1)
+    OASR_WGMMA_F8(64, "e4m3", "e4m3", OASR_R32, OASR_D32, "34", "32", "33");
+  else
+    OASR_WGMMA_F8(64, "e5m2", "e4m3", OASR_R32, OASR_D32, "34", "32", "33");
+}
+template <int F8>
+__device__ __forceinline__ void wgmma_m64n128k32_f8(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+  static_assert(F8 == 1 || F8 == 2, "wgmma fp8: F8 is 1 (e4m3.e4m3) or 2 (e5m2.e4m3)");
+  if constexpr (F8 == 1)
+    OASR_WGMMA_F8(128, "e4m3", "e4m3", OASR_R64, OASR_D64, "66", "64", "65");
+  else
+    OASR_WGMMA_F8(128, "e5m2", "e4m3", OASR_R64, OASR_D64, "66", "64", "65");
+}
+#undef OASR_WGMMA_F8
 #undef OASR_WGMMA_SS
 #undef OASR_R32
 #undef OASR_R64

@@ -114,6 +114,63 @@ def gemm_lowrank(a, b, a2, b2, M, N, K, K2, *, b_mn=False, out=None, out2=None, 
     return out
 
 
+FP8_E4M3, FP8_E5M2 = 0, 1
+FP8_DTYPE = {FP8_E4M3: torch.float8_e4m3fn, FP8_E5M2: torch.float8_e5m2}
+_FP8_FMT = {v: k for k, v in FP8_DTYPE.items()}
+
+
+def quantize_fp8_rows(x, fmt, *, transpose=False):
+    """(q, scale): per-row dynamic fp8 quantisation of a 2-D 16-bit x with unit inner stride (include/oasr_b200.h):
+    q (rows, cols) in FP8_DTYPE[fmt] and scale (rows,) f32 with x ~ q * scale[:, None].  With `transpose` the rows of
+    x^T: q (cols, rows), scale (cols,)."""
+    _req(x.dtype in ACT16 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1, "quantize_fp8_rows: 2-D 16-bit CUDA x")
+    _req(fmt in FP8_DTYPE, f"quantize_fp8_rows: bad format {fmt}")
+    R, C = x.shape
+    if transpose:
+        R, C = C, R
+    q = torch.empty((R, C), device=x.device, dtype=FP8_DTYPE[fmt])
+    scale = torch.empty(R, device=x.device, dtype=torch.float32)
+    call("oasr_quantize_fp8_rows", ptr(x), x.stride(0), x.shape[0], x.shape[1], _DTYPE_CODE[x.dtype], fmt, int(transpose),
+         ptr(q), q.stride(0), ptr(scale), stream())
+    return q, scale
+
+
+def gemm_fp8(a, a_scale, b, b_scale, M, N, K, *, out=None, out2=None, bias=None, aux=None, epi=EPI_BF16, block_n=0):
+    """D[M,N] = epi((a_scale[m] b_scale[n]) sum_k A[m,k] B[n,k]) with bf16 output: a (M, K) e4m3 or e5m2, b (N, K)
+    e4m3, both K-major (K a multiple of 16); the 16-bit epilogues of `gemm` (e4m3 A: BF16, GELU, RESIDUAL; e5m2 A:
+    BF16, RESIDUAL, GELU_BWD)."""
+    _req(a.dtype in _FP8_FMT and b.dtype == torch.float8_e4m3fn, f"gemm_fp8: operands {a.dtype} x {b.dtype}")
+    _req(a.is_cuda and b.is_cuda and a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1,
+         "gemm_fp8: 2-D CUDA operands, unit inner stride")
+    _req(tuple(a.shape) == (M, K) and tuple(b.shape) == (N, K), f"gemm_fp8: A {tuple(a.shape)} B {tuple(b.shape)} vs {M, N, K}")
+    _req(a_scale.dtype == torch.float32 and a_scale.numel() >= M and b_scale.dtype == torch.float32 and b_scale.numel() >= N,
+         "gemm_fp8: f32 scales of M and N entries")
+    if out is None:
+        out = torch.empty((M, N), device=a.device, dtype=torch.bfloat16)
+    _req(out.dtype == torch.bfloat16 and out.dim() == 2 and out.shape[0] == M and out.shape[1] >= N and out.stride(1) == 1,
+         "gemm_fp8: out")
+    if epi == EPI_BF16_GELU and out2 is None:
+        out2 = torch.empty_like(out)
+    if aux is not None:
+        _req(aux.dtype == torch.bfloat16 and aux.stride(1) == 1 and aux.shape[0] == M, "gemm_fp8: aux")
+    if bias is not None:
+        _req(bias.dtype == torch.float32 and bias.numel() >= N and bias.is_contiguous(), "gemm_fp8: bias must be f32")
+    prof = GEMM_PROFILE
+    if prof is not None:
+        e0 = torch.cuda.Event(enable_timing=True)
+        e1 = torch.cuda.Event(enable_timing=True)
+        e0.record()
+    call("oasr_gemm_fp8", ptr(a), a.stride(0), _FP8_FMT[a.dtype], ptr(a_scale), ptr(b), b.stride(0), FP8_E4M3, ptr(b_scale),
+         ptr(out), out.stride(0), ptr(out2), ptr(bias), ptr(aux), aux.stride(0) if aux is not None else 0, M, N, K, epi,
+         block_n, stream())
+    if prof is not None:      # keyed like `gemm`'s launches, with the A format in place of the operand majors
+        e1.record()
+        prof.append((2.0 * M * N * K, e0, e1, (M, N, K, "fp8", _FP8_FMT[a.dtype], epi, 1, block_n)))
+    if epi == EPI_BF16_GELU:
+        return out, out2
+    return out
+
+
 def cast_scaled16(src, scale, dst):
     """dst = dst.dtype(scale * src) for an fp32 (rows, cols) src; dst a 2-D 16-bit view with unit inner stride."""
     _req(src.dtype == torch.float32 and src.is_contiguous() and src.dim() == 2, "cast_scaled16: contiguous 2-D f32 src")
