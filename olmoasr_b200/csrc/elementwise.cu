@@ -334,6 +334,9 @@ colsum_kernel(const T* __restrict__ dy, float* __restrict__ part, int64_t M, int
 
 using namespace oasr;
 
+// The vectorised kernels below read and write whole 8- or 16-byte words: a view that starts inside one is refused.
+static inline bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 static inline int grid_1d(int64_t n_items, int threads, int cap_mult = 32) {
   int64_t b = ceil_div(n_items, threads);
   const int64_t cap = static_cast<int64_t>(num_sms()) * cap_mult;
@@ -375,6 +378,7 @@ template <typename T>
 static int embed_fwd(const int64_t* ids, const float* emb, const float* pos, void* out, int64_t batch, int64_t S, int64_t d,
               int64_t pos_offset, int64_t n_rows_emb, void* stream) {
   OASR_REQUIRE(batch > 0 && S > 0 && (d & 3) == 0, "embed_fwd: bad shape");
+  OASR_REQUIRE(aligned(emb, 16) && aligned(pos, 16) && aligned(out, 8), "embed_fwd: emb / pos 16-byte, out 8-byte alignment required");
   embed_fwd_kernel<T><<<(unsigned)(batch * S), 128, 0, (cudaStream_t)stream>>>(ids, emb, pos, (T*)out, batch * S, (int)S, (int)d,
                                                                            (int)pos_offset, n_rows_emb);
   OASR_LAUNCH_CHECK();
@@ -395,6 +399,7 @@ template <typename T>
 static int embed_fwd_packed(const int64_t* ids, const float* emb, const float* pos, void* out, const int32_t* src_rows,
                             int64_t N, int64_t S, int64_t d, int64_t n_rows_emb, void* stream) {
   OASR_REQUIRE(src_rows && N > 0 && S > 0 && (d & 3) == 0, "embed_fwd_packed: bad shape");
+  OASR_REQUIRE(aligned(emb, 16) && aligned(pos, 16) && aligned(out, 8), "embed_fwd_packed: emb / pos 16-byte, out 8-byte alignment required");
   embed_fwd_kernel<T><<<(unsigned)N, 128, 0, (cudaStream_t)stream>>>(ids, emb, pos, (T*)out, N, (int)S, (int)d, 0, n_rows_emb,
                                                                     src_rows);
   OASR_LAUNCH_CHECK();
@@ -424,6 +429,7 @@ static int im2col_conv1(const float* mel, void* A, int64_t batch, int64_t C, int
 
 extern "C" int oasr_im2col_conv2(const void* h, void* A, int64_t batch, int64_t T_in, int64_t T_out, int64_t d, void* stream) {
   OASR_REQUIRE((d & 7) == 0, "im2col_conv2: d must be a multiple of 8");
+  OASR_REQUIRE(aligned(h, 16) && aligned(A, 16), "im2col_conv2: 16-byte alignment required");
   im2col_conv2_kernel<<<(unsigned)(batch * T_out), 128, 0, (cudaStream_t)stream>>>((const uint16_t*)h, (uint16_t*)A, (int)T_in, (int)T_out, (int)d);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
@@ -441,6 +447,7 @@ static int col2im_conv2_gelu_bwd(const void* dA, const void* pre1, void* dpre1, 
 template <typename E>
 static int add_pos(const void* x, const float* pos, void* out, int64_t rows, int64_t T, int64_t d, void* stream) {
   OASR_REQUIRE((d & 7) == 0, "add_pos: d must be a multiple of 8");
+  OASR_REQUIRE(aligned(x, 16) && aligned(pos, 16) && aligned(out, 16), "add_pos: 16-byte alignment required");
   add_pos_kernel<E><<<grid_1d(rows * (d >> 3), 256), 256, 0, (cudaStream_t)stream>>>((const E*)x, pos, (E*)out, rows, (int)T, (int)d);
   OASR_LAUNCH_CHECK();
   return OASR_OK;
@@ -449,6 +456,7 @@ static int add_pos(const void* x, const float* pos, void* out, int64_t rows, int
 template <typename T>
 static int gelu_bwd(const void* dy, const void* pre, void* out, int64_t n, void* stream) {
   OASR_REQUIRE((n & 7) == 0, "gelu_bwd: n must be a multiple of 8");
+  OASR_REQUIRE(aligned(dy, 16) && aligned(pre, 16) && aligned(out, 16), "gelu_bwd: 16-byte alignment required");
   gelu_bwd_kernel<T><<<grid_1d(n >> 3, 256), 256, 0, (cudaStream_t)stream>>>((const T*)dy, (const T*)pre, (T*)out, n);
   OASR_LAUNCH_CHECK();
   return OASR_OK;

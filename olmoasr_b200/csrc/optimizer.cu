@@ -82,7 +82,7 @@ __device__ __forceinline__ void prepare_step(float nsq, bool skip, float* __rest
   if (skip || !isfinite(nsq)) {
     *found_inf = 1.f;
     st[4] = 1.f;
-    st[5] = nsq;
+    st[5] = sqrtf(nsq);   // the norm, as on an applied step (inf / NaN stay inf / NaN)
     return;
   }
   const float total_norm = sqrtf(nsq);

@@ -34,6 +34,12 @@ def _req(cond, msg):
         raise ValueError(msg)
 
 
+def _aligned(*ts, bytes=16):
+    """Every tensor starts on a `bytes` boundary: the vectorised kernels access whole 8- or 16-byte words, so a view
+    that starts inside one (an element offset) is refused here rather than faulting on the device."""
+    return all(t.data_ptr() % bytes == 0 for t in ts)
+
+
 ACT16 = (torch.bfloat16, torch.float16)
 _TWIN16 = {"oasr_gemm_bf16": "oasr_gemm16", "oasr_colsum_bf16": "oasr_colsum16", "oasr_logits_to_f32": "oasr_logits_to_f32_16",
            "oasr_im2col_conv1": "oasr_im2col_conv1_16"}
@@ -358,6 +364,7 @@ def embed_fwd(ids, emb, pos, pos_offset=0, dtype=torch.bfloat16):
     _req(ids.dtype == torch.int64 and ids.dim() == 2 and ids.is_contiguous(), "embed: ids int64 (B,S)")
     B, S = ids.shape
     d = emb.shape[1]
+    _req(_aligned(emb, pos), "embed: emb and pos must be 16-byte aligned")
     out = torch.empty((B * S, d), device=emb.device, dtype=dtype)
     _call16("oasr_embed_fwd", dtype, ptr(ids), ptr(emb), ptr(pos), ptr(out), B, S, d, pos_offset, emb.shape[0], stream())
     return out
@@ -375,6 +382,7 @@ def embed_fwd_packed(ids, emb, pos, pk, dtype=torch.bfloat16):
     _req(ids.dtype == torch.int64 and ids.dim() == 2 and ids.is_contiguous(), "embed: ids int64 (B,S)")
     _req(tuple(ids.shape) == (pk.B, pk.S), "embed_packed: ids shape must match the packed batch")
     d = emb.shape[1]
+    _req(_aligned(emb, pos), "embed_packed: emb and pos must be 16-byte aligned")
     out = torch.empty((pk.N, d), device=emb.device, dtype=dtype)
     call("oasr_embed_fwd_packed16", ptr(ids), ptr(emb), ptr(pos), ptr(out), ptr(pk.rows), pk.N, pk.S, d, emb.shape[0],
          _DTYPE_CODE[dtype], stream())
@@ -432,6 +440,7 @@ def im2col_conv1(mel, kpad, dtype=torch.bfloat16):
 
 def im2col_conv2(h, B, T_in, d):
     T_out = (T_in + 2 - 3) // 2 + 1
+    _req(h.is_contiguous() and _aligned(h), "im2col_conv2: h must be contiguous and 16-byte aligned")
     A = torch.empty((B * T_out, 3 * d), device=h.device, dtype=h.dtype)   # a copy: one kernel serves both 16-bit types
     call("oasr_im2col_conv2", ptr(h), ptr(A), B, T_in, T_out, d, stream())
     return A
@@ -444,12 +453,14 @@ def col2im_conv2_gelu_bwd(dA, pre1, B, T_in, T_out, d):
 
 
 def add_pos(x, pos, T):
+    _req(x.is_contiguous() and pos.is_contiguous() and _aligned(x, pos), "add_pos: x and pos must be contiguous and 16-byte aligned")
     out = torch.empty_like(x)
     _call16("oasr_add_pos", x.dtype, ptr(x), ptr(pos), ptr(out), x.shape[0], T, x.shape[1], stream())
     return out
 
 
 def gelu_bwd(dy, pre):
+    _req(dy.is_contiguous() and pre.is_contiguous() and _aligned(dy, pre), "gelu_bwd: dy and pre must be contiguous and 16-byte aligned")
     out = torch.empty_like(dy)
     _call16("oasr_gelu_bwd", dy.dtype, ptr(dy), ptr(pre), ptr(out), dy.numel(), stream())
     return out

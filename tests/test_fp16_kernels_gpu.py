@@ -160,50 +160,3 @@ def test_cross_entropy_and_logits(K):
     ref.backward()
     K.ce_bwd_(buf, t, lse, lsc, torch.full((1,), 1024.0, device="cuda"), V, 51864)   # a loss scale rides on grad_out
     assert buf.dtype == H16 and _rel(buf[:, :V], _h(1024.0 * logits.grad)) < 2 * EPS
-
-
-def test_embedding_fwd_bwd(K):
-    torch.manual_seed(6)
-    B, S, d, n = 2, 40, 384, 1000
-    ids = torch.randint(0, n, (B, S), device="cuda")
-    ids[0, :5] = 7
-    emb, pos = torch.randn(n, d, device="cuda"), torch.randn(448, d, device="cuda")
-    out = K.embed_fwd(ids, emb, pos, 3, dtype=H16)
-    assert out.dtype == H16 and torch.equal(out.view(B, S, d), (emb[ids] + pos[3:3 + S]).to(H16))
-    dx = torch.randn(B * S, d, device="cuda").to(H16)
-    demb, dpos = torch.zeros(n, d, device="cuda"), torch.zeros(448, d, device="cuda")
-    K.embed_bwd(ids, dx, demb, dpos[3:], -1)
-    ref_e = torch.zeros(n, d, device="cuda").index_add_(0, ids.view(-1), dx.float())
-    assert _rel(demb, ref_e) < 1e-6 and _rel(dpos[3:3 + S], dx.float().view(B, S, d).sum(0)) < 1e-6
-
-
-def test_stem_kernels(K):
-    torch.manual_seed(7)
-    B, C, T, d = 2, 80, 3000, 384
-    mel = torch.randn(B, C, T, device="cuda")
-    A1 = K.im2col_conv1(mel, 3 * C, dtype=H16)
-    ref = F.pad(mel, (1, 1)).unfold(2, 3, 1).permute(0, 2, 3, 1).reshape(B * T, 3 * C)
-    assert A1.dtype == H16 and torch.equal(A1, ref.to(H16))
-    w = torch.randn(d, C, 3, device="cuda")
-    assert torch.equal(K.cast_conv_weight(w, dtype=H16), w.permute(0, 2, 1).reshape(d, 3 * C).to(H16))
-    h = torch.randn(B * T, d, device="cuda").to(H16)
-    T2 = T // 2
-    A2 = K.im2col_conv2(h, B, T, d)
-    assert A2.dtype == H16 and torch.equal(A2.view(B, T2, 3, d)[:, :, 1], h.view(B, T, d)[:, 0::2])
-    pos = torch.randn(T2, d, device="cuda")
-    x = torch.randn(B * T2, d, device="cuda").to(H16)
-    assert torch.equal(K.add_pos(x, pos, T2), (x.float().view(B, T2, d) + pos).to(H16).view(B * T2, d))
-    pre = torch.randn(B * T2, d, device="cuda").to(H16)
-    gp = lambda p: 0.5 * (1 + torch.erf(p / math.sqrt(2))) + p * torch.exp(-0.5 * p * p) / math.sqrt(2 * math.pi)
-    assert _rel(K.gelu_bwd(x, pre), _h(x.float() * gp(pre.float()))) < 2 * EPS
-    dA = torch.randn(B * T2, 3 * d, device="cuda").to(H16)
-    pre1 = torch.randn(B * T, d, device="cuda").to(H16)
-    g = torch.zeros(B, T + 2, d, device="cuda")
-    dAv = dA.float().view(B, T2, 3, d)
-    for kk in range(3):
-        g[:, kk:kk + 2 * T2:2] += dAv[:, :, kk]
-    ref = _h(_h(g[:, 1:T + 1]).reshape(B * T, d) * gp(pre1.float()))
-    assert _rel(K.col2im_conv2_gelu_bwd(dA, pre1, B, T, T2, d), ref) < 2 * EPS
-    db = torch.zeros(d, device="cuda")
-    K.colsum_(x, db)
-    assert _rel(db, x.float().sum(0)) < 1e-5

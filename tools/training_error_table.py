@@ -23,12 +23,13 @@ from tests import decode_reference as dr          # noqa: E402
 from tests import training_reference as tr        # noqa: E402
 
 
-def main():
+def main(test_file="tests/test_training_parity_gpu.py"):
+    """Run `test_file` with the report on and print its table (tools/step_error_table.py passes its own file)."""
     with tempfile.TemporaryDirectory() as tmp:
         report = os.path.join(tmp, "report.jsonl")
         env = dict(os.environ, OASR_ATTN_REPORT=report)
         cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider",
-               "tests/test_training_parity_gpu.py", *sys.argv[1:]]
+               test_file, *sys.argv[1:]]
         rc = subprocess.call(cmd, cwd=ROOT, env=env)
         lines = Path(report).read_text().splitlines() if os.path.exists(report) else []
     table = collections.defaultdict(lambda: collections.defaultdict(float))
@@ -49,6 +50,8 @@ def main():
         elif kind == "lse":
             row["lse"] = max(row["lse"], rec["lse_tol_units"])
             row["loss"] = max(row["loss"], rec["loss_units"])
+        elif kind == "scalar":
+            row["scalar"] = max(row["scalar"], rec["worst"])
         elif kind == "step":
             row["rows max"] = max(row["rows max"], rec["worst_ratio"])
             row["rows mean"] = max(row["rows mean"], rec["mean_ratio"])
