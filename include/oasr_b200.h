@@ -232,6 +232,26 @@ OASR_API int oasr_dec_attention(const oasr_dec_attn_args* args, void* stream);
  * oasr_dec_attention is the kv_group = 1 case: the same launches and the same bits. */
 OASR_API int oasr_dec_attention_grouped(const oasr_dec_attn_args* args, int kv_group, void* stream);
 
+/* FP8 decoding (`DecodingOptions(fp8=True)`): the block projection weights and the cross-attention K / V are stored as
+ * e4m3 codes Q with fp32 scales s, quantised by oasr_quantize_fp8_rows (s = amax / 448, q = e4m3(x * 448 / amax)).
+ * Activations stay in T (fp16 or bf16); every other rounding point is the one stated above.  Sums are fp32.
+ *
+ * oasr_dec_linear_fp8w: as oasr_dec_linear, with W (N, K) e4m3 codes (one byte each, 16-byte aligned base) and w_scale
+ *   (N,) fp32, one scale per output row.  With x~ the staged input (plain, LayerNorm or partial sum, rounded to T):
+ *     y[m, n] = epi( round_T( s_n * sum_k x~[m, k] Q[n, k] + round_T(b_n) ) )
+ *   and the GELU, residual, QKV-scatter and store epilogues unchanged.
+ *
+ * oasr_dec_attention_fp8kv: as oasr_dec_attention_grouped, with k / v e4m3 codes (strides in elements = bytes) and one
+ *   scale per (key, head): element (n, j, h) of k_scale / v_scale at (n / kv_group) * scale_seq_stride
+ *   + j * scale_row_stride + h.  With q~_c = round_T(q_c hd^-1/4):
+ *     score_j = round_T( sK_j hd^-1/4 * sum_c q~_c QK_jc ),  p_j = round_T(softmax_j(score)),
+ *     partial_c = sum_j (p_j sV_j) QV_jc  (fp32; summed over the splits in order and rounded once by the consumer).
+ *   The engine's cross K / V buffer (L, N * 1500, 2d) has scales (L, N * 1500, 2H): one per (key, head, K|V) group of
+ *   64 elements, i.e. oasr_quantize_fp8_rows of the projection viewed as rows of 64. */
+OASR_API int oasr_dec_linear_fp8w(const oasr_dec_linear_args* args, const float* w_scale, void* stream);
+OASR_API int oasr_dec_attention_fp8kv(const oasr_dec_attn_args* args, const float* k_scale, const float* v_scale,
+                                      int64_t scale_seq_stride, int64_t scale_row_stride, int kv_group, void* stream);
+
 /* Logit filters + greedy choice + bookkeeping (whisper/decoding.py SuppressBlank, SuppressTokens, GreedyDecoder.update,
  * the no-speech probability and the stop test of DecodingTask._main_loop), then *pos += 1.
  * tokens: (n_seq, ld_tokens) int32, position *pos holds the token just fed; the choice is written to *pos + 1 once

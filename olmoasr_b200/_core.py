@@ -1607,14 +1607,15 @@ class OLMoASRBase(nn.Module):
                     hooks.append(att.value.register_forward_hook(store.on_projection))
         return store.cache, hooks
 
-    def decode_engine(self, dtype: torch.dtype = torch.float16, max_batch: int = 64):
-        """The device-resident greedy decoder for this model (one per activation dtype, built on first use)."""
+    def decode_engine(self, dtype: torch.dtype = torch.float16, max_batch: int = 64, *, fp8: bool = False):
+        """The device-resident greedy decoder for this model (one per activation dtype, batch and weight storage, built on
+        first use); `fp8=True` is the engine with e4m3 block weights and cross K / V (DecodingOptions.fp8)."""
         from .decode_engine import DecodeEngine
 
         engines = self.__dict__.setdefault("_engines", {})
-        key = (dtype, max_batch)
+        key = (dtype, max_batch, bool(fp8))
         if key not in engines:
-            engines[key] = DecodeEngine(self, dtype, max_batch)
+            engines[key] = DecodeEngine(self, dtype, max_batch, fp8=bool(fp8))
         return engines[key]
 
 

@@ -124,6 +124,9 @@ _SIGNATURES = {
     "oasr_dec_sample": [ctypes.POINTER(DecSampleArgs), c_void_p],
     "oasr_dec_sample_rules": [ctypes.POINTER(DecSampleRulesArgs), c_void_p],
     "oasr_dec_attention_grouped": [ctypes.POINTER(DecAttnArgs), c_int, c_void_p],
+    # fp8 decoding: e4m3 weights + (N,) scales; e4m3 K / V + per-(key, head) scales (k, v, seq stride, row stride)
+    "oasr_dec_linear_fp8w": [ctypes.POINTER(DecLinearArgs), c_void_p, c_void_p],
+    "oasr_dec_attention_fp8kv": [ctypes.POINTER(DecAttnArgs), c_void_p, c_void_p, c_i64, c_i64, c_int, c_void_p],
     "oasr_dec_beam_candidates": [ctypes.POINTER(DecBeamArgs), c_void_p],
     "oasr_dec_beam_select": [ctypes.POINTER(DecBeamArgs), c_void_p],
     "oasr_dec_beam_reorder": [c_void_p, c_void_p, c_i64, c_i64, c_i64, c_void_p, c_void_p, c_i32, c_i32, c_i32, c_i32, c_int,
@@ -242,7 +245,7 @@ def stream():
 
 # kernels launched per entry point (memsets not counted) -- bench.py reports the total as `gpu_launches`
 _LAUNCHES_PER_CALL = {"oasr_logmel": 3, "oasr_attention_bwd": 3, "oasr_dec_attention": 2, "oasr_dec_sample": 2,
-                      "oasr_dec_sample_rules": 2, "oasr_dec_attention_grouped": 2, "oasr_dec_beam_select": 2,
+                      "oasr_dec_sample_rules": 2, "oasr_dec_attention_grouped": 2, "oasr_dec_attention_fp8kv": 2, "oasr_dec_beam_select": 2,
                       "oasr_ce_fwd": 2, "oasr_colsum_bf16": 2, "oasr_layernorm_bwd": 3, "oasr_grad_sqnorm": 2,
                       "oasr_grad_sqnorm_flat": 2, "oasr_attention_bwd16": 3, "oasr_ce_fwd16": 2, "oasr_colsum16": 2,
                       "oasr_layernorm_bwd16": 3, "oasr_attention_bwd_varlen16": 3, "oasr_align_cost": 2, "oasr_align_cost_batched": 2}

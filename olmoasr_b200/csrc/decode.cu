@@ -15,7 +15,10 @@
 //     scatter of new K/V rows into the pre-allocated cache are all fused into it -- 6 of the 10 launches per layer;
 //   * dec_attn_scores / dec_attn_pv: single-query attention that reads every cached K and V element once (16-byte
 //     loads, 8 lanes per key row), key ranges split over CTAs when batch x heads cannot fill the SMs;
-//   * dec_sample: logit filters + argmax + log-prob + eot bookkeeping in one pass over the fp32 logits.
+//   * dec_sample: logit filters + argmax + log-prob + eot bookkeeping in one pass over the fp32 logits;
+//   * fp8 decoding (oasr_dec_linear_fp8w / oasr_dec_attention_fp8kv): the same kernels instantiated on e4m3 weight or
+//     cross K / V storage, half the bytes of the two streams that dominate the step; codes become T in registers and
+//     the fp32 scales multiply outside the dot products (include/oasr_b200.h states the arithmetic).
 //
 // Rounding points are the reference's in the activation dtype T (inf_model.py:172-196): q*hd^-0.25 and k*hd^-0.25 rounded
 // to T, q.k accumulated in fp32 and rounded to T, softmax in fp32, probabilities rounded to T, p.v accumulated in fp32 and
@@ -62,6 +65,56 @@ template <> struct DT<bf16> {
   }
 };
 template <typename T> __device__ __forceinline__ float rnd(float v) { return DT<T>::to_f(DT<T>::from_f(v)); }
+
+// ---------------------------------------------------------------------------------------------------------- stored operands
+// Weights and cross K / V are stored either in the activation type T or as e4m3 codes (uint8_t) with fp32 scales applied
+// outside the dot product (`fp8=True`, include/oasr_b200.h).  Either way a thread reads 8 consecutive elements at a time
+// -- 16 bytes of T or 8 bytes of codes, so 8 lanes on one row still cover whole 32-byte sectors -- and hands them on as
+// 8 T values in the uint4 layout of an MMA fragment.  Every e4m3 value is exact in fp16 and in bf16.
+__device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t lo16) {
+  uint32_t r;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"(static_cast<uint16_t>(lo16)));
+  return r;
+}
+template <typename T> __device__ __forceinline__ uint32_t e4m3x2_to(uint32_t lo16);
+template <> __device__ __forceinline__ uint32_t e4m3x2_to<__half>(uint32_t lo16) { return e4m3x2_to_f16x2(lo16); }
+template <> __device__ __forceinline__ uint32_t e4m3x2_to<bf16>(uint32_t lo16) {
+  const uint32_t h = e4m3x2_to_f16x2(lo16);
+  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
+  return pack_bf16x2(f.x, f.y);
+}
+
+template <typename T, typename TS> struct Stored;
+// Argument block of the skinny-GEMM kernels: 16-bit weights take the public one as it is (so those instantiations keep
+// the parameter list, and the code, they had before fp8 existed); e4m3 weights add the (N,) fp32 per-row scales.
+struct LinearArgsFp8 : oasr_dec_linear_args {
+  const float* w_scale;
+};
+
+template <typename T> struct Stored<T, T> {       // 16-bit storage: the loaded bytes are the fragment
+  using V = uint4;
+  using LinearArgs = oasr_dec_linear_args;
+  static constexpr bool kFp8 = false;
+  static __device__ __forceinline__ V zero() { return make_uint4(0, 0, 0, 0); }
+  static __device__ __forceinline__ V ldg(const T* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
+  static __device__ __forceinline__ uint4 frag(V v) { return v; }
+};
+template <typename T> struct Stored<T, uint8_t> {  // e4m3 codes, converted in registers
+  using V = uint2;
+  using LinearArgs = LinearArgsFp8;
+  static constexpr bool kFp8 = true;
+  static __device__ __forceinline__ V zero() { return make_uint2(0, 0); }
+  static __device__ __forceinline__ V ldg(const uint8_t* p) { return __ldg(reinterpret_cast<const uint2*>(p)); }
+  static __device__ __forceinline__ uint4 frag(V v) {
+    return make_uint4(e4m3x2_to<T>(v.x & 0xffffu), e4m3x2_to<T>(v.x >> 16), e4m3x2_to<T>(v.y & 0xffffu), e4m3x2_to<T>(v.y >> 16));
+  }
+};
+
+// Per-(key, head) scales of e4m3 cross K / V: element (n, j, h) at k / v + n * seq + j * row + h.  Unused (null) when
+// K / V are stored in T.
+struct KvScales {
+  const float* k; const float* v; int64_t seq; int64_t row;
+};
 
 __device__ __forceinline__ float gelu_exact(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
@@ -126,8 +179,10 @@ __device__ __forceinline__ uint4 load_x8(const oasr_dec_linear_args& a, const fl
 // 64 B: whole sectors) and the SAME 8 k positions of x rows g, g + 8 of every 16-row tile: the two m16n8k16 MMAs per
 // 32-wide k step then use a permuted k order that A and B agree on, so no shuffles and no shared-memory staging are
 // needed; x (<= 64 x K, L2 / L1 resident) is re-read by every CTA, W (the HBM stream) exactly once.
-template <typename T, int MT>
-__global__ void __launch_bounds__(256) dec_linear_direct_kernel(const oasr_dec_linear_args a) {
+// TW: the weight storage (see Stored)
+template <typename T, typename TW, int MT>
+__global__ void __launch_bounds__(256) dec_linear_direct_kernel(const typename Stored<T, TW>::LinearArgs a) {
+  using WS = Stored<T, TW>;
   __shared__ float s_stat[16 * MT][2];
   __shared__ float s_red[8][16 * MT][17];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
@@ -135,17 +190,17 @@ __global__ void __launch_bounds__(256) dec_linear_direct_kernel(const oasr_dec_l
   const int K = a.K;
   pdl_launch_dependents();
   // the weight stream does not depend on the previous kernel: its first round is in flight before pdl_wait()
-  const T* W = static_cast<const T*>(a.W);
+  const TW* W = static_cast<const TW*>(a.W);
   const int r0 = n0 + g, r1 = n0 + 8 + g;
-  const T* w0 = W + static_cast<int64_t>(r0 < a.N ? r0 : 0) * K + 8 * t;
-  const T* w1 = W + static_cast<int64_t>(r1 < a.N ? r1 : 0) * K + 8 * t;
+  const TW* w0 = W + static_cast<int64_t>(r0 < a.N ? r0 : 0) * K + 8 * t;
+  const TW* w1 = W + static_cast<int64_t>(r1 < a.N ? r1 : 0) * K + 8 * t;
   const bool ok0 = r0 < a.N, ok1 = r1 < a.N;
   const uint4 zero = make_uint4(0, 0, 0, 0);
   int k0 = warp * 32;
-  uint4 b0 = zero, b1 = zero;
+  typename WS::V b0 = WS::zero(), b1 = WS::zero();
   if (k0 < K) {
-    b0 = ok0 ? __ldg(reinterpret_cast<const uint4*>(w0 + k0)) : zero;
-    b1 = ok1 ? __ldg(reinterpret_cast<const uint4*>(w1 + k0)) : zero;
+    b0 = ok0 ? WS::ldg(w0 + k0) : WS::zero();
+    b1 = ok1 ? WS::ldg(w1 + k0) : WS::zero();
   }
   pdl_wait();
   if (a.x_mode == X_LAYERNORM) {   // the affine parameters this thread will need: into L1 now, read as hits in the k loop
@@ -197,11 +252,11 @@ __global__ void __launch_bounds__(256) dec_linear_direct_kernel(const oasr_dec_l
   }
   for (; k0 < K; k0 += 256) {
     const int kn = k0 + 256;
-    uint4 nb0 = zero, nb1 = zero;
+    typename WS::V nb0 = WS::zero(), nb1 = WS::zero();
     uint4 nxa[MT], nxb[MT];
     if (kn < K) {   // the HBM stream and the x fragments run one round ahead of the MMAs
-      nb0 = ok0 ? __ldg(reinterpret_cast<const uint4*>(w0 + kn)) : zero;
-      nb1 = ok1 ? __ldg(reinterpret_cast<const uint4*>(w1 + kn)) : zero;
+      nb0 = ok0 ? WS::ldg(w0 + kn) : WS::zero();
+      nb1 = ok1 ? WS::ldg(w1 + kn) : WS::zero();
 #pragma unroll
       for (int i = 0; i < MT; ++i) {
         nxa[i] = load_x8<T>(a, s_stat, i * 16 + g, kn + 8 * t);
@@ -213,10 +268,11 @@ __global__ void __launch_bounds__(256) dec_linear_direct_kernel(const oasr_dec_l
     }
 #pragma unroll
     for (int i = 0; i < MT; ++i) {
-      DT<T>::mma(acc[i][0], xa[i].x, xb[i].x, xa[i].y, xb[i].y, b0.x, b0.y);
-      DT<T>::mma(acc[i][0], xa[i].z, xb[i].z, xa[i].w, xb[i].w, b0.z, b0.w);
-      DT<T>::mma(acc[i][1], xa[i].x, xb[i].x, xa[i].y, xb[i].y, b1.x, b1.y);
-      DT<T>::mma(acc[i][1], xa[i].z, xb[i].z, xa[i].w, xb[i].w, b1.z, b1.w);
+      const uint4 f0 = WS::frag(b0), f1 = WS::frag(b1);
+      DT<T>::mma(acc[i][0], xa[i].x, xb[i].x, xa[i].y, xb[i].y, f0.x, f0.y);
+      DT<T>::mma(acc[i][0], xa[i].z, xb[i].z, xa[i].w, xb[i].w, f0.z, f0.w);
+      DT<T>::mma(acc[i][1], xa[i].x, xb[i].x, xa[i].y, xb[i].y, f1.x, f1.y);
+      DT<T>::mma(acc[i][1], xa[i].z, xb[i].z, xa[i].w, xb[i].w, f1.z, f1.w);
     }
     b0 = nb0; b1 = nb1;
 #pragma unroll
@@ -240,6 +296,7 @@ __global__ void __launch_bounds__(256) dec_linear_direct_kernel(const oasr_dec_l
     float v = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) v += s_red[w][row][col];
+    if constexpr (WS::kFp8) v *= __ldg(a.w_scale + n);                // s_n sum_k x Q (include/oasr_b200.h)
     if (a.epi == EPI_LOGITS_F32) {   // (x @ E^T).float(): the matmul output is rounded to T first (inf_model.py:357-360)
       static_cast<float*>(a.out)[static_cast<int64_t>(row) * a.ldo + n] = rnd<T>(v);
       continue;
@@ -359,8 +416,10 @@ __device__ __forceinline__ uint4 load_x_plain_or_partial(const oasr_dec_linear_a
   return *reinterpret_cast<const uint4*>(static_cast<const T*>(a.x) + static_cast<int64_t>(row) * a.ldx + k);
 }
 
-template <typename T, int MT>
-__global__ void __launch_bounds__(256, (MT <= 2 ? 2 : 1)) dec_linear_kernel(const oasr_dec_linear_args a, const int KC, const int groups) {
+template <typename T, typename TW, int MT>
+__global__ void __launch_bounds__(256, (MT <= 2 ? 2 : 1)) dec_linear_kernel(const typename Stored<T, TW>::LinearArgs a, const int KC,
+                                                                          const int groups) {
+  using WS = Stored<T, TW>;
   constexpr int MP = 16 * MT;
   extern __shared__ __align__(16) uint8_t dec_smem[];
   const int K = a.K;
@@ -368,28 +427,28 @@ __global__ void __launch_bounds__(256, (MT <= 2 ? 2 : 1)) dec_linear_kernel(cons
   T* x_s = reinterpret_cast<T*>(dec_smem);
   float (*s_red)[MP][17] = reinterpret_cast<float (*)[MP][17]>(dec_smem + static_cast<size_t>(MP) * lds * sizeof(T));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const T* W = static_cast<const T*>(a.W);
+  const TW* W = static_cast<const TW*>(a.W);
   const uint4 zero = make_uint4(0, 0, 0, 0);
   const int group0 = blockIdx.x * groups;
   const int n_groups_total = (a.N + 15) / 16;
   pdl_launch_dependents();
 
   // W rows of a column group for this thread, and the prefetch ring (DEC_PF rounds x 2 n8 tiles)
-  uint4 wb0[DEC_PF], wb1[DEC_PF];
-  auto w_ptrs = [&](int grp, const T*& w0, const T*& w1, bool& ok0, bool& ok1) {
+  typename WS::V wb0[DEC_PF], wb1[DEC_PF];
+  auto w_ptrs = [&](int grp, const TW*& w0, const TW*& w1, bool& ok0, bool& ok1) {
     const int r0 = grp * 16 + g, r1 = r0 + 8;
     ok0 = r0 < a.N; ok1 = r1 < a.N;
     w0 = W + static_cast<int64_t>(ok0 ? r0 : 0) * K + 8 * t;
     w1 = W + static_cast<int64_t>(ok1 ? r1 : 0) * K + 8 * t;
   };
-  const T *w0, *w1;
+  const TW *w0, *w1;
   bool ok0, ok1;
   w_ptrs(group0, w0, w1, ok0, ok1);
 #pragma unroll
   for (int p = 0; p < DEC_PF; ++p) {
     const int k = warp * 32 + 256 * p;
-    wb0[p] = (ok0 && k < K) ? __ldg(reinterpret_cast<const uint4*>(w0 + k)) : zero;
-    wb1[p] = (ok1 && k < K) ? __ldg(reinterpret_cast<const uint4*>(w1 + k)) : zero;
+    wb0[p] = (ok0 && k < K) ? WS::ldg(w0 + k) : WS::zero();
+    wb1[p] = (ok1 && k < K) ? WS::ldg(w1 + k) : WS::zero();
   }
   pdl_wait();     // from here on data written by earlier kernels of the step (x, partials, pos) may be read
 
@@ -439,7 +498,7 @@ __global__ void __launch_bounds__(256, (MT <= 2 ? 2 : 1)) dec_linear_kernel(cons
 #pragma unroll
         for (int e = 0; e < 4; ++e) acc[i][j][e] = 0.f;
     // W pointers of the NEXT group: the ring is refilled from it once this group's rounds are all in flight
-    const T *nw0 = w0, *nw1 = w1;
+    const TW *nw0 = w0, *nw1 = w1;
     bool nok0 = false, nok1 = false;
     const bool has_next = (gi + 1 < groups) && (grp + 1 < n_groups_total);
     if (has_next) w_ptrs(grp + 1, nw0, nw1, nok0, nok1);
@@ -456,12 +515,12 @@ __global__ void __launch_bounds__(256, (MT <= 2 ? 2 : 1)) dec_linear_kernel(cons
       for (int p = 0; p < DEC_PF; ++p) {
         const int k0 = base + 256 * p;
         if (k0 < K) {
-          const uint4 b0 = wb0[p], b1 = wb1[p];
+          const uint4 b0 = WS::frag(wb0[p]), b1 = WS::frag(wb1[p]);
           // refill this ring slot with the same group's round p + DEC_PF (if there is one)
           const int kn = k0 + 256 * DEC_PF;
           if (kn < K) {
-            wb0[p] = ok0 ? __ldg(reinterpret_cast<const uint4*>(w0 + kn)) : zero;
-            wb1[p] = ok1 ? __ldg(reinterpret_cast<const uint4*>(w1 + kn)) : zero;
+            wb0[p] = ok0 ? WS::ldg(w0 + kn) : WS::zero();
+            wb1[p] = ok1 ? WS::ldg(w1 + kn) : WS::zero();
           }
           const T* xrow = x_s + (k0 - kc0) + 8 * t;
 #pragma unroll
@@ -482,8 +541,8 @@ __global__ void __launch_bounds__(256, (MT <= 2 ? 2 : 1)) dec_linear_kernel(cons
 #pragma unroll
       for (int p = 0; p < DEC_PF; ++p) {
         const int k = warp * 32 + 256 * p;
-        wb0[p] = (ok0 && k < K) ? __ldg(reinterpret_cast<const uint4*>(w0 + k)) : zero;
-        wb1[p] = (ok1 && k < K) ? __ldg(reinterpret_cast<const uint4*>(w1 + k)) : zero;
+        wb0[p] = (ok0 && k < K) ? WS::ldg(w0 + k) : WS::zero();
+        wb1[p] = (ok1 && k < K) ? WS::ldg(w1 + k) : WS::zero();
       }
     }
     // fixed-order reduction over the 8 K slices (deterministic), then the epilogue
@@ -503,6 +562,7 @@ __global__ void __launch_bounds__(256, (MT <= 2 ? 2 : 1)) dec_linear_kernel(cons
       float v = 0.f;
 #pragma unroll
       for (int w = 0; w < 8; ++w) v += s_red[w][row][col];
+      if constexpr (WS::kFp8) v *= __ldg(a.w_scale + n);              // s_n sum_k x Q (include/oasr_b200.h)
       if (a.epi == EPI_LOGITS_F32) {   // (x @ E^T).float(): the matmul output is rounded to T first (inf_model.py:357-360)
         static_cast<float*>(a.out)[static_cast<int64_t>(row) * a.ldo + n] = rnd<T>(v);
         continue;
@@ -528,8 +588,9 @@ __global__ void __launch_bounds__(256, (MT <= 2 ? 2 : 1)) dec_linear_kernel(cons
 // ---------------------------------------------------------------------------------------------------------- attention
 // scores[n, h, j] = float(round_T( sum_c round_T(q[c] * hd^-.25) * round_T(k_j[c] * hd^-.25) ))    (inf_model.py:176-181)
 // grid (splits, H, N), 128 threads: 8 lanes per key row (16 bytes = 8 dims each), 16 keys per pass.
-template <typename T>
-__global__ void __launch_bounds__(128) dec_attn_scores_kernel(const oasr_dec_attn_args a, const int kv_group) {
+template <typename T, typename TKV>
+__global__ void __launch_bounds__(128) dec_attn_scores_kernel(const oasr_dec_attn_args a, const int kv_group, const KvScales ks) {
+  using KS = Stored<T, TKV>;
   pdl_launch_dependents();
   pdl_wait();
   const int s = blockIdx.x, h = blockIdx.y, n = blockIdx.z;
@@ -548,28 +609,38 @@ __global__ void __launch_bounds__(128) dec_attn_scores_kernel(const oasr_dec_att
       qs[2 * i] = rnd<T>(p.x * scale); qs[2 * i + 1] = rnd<T>(p.y * scale);
     }
   }
-  const T* kb = static_cast<const T*>(a.k) + static_cast<int64_t>(n / kv_group) * a.kv_seq_stride + h * 64 + c8 * 8;
+  const int64_t kv_n = n / kv_group;
+  const TKV* kb = static_cast<const TKV*>(a.k) + kv_n * a.kv_seq_stride + h * 64 + c8 * 8;
   float* out = a.scores + (static_cast<int64_t>(n) * gridDim.y + h) * a.scores_ld;
-  for (int jb = j0; jb < j1; jb += 128) {   // 8 independent 16-byte loads in flight per thread
-    uint4 u[8];
+  for (int jb = j0; jb < j1; jb += 128) {   // 8 independent 16-byte (e4m3: 8-byte) loads in flight per thread
+    typename KS::V u[8];
+    float sk[8];
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
       const int j = jb + r * 16 + slot;
-      u[r] = (j < j1) ? __ldg(reinterpret_cast<const uint4*>(kb + static_cast<int64_t>(j) * a.kv_row_stride)) : make_uint4(0, 0, 0, 0);
+      u[r] = (j < j1) ? KS::ldg(kb + static_cast<int64_t>(j) * a.kv_row_stride) : KS::zero();
+      if constexpr (KS::kFp8) sk[r] = (j < j1) ? __ldg(ks.k + kv_n * ks.seq + static_cast<int64_t>(j) * ks.row + h) : 0.f;
     }
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
-      const uint32_t w[4] = {u[r].x, u[r].y, u[r].z, u[r].w};
+      const uint4 f = KS::frag(u[r]);
+      const uint32_t w[4] = {f.x, f.y, f.z, f.w};
       float acc = 0.f;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float2 p = DT<T>::unpack2(w[i]);
-        acc = fmaf(qs[2 * i], rnd<T>(p.x * scale), acc);
-        acc = fmaf(qs[2 * i + 1], rnd<T>(p.y * scale), acc);
+        if constexpr (KS::kFp8) {          // q~ . QK, scaled once below
+          acc = fmaf(qs[2 * i], p.x, acc);
+          acc = fmaf(qs[2 * i + 1], p.y, acc);
+        } else {
+          acc = fmaf(qs[2 * i], rnd<T>(p.x * scale), acc);
+          acc = fmaf(qs[2 * i + 1], rnd<T>(p.y * scale), acc);
+        }
       }
       acc += __shfl_xor_sync(0xffffffffu, acc, 1);
       acc += __shfl_xor_sync(0xffffffffu, acc, 2);
       acc += __shfl_xor_sync(0xffffffffu, acc, 4);
+      if constexpr (KS::kFp8) acc *= sk[r] * scale;
       const int j = jb + r * 16 + slot;
       if (c8 == 0 && j < j1) out[j] = rnd<T>(acc);
     }
@@ -579,8 +650,9 @@ __global__ void __launch_bounds__(128) dec_attn_scores_kernel(const oasr_dec_att
 // partial[s, n, h*64 + c] = sum_{j in split s} float(round_T(softmax(scores)[j])) * v_j[c]   (fp32; the consumer adds the
 // splits in order and rounds once = the single rounding of `w @ v`).  Every CTA first derives the row maximum and the
 // normaliser from ALL scores of its (n, h) (<= 1500 floats, L2-resident), as F.softmax(qk.float()) does.
-template <typename T>
-__global__ void __launch_bounds__(128) dec_attn_pv_kernel(const oasr_dec_attn_args a, const int kv_group) {
+template <typename T, typename TKV>
+__global__ void __launch_bounds__(128) dec_attn_pv_kernel(const oasr_dec_attn_args a, const int kv_group, const KvScales ks) {
+  using KS = Stored<T, TKV>;
   __shared__ float s_part[4];
   __shared__ float s_o[4][64];
   pdl_launch_dependents();
@@ -607,21 +679,24 @@ __global__ void __launch_bounds__(128) dec_attn_pv_kernel(const oasr_dec_attn_ar
   const float inv_l = 1.0f / l;
 
   const int c8 = threadIdx.x & 7, slot = threadIdx.x >> 3;
-  const T* vb = static_cast<const T*>(a.v) + static_cast<int64_t>(n / kv_group) * a.kv_seq_stride + h * 64 + c8 * 8;
+  const int64_t kv_n = n / kv_group;
+  const TKV* vb = static_cast<const TKV*>(a.v) + kv_n * a.kv_seq_stride + h * 64 + c8 * 8;
   float o[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   for (int jb = j0; jb < j1; jb += 128) {
-    uint4 u[8];
+    typename KS::V u[8];
     float p[8];
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
       const int j = jb + r * 16 + slot;
       const bool ok = j < j1;
-      u[r] = ok ? __ldg(reinterpret_cast<const uint4*>(vb + static_cast<int64_t>(j) * a.kv_row_stride)) : make_uint4(0, 0, 0, 0);
+      u[r] = ok ? KS::ldg(vb + static_cast<int64_t>(j) * a.kv_row_stride) : KS::zero();
       p[r] = ok ? rnd<T>(expf(sc[j] - m) * inv_l) : 0.f;            // softmax(...).to(q.dtype)
+      if constexpr (KS::kFp8) p[r] *= ok ? __ldg(ks.v + kv_n * ks.seq + static_cast<int64_t>(j) * ks.row + h) : 0.f;   // p_j sV_j
     }
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
-      const uint32_t w[4] = {u[r].x, u[r].y, u[r].z, u[r].w};
+      const uint4 f = KS::frag(u[r]);
+      const uint32_t w[4] = {f.x, f.y, f.z, f.w};
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float2 vv = DT<T>::unpack2(w[i]);
@@ -651,8 +726,9 @@ __global__ void __launch_bounds__(128) dec_attn_pv_kernel(const oasr_dec_attn_ar
 // One CTA per (n, h) when the key range is not split (self-attention always; cross-attention once n x heads fills the
 // machine): scores stay in shared memory, softmax and P V follow in the same kernel -- one launch and no round trip through
 // global memory instead of two.  Same arithmetic and rounding points as the two-kernel form above.
-template <typename T>
-__global__ void __launch_bounds__(128) dec_attn_fused_kernel(const oasr_dec_attn_args a, const int kv_group) {
+template <typename T, typename TKV>
+__global__ void __launch_bounds__(128) dec_attn_fused_kernel(const oasr_dec_attn_args a, const int kv_group, const KvScales ks) {
+  using KS = Stored<T, TKV>;
   __shared__ float s_sc[1536];
   __shared__ float s_part[4];
   __shared__ float s_o[4][64];
@@ -673,29 +749,39 @@ __global__ void __launch_bounds__(128) dec_attn_fused_kernel(const oasr_dec_attn
       qs[2 * i] = rnd<T>(p.x * scale); qs[2 * i + 1] = rnd<T>(p.y * scale);
     }
   }
-  const T* kb = static_cast<const T*>(a.k) + static_cast<int64_t>(n / kv_group) * a.kv_seq_stride + h * 64 + c8 * 8;
-  const T* vb = static_cast<const T*>(a.v) + static_cast<int64_t>(n / kv_group) * a.kv_seq_stride + h * 64 + c8 * 8;
+  const int64_t kv_n = n / kv_group;
+  const TKV* kb = static_cast<const TKV*>(a.k) + kv_n * a.kv_seq_stride + h * 64 + c8 * 8;
+  const TKV* vb = static_cast<const TKV*>(a.v) + kv_n * a.kv_seq_stride + h * 64 + c8 * 8;
   float m = -INFINITY;
   for (int jb = 0; jb < nkeys; jb += 128) {
-    uint4 u[8];
+    typename KS::V u[8];
+    float sk[8];
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
       const int j = jb + r * 16 + slot;
-      u[r] = (j < nkeys) ? __ldg(reinterpret_cast<const uint4*>(kb + static_cast<int64_t>(j) * a.kv_row_stride)) : make_uint4(0, 0, 0, 0);
+      u[r] = (j < nkeys) ? KS::ldg(kb + static_cast<int64_t>(j) * a.kv_row_stride) : KS::zero();
+      if constexpr (KS::kFp8) sk[r] = (j < nkeys) ? __ldg(ks.k + kv_n * ks.seq + static_cast<int64_t>(j) * ks.row + h) : 0.f;
     }
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
-      const uint32_t w[4] = {u[r].x, u[r].y, u[r].z, u[r].w};
+      const uint4 f = KS::frag(u[r]);
+      const uint32_t w[4] = {f.x, f.y, f.z, f.w};
       float acc = 0.f;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float2 p = DT<T>::unpack2(w[i]);
-        acc = fmaf(qs[2 * i], rnd<T>(p.x * scale), acc);
-        acc = fmaf(qs[2 * i + 1], rnd<T>(p.y * scale), acc);
+        if constexpr (KS::kFp8) {
+          acc = fmaf(qs[2 * i], p.x, acc);
+          acc = fmaf(qs[2 * i + 1], p.y, acc);
+        } else {
+          acc = fmaf(qs[2 * i], rnd<T>(p.x * scale), acc);
+          acc = fmaf(qs[2 * i + 1], rnd<T>(p.y * scale), acc);
+        }
       }
       acc += __shfl_xor_sync(0xffffffffu, acc, 1);
       acc += __shfl_xor_sync(0xffffffffu, acc, 2);
       acc += __shfl_xor_sync(0xffffffffu, acc, 4);
+      if constexpr (KS::kFp8) acc *= sk[r] * scale;
       const int j = jb + r * 16 + slot;
       if (j < nkeys) {
         const float sc = rnd<T>(acc);
@@ -718,18 +804,20 @@ __global__ void __launch_bounds__(128) dec_attn_fused_kernel(const oasr_dec_attn
   const float inv_l = 1.0f / l;
   float o[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   for (int jb = 0; jb < nkeys; jb += 128) {
-    uint4 u[8];
+    typename KS::V u[8];
     float p[8];
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
       const int j = jb + r * 16 + slot;
       const bool ok = j < nkeys;
-      u[r] = ok ? __ldg(reinterpret_cast<const uint4*>(vb + static_cast<int64_t>(j) * a.kv_row_stride)) : make_uint4(0, 0, 0, 0);
+      u[r] = ok ? KS::ldg(vb + static_cast<int64_t>(j) * a.kv_row_stride) : KS::zero();
       p[r] = ok ? rnd<T>(expf(s_sc[j] - m) * inv_l) : 0.f;
+      if constexpr (KS::kFp8) p[r] *= ok ? __ldg(ks.v + kv_n * ks.seq + static_cast<int64_t>(j) * ks.row + h) : 0.f;
     }
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
-      const uint32_t w[4] = {u[r].x, u[r].y, u[r].z, u[r].w};
+      const uint4 f = KS::frag(u[r]);
+      const uint32_t w[4] = {f.x, f.y, f.z, f.w};
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float2 vv = DT<T>::unpack2(w[i]);
@@ -1398,8 +1486,8 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, cudaStre
   return cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 
-template <typename T, int MT>
-int launch_linear(const oasr_dec_linear_args& a, cudaStream_t st) {
+template <typename T, typename TW, int MT>
+int launch_linear(const typename Stored<T, TW>::LinearArgs& a, cudaStream_t st) {
   constexpr int MP = 16 * MT;
   // whole-K staging when it fits (always for the LayerNorm prologue, K = d <= 1280); otherwise chunks of 256 * DEC_PF
   int KC = a.K;
@@ -1417,7 +1505,7 @@ int launch_linear(const oasr_dec_linear_args& a, cudaStream_t st) {
   const int grid = (int)ceil_div(n_groups, groups);
   static size_t attr_smem = 0;
   if (smem > attr_smem) {
-    OASR_CUDA_OK(cudaFuncSetAttribute(dec_linear_kernel<T, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget));
+    OASR_CUDA_OK(cudaFuncSetAttribute(dec_linear_kernel<T, TW, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget));
     attr_smem = budget;
   }
   cudaLaunchConfig_t cfg = {};
@@ -1430,20 +1518,38 @@ int launch_linear(const oasr_dec_linear_args& a, cudaStream_t st) {
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  OASR_CUDA_OK(cudaLaunchKernelEx(&cfg, dec_linear_kernel<T, MT>, a, KC, groups));
+  OASR_CUDA_OK(cudaLaunchKernelEx(&cfg, dec_linear_kernel<T, TW, MT>, a, KC, groups));
   return OASR_OK;
 }
-template <typename T, int MT>
-int launch_linear_direct(const oasr_dec_linear_args& a, cudaStream_t st) {
-  OASR_CUDA_OK(launch_pdl(dec_linear_direct_kernel<T, MT>, dim3((unsigned)ceil_div(a.N, 16)), dim3(256), st, a));
+template <typename T, typename TW, int MT>
+int launch_linear_direct(const typename Stored<T, TW>::LinearArgs& a, cudaStream_t st) {
+  OASR_CUDA_OK(launch_pdl(dec_linear_direct_kernel<T, TW, MT>, dim3((unsigned)ceil_div(a.N, 16)), dim3(256), st, a));
   return OASR_OK;
 }
-template <typename T>
-int dispatch_linear(const oasr_dec_linear_args& a, cudaStream_t st) {
+// TW: the weight storage, T or uint8_t e4m3 codes (whose argument block carries the per-row scales)
+template <typename T, typename TW>
+int dispatch_linear(const typename Stored<T, TW>::LinearArgs& a, cudaStream_t st) {
   // the direct form up to 32 rows (no staging round trip for a handful of rows), the staged form from there on
-  if (a.M <= 16) return launch_linear_direct<T, 1>(a, st);
-  if (a.M <= 32) return launch_linear_direct<T, 2>(a, st);
-  return launch_linear<T, 4>(a, st);
+  if (a.M <= 16) return launch_linear_direct<T, TW, 1>(a, st);
+  if (a.M <= 32) return launch_linear_direct<T, TW, 2>(a, st);
+  return launch_linear<T, TW, 4>(a, st);
+}
+
+int check_linear_args(const oasr_dec_linear_args* a) {
+  OASR_REQUIRE(a != nullptr, "dec_linear: null arguments");
+  OASR_REQUIRE(a->M >= 1 && a->M <= 64, "dec_linear: 1 <= M <= 64 sequences (got %d)", a->M);
+  OASR_REQUIRE(a->N >= 1 && a->K >= 32 && (a->K % 32) == 0, "dec_linear: K must be a multiple of 32 (got %d)", a->K);
+  OASR_REQUIRE(a->x && a->W && a->out, "dec_linear: null tensor");
+  OASR_REQUIRE(((uintptr_t)a->x & 15) == 0 && ((uintptr_t)a->W & 15) == 0, "dec_linear: x and W must be 16-byte aligned");
+  OASR_REQUIRE(a->x_mode >= 0 && a->x_mode <= 2 && a->epi >= 0 && a->epi <= 4, "dec_linear: bad mode");
+  OASR_REQUIRE(a->x_mode != X_LAYERNORM || (a->ln_gamma && a->ln_beta), "dec_linear: LayerNorm mode needs gamma / beta");
+  OASR_REQUIRE(a->x_mode != X_LAYERNORM || (a->K <= 1280 && a->K % 8 == 0), "dec_linear: LayerNorm prologue supports K <= 1280 (got %d)", a->K);
+  OASR_REQUIRE(a->x_mode != X_PARTIAL_SUM || a->n_partials >= 1, "dec_linear: partial-sum mode needs n_partials >= 1");
+  OASR_REQUIRE(a->x_mode == X_PARTIAL_SUM || (a->ldx % 8) == 0, "dec_linear: ldx must be a multiple of 8");
+  OASR_REQUIRE(a->epi != EPI_RESIDUAL || a->res, "dec_linear: residual epilogue needs res");
+  OASR_REQUIRE(a->epi != EPI_QKV_SCATTER || (a->k_cache && a->v_cache && a->pos_ptr && a->N % 3 == 0), "dec_linear: qkv scatter needs caches and pos");
+  OASR_REQUIRE(a->dtype == OASR_DTYPE_F16 || a->dtype == OASR_DTYPE_BF16, "dec_linear: unknown dtype %d", a->dtype);
+  return OASR_OK;
 }
 
 }  // namespace
@@ -1465,46 +1571,50 @@ extern "C" int oasr_dec_embed(const int32_t* tokens, int64_t ld_tokens, const in
 }
 
 extern "C" int oasr_dec_linear(const oasr_dec_linear_args* a, void* stream) {
-  OASR_REQUIRE(a != nullptr, "dec_linear: null arguments");
-  OASR_REQUIRE(a->M >= 1 && a->M <= 64, "dec_linear: 1 <= M <= 64 sequences (got %d)", a->M);
-  OASR_REQUIRE(a->N >= 1 && a->K >= 32 && (a->K % 32) == 0, "dec_linear: K must be a multiple of 32 (got %d)", a->K);
-  OASR_REQUIRE(a->x && a->W && a->out, "dec_linear: null tensor");
-  OASR_REQUIRE(((uintptr_t)a->x & 15) == 0 && ((uintptr_t)a->W & 15) == 0, "dec_linear: x and W must be 16-byte aligned");
-  OASR_REQUIRE(a->x_mode >= 0 && a->x_mode <= 2 && a->epi >= 0 && a->epi <= 4, "dec_linear: bad mode");
-  OASR_REQUIRE(a->x_mode != X_LAYERNORM || (a->ln_gamma && a->ln_beta), "dec_linear: LayerNorm mode needs gamma / beta");
-  OASR_REQUIRE(a->x_mode != X_LAYERNORM || (a->K <= 1280 && a->K % 8 == 0), "dec_linear: LayerNorm prologue supports K <= 1280 (got %d)", a->K);
-  OASR_REQUIRE(a->x_mode != X_PARTIAL_SUM || a->n_partials >= 1, "dec_linear: partial-sum mode needs n_partials >= 1");
-  OASR_REQUIRE(a->x_mode == X_PARTIAL_SUM || (a->ldx % 8) == 0, "dec_linear: ldx must be a multiple of 8");
-  OASR_REQUIRE(a->epi != EPI_RESIDUAL || a->res, "dec_linear: residual epilogue needs res");
-  OASR_REQUIRE(a->epi != EPI_QKV_SCATTER || (a->k_cache && a->v_cache && a->pos_ptr && a->N % 3 == 0), "dec_linear: qkv scatter needs caches and pos");
-  if (a->dtype == OASR_DTYPE_F16) return dispatch_linear<__half>(*a, (cudaStream_t)stream);
-  if (a->dtype == OASR_DTYPE_BF16) return dispatch_linear<bf16>(*a, (cudaStream_t)stream);
-  OASR_REQUIRE(false, "dec_linear: unknown dtype %d", a->dtype);
+  if (int rc = check_linear_args(a)) return rc;
+  if (a->dtype == OASR_DTYPE_F16) return dispatch_linear<__half, __half>(*a, (cudaStream_t)stream);
+  return dispatch_linear<bf16, bf16>(*a, (cudaStream_t)stream);
+}
+
+extern "C" int oasr_dec_linear_fp8w(const oasr_dec_linear_args* a, const float* w_scale, void* stream) {
+  if (int rc = check_linear_args(a)) return rc;
+  OASR_REQUIRE(w_scale != nullptr, "dec_linear_fp8w: null weight scales");
+  LinearArgsFp8 a8;
+  static_cast<oasr_dec_linear_args&>(a8) = *a;
+  a8.w_scale = w_scale;
+  if (a->dtype == OASR_DTYPE_F16) return dispatch_linear<__half, uint8_t>(a8, (cudaStream_t)stream);
+  return dispatch_linear<bf16, uint8_t>(a8, (cudaStream_t)stream);
 }
 
 namespace {
-int dec_attention(const oasr_dec_attn_args* a, int kv_group, cudaStream_t st) {
+// TKV: the K / V storage, T (ks unused) or uint8_t e4m3 codes with per-(key, head) scales
+template <typename T, typename TKV>
+int launch_attention(const oasr_dec_attn_args* a, int kv_group, const KvScales& ks, cudaStream_t st) {
+  dim3 grid((unsigned)a->n_splits, (unsigned)a->n_head, (unsigned)a->n_seq);
+  if (a->n_splits == 1 && (a->pos_ptr != nullptr || a->n_keys <= 1536)) {   // whole key range in one CTA: fused form
+    OASR_CUDA_OK(launch_pdl(dec_attn_fused_kernel<T, TKV>, grid, dim3(128), st, *a, kv_group, ks));
+    return OASR_OK;
+  }
+  OASR_CUDA_OK(launch_pdl(dec_attn_scores_kernel<T, TKV>, grid, dim3(128), st, *a, kv_group, ks));
+  OASR_CUDA_OK(launch_pdl(dec_attn_pv_kernel<T, TKV>, grid, dim3(128), st, *a, kv_group, ks));
+  return OASR_OK;
+}
+
+int check_attention_args(const oasr_dec_attn_args* a, int kv_group) {
   OASR_REQUIRE(a != nullptr && a->q && a->k && a->v && a->scores && a->out_partial, "dec_attention: null tensor");
   OASR_REQUIRE(a->n_seq >= 1 && a->n_head >= 1 && a->n_splits >= 1, "dec_attention: bad sizes");
   OASR_REQUIRE(kv_group >= 1, "dec_attention: kv_group must be >= 1 (got %d)", kv_group);
   OASR_REQUIRE(a->pos_ptr != nullptr || a->n_keys >= 1, "dec_attention: key count missing");
   OASR_REQUIRE((a->ldq % 8) == 0 && (a->kv_row_stride % 8) == 0 && (a->kv_seq_stride % 8) == 0, "dec_attention: strides must be multiples of 8");
-  dim3 grid((unsigned)a->n_splits, (unsigned)a->n_head, (unsigned)a->n_seq);
   OASR_REQUIRE(a->dtype == OASR_DTYPE_F16 || a->dtype == OASR_DTYPE_BF16, "dec_attention: unknown dtype %d", a->dtype);
-  const bool f16 = a->dtype == OASR_DTYPE_F16;
-  if (a->n_splits == 1 && (a->pos_ptr != nullptr || a->n_keys <= 1536)) {   // whole key range in one CTA: fused form
-    if (f16) OASR_CUDA_OK(launch_pdl(dec_attn_fused_kernel<__half>, grid, dim3(128), st, *a, kv_group));
-    else OASR_CUDA_OK(launch_pdl(dec_attn_fused_kernel<bf16>, grid, dim3(128), st, *a, kv_group));
-    return OASR_OK;
-  }
-  if (f16) {
-    OASR_CUDA_OK(launch_pdl(dec_attn_scores_kernel<__half>, grid, dim3(128), st, *a, kv_group));
-    OASR_CUDA_OK(launch_pdl(dec_attn_pv_kernel<__half>, grid, dim3(128), st, *a, kv_group));
-  } else {
-    OASR_CUDA_OK(launch_pdl(dec_attn_scores_kernel<bf16>, grid, dim3(128), st, *a, kv_group));
-    OASR_CUDA_OK(launch_pdl(dec_attn_pv_kernel<bf16>, grid, dim3(128), st, *a, kv_group));
-  }
   return OASR_OK;
+}
+
+int dec_attention(const oasr_dec_attn_args* a, int kv_group, cudaStream_t st) {
+  if (int rc = check_attention_args(a, kv_group)) return rc;
+  const KvScales none = {nullptr, nullptr, 0, 0};
+  if (a->dtype == OASR_DTYPE_F16) return launch_attention<__half, __half>(a, kv_group, none, st);
+  return launch_attention<bf16, bf16>(a, kv_group, none, st);
 }
 }  // namespace
 
@@ -1512,6 +1622,16 @@ extern "C" int oasr_dec_attention(const oasr_dec_attn_args* a, void* stream) { r
 
 extern "C" int oasr_dec_attention_grouped(const oasr_dec_attn_args* a, int kv_group, void* stream) {
   return dec_attention(a, kv_group, (cudaStream_t)stream);
+}
+
+extern "C" int oasr_dec_attention_fp8kv(const oasr_dec_attn_args* a, const float* k_scale, const float* v_scale,
+                                        int64_t scale_seq_stride, int64_t scale_row_stride, int kv_group, void* stream) {
+  if (int rc = check_attention_args(a, kv_group)) return rc;
+  OASR_REQUIRE(k_scale && v_scale && scale_seq_stride >= 0 && scale_row_stride >= a->n_head,
+               "dec_attention_fp8kv: scales missing or row stride < n_head");
+  const KvScales ks = {k_scale, v_scale, scale_seq_stride, scale_row_stride};
+  if (a->dtype == OASR_DTYPE_F16) return launch_attention<__half, uint8_t>(a, kv_group, ks, (cudaStream_t)stream);
+  return launch_attention<bf16, uint8_t>(a, kv_group, ks, (cudaStream_t)stream);
 }
 
 extern "C" int oasr_dec_sample(const oasr_dec_sample_args* a, void* stream) {

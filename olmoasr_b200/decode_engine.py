@@ -25,6 +25,12 @@ cross-attention K / V: one projection per clip.
 The activation dtype is fp16 (upstream default `fp16=True`) or bf16; the decoder-step kernels reproduce the reference's
 rounding points in that dtype.  The audio encoder and the cross K/V projection run on the bf16 wgmma kernels in both
 cases (their bf16 outputs are converted to fp16 for an fp16 decoder).
+
+`fp8=True` (DecodingOptions.fp8) halves the two large byte streams of the step.  The six block projections of every
+layer are stored as e4m3 codes with one fp32 scale per output row, quantised in refresh_weights() from the 16-bit cast;
+cross K / V is quantised in prepare() from the bf16 projection, with one scale per (key, head, K|V) group of 64.  Both
+are decoded to the activation dtype in registers (include/oasr_b200.h states the arithmetic).  The tied logits head, the
+self-attention cache and every activation stay 16-bit; the step issues the same launches as the 16-bit engine.
 """
 from __future__ import annotations
 
@@ -39,6 +45,7 @@ from torch import Tensor, nn
 from . import _lib
 from ._lib import (DTYPE_BF16, DTYPE_F16, DTYPE_F32, DecAttnArgs, DecBeamArgs, DecLinearArgs, DecSampleArgs, DecSampleRulesArgs,
                    call, ptr, stream)
+from .kernels import FP8_E4M3, quantize_fp8_rows
 
 X_PLAIN, X_LAYERNORM, X_PARTIAL_SUM = 0, 1, 2
 EPI_STORE, EPI_GELU, EPI_RESIDUAL, EPI_LOGITS_F32, EPI_QKV_SCATTER = 0, 1, 2, 3, 4
@@ -46,6 +53,7 @@ _DT = {torch.float16: DTYPE_F16, torch.bfloat16: DTYPE_BF16, torch.float32: DTYP
 TIMESTAMP_BEGIN, NO_TIMESTAMPS = 50363, 50362
 BEAM_MAX, MAX_CANDIDATES = 8, 32
 BEAM_SCRATCH = 48      # floats per (row, slice) of the beam candidate and rule-aware sampling kernels
+FP8_WEIGHTS = ("wqkv", "wo", "wcq", "wco", "w1", "w2")    # the per-layer projections an fp8 engine stores as e4m3
 
 
 _M64 = (1 << 64) - 1
@@ -80,7 +88,7 @@ def _convert(src: Tensor, dst: Tensor) -> Tensor:
 class DecodeEngine:
     MAX_BATCH = 64
 
-    def __init__(self, model, dtype: torch.dtype = torch.float16, max_batch: int = 64):
+    def __init__(self, model, dtype: torch.dtype = torch.float16, max_batch: int = 64, fp8: bool = False):
         if dtype not in (torch.float16, torch.bfloat16):
             raise ValueError("DecodeEngine: dtype must be torch.float16 or torch.bfloat16")
         if not 1 <= max_batch <= self.MAX_BATCH:
@@ -99,12 +107,18 @@ class DecodeEngine:
         if self.d != self.H * 64:
             raise ValueError("DecodeEngine: head dimension must be 64")
         self.max_batch = max_batch
+        self.fp8 = bool(fp8)
         N, d, L = max_batch, self.d, self.L
         dev = self.dev
         z = lambda *shape, dt=dtype: torch.zeros(shape, device=dev, dtype=dt)
         # static state -- addresses are baked into the CUDA graphs
         self.self_k, self.self_v = z(L, N, self.n_ctx, d), z(L, N, self.n_ctx, d)
-        self.cross_kv = z(L, N * self.n_audio_ctx, 2 * d)
+        if self.fp8:    # e4m3 codes; one fp32 scale per (key, head, K|V): K heads first, then V heads
+            self.cross_kv = z(L, N * self.n_audio_ctx, 2 * d, dt=torch.uint8)
+            self.cross_scale = z(L, N * self.n_audio_ctx, 2 * self.H, dt=torch.float32)
+        else:
+            self.cross_kv = z(L, N * self.n_audio_ctx, 2 * d)
+            self.cross_scale = None
         self.x, self.q, self.h = z(N, d), z(N, d), z(N, 4 * d)
         self.scores = z(N, self.H, 1536, dt=torch.float32)
         self.max_splits = 8       # key-range splits of the cross-attention at small batches (each split's fp32 partial is re-read by the out projection)
@@ -147,7 +161,9 @@ class DecodeEngine:
         return [p for p in self.model.decoder.parameters()]
 
     def refresh_weights(self):
-        """(Re)cast the decoder weights into the activation dtype when a parameter changed (checkpoint load, training)."""
+        """(Re)cast the decoder weights into the activation dtype when a parameter changed (checkpoint load, training);
+        an fp8 engine then quantises the block projections (FP8_WEIGHTS) per output row and keeps only the e4m3 codes
+        and their scales (`<name>_s`)."""
         sig = tuple((p.data_ptr(), p._version) for p in self._params())
         if sig == self._w_sig:
             return
@@ -181,13 +197,19 @@ class DecodeEngine:
                 ln1=(blk.attn_ln.weight.detach(), blk.attn_ln.bias.detach(), blk.attn_ln.eps),
                 lnc=(blk.cross_attn_ln.weight.detach(), blk.cross_attn_ln.bias.detach(), blk.cross_attn_ln.eps),
                 ln2=(blk.mlp_ln.weight.detach(), blk.mlp_ln.bias.detach(), blk.mlp_ln.eps)))
+            if self.fp8:
+                lw = layers[-1]
+                for name in FP8_WEIGHTS:
+                    lw[name], lw[name + "_s"] = quantize_fp8_rows(lw[name], FP8_E4M3)
         self._w = dict(layers=layers, emb_t=cast(dec.token_embedding.weight), emb=dec.token_embedding.weight.detach(),
                        pos=dec.positional_embedding.detach(), ln=(dec.ln.weight.detach(), dec.ln.bias.detach(), dec.ln.eps))
         self._w_sig = sig
         self._graphs.clear()        # weight buffers were re-allocated: graphs hold their addresses
 
     # ---- kernel wrappers ----------------------------------------------------------------------------------------
-    def _linear(self, n, x, W, bias, out, *, x_mode=X_PLAIN, ln=None, epi=EPI_STORE, res=None, n_partials=0, kv=None, K_=None):
+    def _linear(self, n, x, W, bias, out, *, x_mode=X_PLAIN, ln=None, epi=EPI_STORE, res=None, n_partials=0, kv=None, K_=None,
+                w_scale=None):
+        """One skinny Linear; `w_scale` (N,) fp32 means W holds e4m3 codes (oasr_dec_linear_fp8w)."""
         a = DecLinearArgs()
         a.x, a.x_mode, a.n_partials = ptr(x), x_mode, n_partials
         a.K = W.shape[1] if K_ is None else K_
@@ -202,9 +224,14 @@ class DecodeEngine:
         if kv is not None:
             a.k_cache, a.v_cache, a.cache_len, a.pos_ptr = ptr(kv[0]), ptr(kv[1]), self.n_ctx, ptr(self.pos)
         a.M, a.N, a.dtype = n, W.shape[0], self.dt
-        call("oasr_dec_linear", ctypes.byref(a), stream())
+        if w_scale is None:
+            call("oasr_dec_linear", ctypes.byref(a), stream())
+        else:
+            call("oasr_dec_linear_fp8w", ctypes.byref(a), ptr(w_scale), stream())
 
-    def _attention(self, n, k, v, seq_stride, row_stride, part, splits, n_keys=None, kv_group=1):
+    def _attention(self, n, k, v, seq_stride, row_stride, part, splits, n_keys=None, kv_group=1, kv_scales=None):
+        """One decode attention; kv_scales = (k_scale, v_scale, seq stride, row stride) means k / v hold e4m3 codes with
+        one scale per (key, head) (oasr_dec_attention_fp8kv)."""
         a = DecAttnArgs()
         a.q, a.ldq = ptr(self.q), self.q.stride(0)
         a.k, a.v, a.kv_seq_stride, a.kv_row_stride = ptr(k), ptr(v), seq_stride, row_stride
@@ -213,7 +240,10 @@ class DecodeEngine:
         a.pos_ptr = None if n_keys is not None else ptr(self.pos)
         a.n_keys = n_keys or 0
         a.n_seq, a.n_head, a.n_splits, a.scale, a.dtype = n, self.H, splits, 64 ** -0.25, self.dt
-        if kv_group == 1:
+        if kv_scales is not None:
+            ks, vs, s_seq, s_row = kv_scales
+            call("oasr_dec_attention_fp8kv", ctypes.byref(a), ptr(ks), ptr(vs), s_seq, s_row, kv_group, stream())
+        elif kv_group == 1:
             call("oasr_dec_attention", ctypes.byref(a), stream())
         else:                           # sequence r reads cross K / V entry r // kv_group (the beams of one clip)
             call("oasr_dec_attention_grouped", ctypes.byref(a), kv_group, stream())
@@ -249,17 +279,26 @@ class DecodeEngine:
         part_self = self.part_self.view(-1)[: n * d].view(1, n, d)
         part_cross = self.part_cross.view(-1)[: sc * n * d].view(sc, n, d)
         kv_group = self._group
+        # fp8: the scales ride along as keyword arguments (the 16-bit engine's calls are exactly what they were)
+        ws = (lambda lw, name: {"w_scale": lw[name + "_s"]}) if self.fp8 else (lambda lw, name: {})
         for l, lw in enumerate(w["layers"]):
             self._linear(n, x, lw["wqkv"], lw["bqkv"], q, x_mode=X_LAYERNORM, ln=lw["ln1"], epi=EPI_QKV_SCATTER,
-                         kv=(self.self_k[l], self.self_v[l]))
+                         kv=(self.self_k[l], self.self_v[l]), **ws(lw, "wqkv"))
             self._attention(n, self.self_k[l], self.self_v[l], seq_self, d, part_self, 1)
-            self._linear(n, part_self, lw["wo"], lw["bo"], x, x_mode=X_PARTIAL_SUM, n_partials=1, epi=EPI_RESIDUAL, res=x)
-            self._linear(n, x, lw["wcq"], lw["bcq"], q, x_mode=X_LAYERNORM, ln=lw["lnc"])
+            self._linear(n, part_self, lw["wo"], lw["bo"], x, x_mode=X_PARTIAL_SUM, n_partials=1, epi=EPI_RESIDUAL, res=x,
+                         **ws(lw, "wo"))
+            self._linear(n, x, lw["wcq"], lw["bcq"], q, x_mode=X_LAYERNORM, ln=lw["lnc"], **ws(lw, "wcq"))
             ckv = self.cross_kv[l]
-            self._attention(n, ckv, ckv[:, d:], seq_cross, 2 * d, part_cross, sc, n_keys=self.n_audio_ctx, kv_group=kv_group)
-            self._linear(n, part_cross, lw["wco"], lw["bco"], x, x_mode=X_PARTIAL_SUM, n_partials=sc, epi=EPI_RESIDUAL, res=x)
-            self._linear(n, x, lw["w1"], lw["b1"], h, x_mode=X_LAYERNORM, ln=lw["ln2"], epi=EPI_GELU)
-            self._linear(n, h, lw["w2"], lw["b2"], x, epi=EPI_RESIDUAL, res=x)
+            kvs = {}
+            if self.fp8:
+                cs = self.cross_scale[l]
+                kvs = {"kv_scales": (cs, cs[:, self.H:], self.n_audio_ctx * cs.stride(0), cs.stride(0))}
+            self._attention(n, ckv, ckv[:, d:], seq_cross, 2 * d, part_cross, sc, n_keys=self.n_audio_ctx, kv_group=kv_group,
+                            **kvs)
+            self._linear(n, part_cross, lw["wco"], lw["bco"], x, x_mode=X_PARTIAL_SUM, n_partials=sc, epi=EPI_RESIDUAL, res=x,
+                         **ws(lw, "wco"))
+            self._linear(n, x, lw["w1"], lw["b1"], h, x_mode=X_LAYERNORM, ln=lw["ln2"], epi=EPI_GELU, **ws(lw, "w1"))
+            self._linear(n, h, lw["w2"], lw["b2"], x, epi=EPI_RESIDUAL, res=x, **ws(lw, "w2"))
         self._linear(n, x, w["emb_t"], None, self.logits, x_mode=X_LAYERNORM, ln=w["ln"], epi=EPI_LOGITS_F32)
         if self._beam_cfg is not None:
             self._enqueue_beam_select()
@@ -321,7 +360,8 @@ class DecodeEngine:
     @torch.no_grad()
     def prepare(self, audio_features: Tensor):
         """Project the encoder output into every layer's cross-attention K / V once (inf_model.py:164-167: `kv_cache[self.key]`
-        is filled on the first call and only read afterwards) with the wgmma GEMM."""
+        is filled on the first call and only read afterwards) with the wgmma GEMM.  An fp8 engine quantises the bf16
+        projection as rows of 64 (one per key, head and K|V) into the e4m3 buffer and its scales, for either dtype."""
         from ._core import _as_bf16_2d, linear_fwd
 
         self.refresh_weights()
@@ -338,7 +378,11 @@ class DecodeEngine:
             wkv, bkv = blk.cross_attn.fused_kv()
             if self._w["layers"][l]["wckv"] is not None:
                 wkv = self._w["layers"][l]["wckv"]
-            if self.dtype == torch.bfloat16:
+            if self.fp8:
+                kv = linear_fwd(xa, wkv, bkv)
+                call("oasr_quantize_fp8_rows", ptr(kv), 64, rows * 2 * self.H, 64, DTYPE_BF16, FP8_E4M3, 0,
+                     ptr(self.cross_kv[l]), 64, ptr(self.cross_scale[l]), stream())
+            elif self.dtype == torch.bfloat16:
                 linear_fwd(xa, wkv, bkv, out=self.cross_kv[l][:rows])
             else:
                 _convert(linear_fwd(xa, wkv, bkv), self.cross_kv[l][:rows])
@@ -552,10 +596,18 @@ class DecodeEngine:
     # ---- roofline bookkeeping --------------------------------------------------------------------------------------
     def step_bytes(self, n: int, t: int) -> int:
         """Algorithmic HBM bytes of one step at self-attention length t (SURVEY.md 8(d)): every decoder weight once (shared by
-        the batch), per sequence the cross K/V of every layer, the self K/V read so far, and the fp32 logits row."""
+        the batch), per sequence the cross K/V of every layer, the self K/V read so far, and the fp32 logits row.  An
+        fp8 engine reads one byte per block-projection weight plus a 4-byte scale per output row, and one byte per cross
+        K/V element plus a 4-byte scale per (key, head, K|V); the logits head and the self K/V stay 16-bit."""
         e = 2
-        d, L = self.d, self.L
-        weights = L * (3 * d * d + d * d + d * d + d * d + 8 * d * d) * e + self.V * d * e
-        cross = L * 2 * self.n_audio_ctx * d * e
+        d, L, H = self.d, self.L, self.H
+        block = 3 * d * d + d * d + d * d + d * d + 8 * d * d    # qkv, out, cross q, cross out, fc1 + fc2
+        rows = 3 * d + d + d + d + 4 * d + d                      # their output rows
+        if self.fp8:
+            weights = L * (block + 4 * rows) + self.V * d * e
+            cross = L * self.n_audio_ctx * (2 * d + 4 * 2 * H)
+        else:
+            weights = L * block * e + self.V * d * e
+            cross = L * 2 * self.n_audio_ctx * d * e
         self_kv = L * 2 * t * d * e
         return weights + n * (cross + self_kv + self.V * 4)

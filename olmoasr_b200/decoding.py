@@ -11,8 +11,8 @@ SuppressTokens, ApplyTimestampRules.
 Routes: every configuration runs on the device decoder (olmoasr_b200/decode_engine.py) as replays of one CUDA graph per
 step: greedy decoding with or without timestamp rules, temperature sampling (best_of samples per clip sharing the clip's
 cross-attention K/V, ranked like upstream) and beam search.  The hook loop below remains for OASR_DECODE_ENGINE=0, models
-without `decode_engine` and best_of above the engine's batch (64 rows).  Beam search needs the device decoder: without
-it, `beam_size` raises NotImplementedError.  Sampled ids follow softmax(logits / T) like upstream's
+without `decode_engine` and best_of above the engine's batch (64 rows).  Beam search and `fp8` need the device decoder:
+without it, `beam_size` and `fp8=True` raise NotImplementedError.  Sampled ids follow softmax(logits / T) like upstream's
 `Categorical(...).sample()` but from the engine's own keyed random stream (reproducible under `torch.manual_seed`).
 
 Token ids are the contract: text<->id conversion needs the `gpt2.tiktoken` vocabulary, which is not available offline;
@@ -67,6 +67,7 @@ class DecodingOptions:
     without_timestamps: bool = False
     max_initial_timestamp: Optional[float] = 1.0
     fp16: bool = True  # decoder-step activation dtype: fp16 (upstream default) or, when False, bf16 (there are no fp32 kernels)
+    fp8: bool = False  # store the decoder's block projection weights and cross-attention K/V as e4m3 (device decoder only)
 
 
 @dataclass(frozen=True)
@@ -173,6 +174,8 @@ class DecodingTask:
                 raise ValueError(f"beam_size must be in 1 .. {BEAM_MAX}")
             if not 1 <= round(options.beam_size * (options.patience or 1.0)) <= MAX_CANDIDATES:
                 raise ValueError(f"round(beam_size * patience) must be in 1 .. {MAX_CANDIDATES}")
+        if options.fp8 and not (USE_ENGINE and hasattr(model, "decode_engine")):
+            raise NotImplementedError("fp8 decoding runs on the device decoder only (model.decode_engine)")
         if model.is_multilingual:
             raise NotImplementedError("only the English-only vocabulary of the OLMoASR checkpoints is supported")
         self.model, self.options = model, options
@@ -212,7 +215,13 @@ class DecodingTask:
     def _window_splits(self, sample_keys):
         if sample_keys is None or not (USE_ENGINE and hasattr(self.model, "decode_engine")):
             return contextlib.nullcontext()
-        return self.model.decode_engine(torch.float16 if self.options.fp16 else torch.bfloat16).splits_of(self.n_group)
+        return self._engine().splits_of(self.n_group)
+
+    def _engine(self):
+        """The device decoder these options select: activation dtype and weight / cross K/V storage.  The 16-bit engine
+        is asked for as `decode_engine(dtype)`, the signature models without fp8 decoding implement."""
+        dtype = torch.float16 if self.options.fp16 else torch.bfloat16
+        return self.model.decode_engine(dtype, fp8=True) if self.options.fp8 else self.model.decode_engine(dtype)
 
     def _run(self, mel: Tensor, tokenizer=None, sample_keys=None) -> List[DecodingResult]:
         model, opt = self.model, self.options
@@ -225,11 +234,14 @@ class DecodingTask:
         if opt.beam_size is not None:
             return self._run_beam_on_device(audio_features, tokenizer)
         if USE_ENGINE and hasattr(model, "decode_engine"):
-            eng = model.decode_engine(torch.float16 if opt.fp16 else torch.bfloat16)
+            eng = self._engine()
             if opt.temperature == 0:
                 return self._run_on_device(audio_features, tokenizer, eng)
             if self.n_group <= eng.max_batch:
                 return self._run_sampling_on_device(audio_features, tokenizer, eng, sample_keys)
+        if opt.fp8:
+            raise NotImplementedError(f"fp8 decoding runs on the device decoder only: best_of {self.n_group} needs the "
+                                      "hook loop (more rows than the device decoder's batch)")
         G = self.n_group                           # best_of samples per clip (temperature > 0), rows clip-major
         xa = audio_features.repeat_interleave(G, dim=0) if G > 1 else audio_features
         n_rows = n_audio * G
@@ -278,7 +290,7 @@ class DecodingTask:
         """Beam search (the long-form eval configuration, scripts/eval/eval.py:2077-2084) on the device decoder: one CUDA
         graph replay per step, candidates / ranking / kv reorder in kernels, up to 64 // beam_size clips per call."""
         opt = self.options
-        eng = self.model.decode_engine(torch.float16 if opt.fp16 else torch.bfloat16)
+        eng = self._engine()
         per = eng.max_batch // opt.beam_size
         ts = self.ts_rules is not None
         mi = self.ts_rules.max_initial_timestamp_index if ts else None
