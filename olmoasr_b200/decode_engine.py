@@ -124,7 +124,9 @@ class DecodeEngine:
         self.max_splits = 8       # key-range splits of the cross-attention at small batches (each split's fp32 partial is re-read by the out projection)
         self.part_self = z(1, N, d, dt=torch.float32)
         self.part_cross = z(self.max_splits, N, d, dt=torch.float32)
-        self.logits = z(N, self.V, dt=torch.float32)
+        # rows padded to a multiple of 4 floats: the selection kernels read them with 16-byte loads, and a training-layout
+        # model's vocabulary (n_vocab + 1 = 51865 with the pad row) is odd
+        self.logits = z(N, (self.V + 3) & ~3, dt=torch.float32)[:, : self.V]
         self.tokens = torch.zeros((N, self.n_ctx + 2), device=dev, dtype=torch.int32)
         self.pos = torch.zeros(1, device=dev, dtype=torch.int32)
         self.sum_logprobs = z(N, dt=torch.float32)

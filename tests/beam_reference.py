@@ -217,9 +217,9 @@ def beam_search(step_fn: Callable[[torch.Tensor, Optional[List[int]]], torch.Ten
 
 
 def beam_decode(sd, dims, xa: torch.Tensor, beam_size: int, initial_tokens: Sequence[int], sample_len: int,
-                dtype=torch.float32, **kw) -> BeamResult:
-    """beam_search over oracle/model.py's kv-cache decoder (inf_model.py), one copy of the audio features per beam as
-    upstream; the self-attention cache is rearranged with index_select."""
+                dtype=torch.float32, train_model: bool = False, **kw) -> BeamResult:
+    """beam_search over oracle/model.py's kv-cache decoder (inf_model.py, or model.py's with `train_model`), one copy of
+    the audio features per beam as upstream; the self-attention cache is rearranged with index_select."""
     from oracle import model as OM
 
     n_audio = xa.shape[0]
@@ -232,6 +232,6 @@ def beam_decode(sd, dims, xa: torch.Tensor, beam_size: int, initial_tokens: Sequ
             for key in list(cache):
                 if ".cross_attn." not in key:
                     cache[key] = cache[key].index_select(0, idx)
-        return OM.decoder_forward(sd, dims, inp, xa_rep, None, train_model=False, cache=cache)
+        return OM.decoder_forward(sd, dims, inp, xa_rep, None, train_model=train_model, cache=cache)
 
     return beam_search(step, n_audio, initial_tokens, sample_len, beam_size, n_ctx=dims.n_text_ctx, device=xa.device, **kw)

@@ -184,7 +184,7 @@ def _index_mask(logits, tokens, sb, sup, mi):
     return banned
 
 
-def _ref_greedy_ts(OM, sd, dims, xa, dtype, n_steps, suppress, mi):
+def _ref_greedy_ts(OM, sd, dims, xa, dtype, n_steps, suppress, mi, train_model=False):
     """DecodingTask._main_loop at temperature 0 with ApplyTimestampRules over oracle/model.py, stock torch on the GPU.
     Returns tokens, per-step relative margins (top-1 / top-2 after every filter, and |lse(ts) - max(text)| before the
     mass rule, over unfinished rows), sum_logprobs and no-speech probabilities."""
@@ -194,7 +194,7 @@ def _ref_greedy_ts(OM, sd, dims, xa, dtype, n_steps, suppress, mi):
     with torch.no_grad():
         for i in range(n_steps):
             inp = tokens if i == 0 else tokens[:, -1:]
-            logits = OM.decoder_forward(sd, dims, inp.cuda(), xa.to(dtype), None, train_model=False, cache=cache)
+            logits = OM.decoder_forward(sd, dims, inp.cuda(), xa.to(dtype), None, train_model=train_model, cache=cache)
             if i == 0:
                 nsp = logits[:, 0].float().softmax(-1)[:, NO_SPEECH].cpu()
             logits = logits[:, -1].float().cpu()

@@ -84,6 +84,11 @@ def main():
         eng.sample(xa, [50257, 50362], 4, 0.6, best_of=5, seed=1, suppress=(7, 9))
         eng.sample(xa[:2], [50257], 4, 1.0, best_of=3, seed=2, clip_offset=5, suppress=(7, 9), timestamps=True,
                    max_initial_timestamp_index=50)
+    # a training-layout engine (51865 logits per row, the pad row included): the only vocabulary whose last slice ends in a
+    # partial float4, so the selection kernels' tail branch runs -- beam search with timestamp rules
+    eng = m.decode_engine(torch.float16)
+    eng.beam_search(torch.randn(2, 1500, 64, device=dev).bfloat16(), [50257], 4, 5, suppress=(7, 9), timestamps=True,
+                    max_initial_timestamp_index=50)
     # word alignment: single-window and batched cost and DTW over ragged windows (edge tiles, one frame, 448 tokens)
     for dtype in (torch.float16, torch.bfloat16):
         windows = []
